@@ -2,7 +2,8 @@
 """bench.py — VideoTokenizer train-step frames/sec @ 16x64x64 (BASELINE.json's metric, configs[1]).
 
     python bench.py --gpus N --steps K --warmup W                 # our arm (one process per GPU via torchrun for N>1)
-    python bench.py --impl reference --gpus N --steps K --warmup W  # the reference itself on the host CPU (baseline/_ref), rank 0 only
+    python bench.py --impl reference --gpus N --steps K --warmup W  # the reference itself on the host CPU (oracle/_ref), rank 0 only
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR  # also write one timed-path step's results as .npy
 
 A "step" is one full training step of the MAGVIT2 VideoTokenizer (GAN / perceptual terms disabled — the
 only configuration in which the reference runs offline, SURVEY.md §8) on one synthetic batch of
@@ -37,7 +38,7 @@ def load_peaks():
         with open(p) as f:
             d = json.load(f)
         return d, 'measured (MEASURED_PEAKS.json)'
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0}, 'fallback (B200_PROFILING.md)'
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0}, 'fallback (H100 SXM data sheet, dense bf16, 700 W)'
 
 
 class ClockSampler:
@@ -92,11 +93,11 @@ class ClockSampler:
 
 # --------------------------------------------------------------------------------------------------
 # CPU leg: the reference's OWN implementation (the unmodified myscience/open-genie package vendored by
-# __graft_entry__.build() into baseline/_ref, imported through the `lightning` stand-in of oracle/_shim) on the
+# __graft_entry__.build() into oracle/_ref by oracle/vendor_reference.py, imported through the `lightning` stand-in of oracle/_shim) on the
 # host cores; if that copy is absent, the oracle port of the same algorithm (oracle/genie_oracle.py). A measured
 # baseline only — never on the product path.
 # --------------------------------------------------------------------------------------------------
-REF_DIR = os.path.join(ROOT, 'baseline', '_ref')
+REF_DIR = os.path.join(ROOT, 'oracle', '_ref')
 
 
 def usable_cores():
@@ -108,9 +109,8 @@ def usable_cores():
 
 def pick_cpu_threads():
     """Thread policy of the CPU arm, stated in the JSON line: a FIXED min(32, usable cores) threads (OG_CPU_THREADS
-    overrides). Measured on this pool's 128-thread hosts with the whole reference training step: 32 threads 1.99-2.27
-    frames/s, 64 threads 1.32 frames/s (profiles/r02bb_*), and with all 128 threads a conv3d probe is 25-50x slower
-    (oversubscription) — so `os.cpu_count()` threads would flatter the GPU/CPU ratio. Earlier rounds PICKED the count with
+    overrides). On 128-thread hosts, 64 threads ran the whole reference training step slower than 32, and all 128 threads
+    made a conv3d probe 25-50x slower (oversubscription) — so `os.cpu_count()` threads would flatter the GPU/CPU ratio. Earlier rounds PICKED the count with
     a conv3d probe; the probe put 32 and 64 within 5 % of each other and flipped between runs, so it is now reported
     only (`thread_probe_ms`, conv3d forward+backward, best of 3) and no longer decides."""
     import torch.nn.functional as F
@@ -187,7 +187,7 @@ WORKLOAD = ('BASELINE configs[1]: MAGVIT2_ENC/DEC VideoTokenizer training step (
 
 
 def cpu_sample_text(batch, threads, avail, kind):
-    what = ('unmodified reference package (baseline/_ref) through its own VideoTokenizer.training_step + AdamW'
+    what = ('unmodified reference package (oracle/_ref) through its own VideoTokenizer.training_step + AdamW'
             if kind == 'reference' else 'oracle/genie_oracle.py port of the reference (pinned to reference outputs)')
     return (f'{batch} clip(s) x {FRAMES} frames per step, fp32 torch CPU, {threads} threads (fixed policy min(32, cores): '
             f'the fastest count for this step on the {avail}-thread hosts, 64 threads measured 1.5x slower); {what}')
@@ -253,6 +253,55 @@ def _hbm_bytes(name, a):
     return None
 
 
+DUMP_PARAM_SAMPLES = 1 << 22    # 16 MB of float32
+
+
+def restore_initial_state(model, opt, init_state):
+    """Put the model and the optimizer back to the seeded state they had before the first step, in place (the captured
+    graph keeps its pointers): parameters and buffers, the bf16 GEMM operand copies of the conv weights, zero AdamW
+    moments and a zero step counter."""
+    with torch.no_grad():
+        for t, c in init_state:
+            t.copy_(c)
+        for m in model.modules():
+            if hasattr(m, 'bf16_target'):
+                m.bf16_target()                 # re-packs the bf16 operand from the restored weight
+        for st in opt.state.values():
+            for k in ('exp_avg', 'exp_avg_sq'):
+                if k in st:
+                    st[k].zero_()
+        if opt._step_dev is not None:
+            opt._step_dev.zero_()
+        opt._step = 0
+
+
+def snapshot_outputs(model, loss):
+    """What the timed step hands back: its loss, and the parameters it updated — all of them when they fit the budget,
+    otherwise a fixed seeded sample of the flattened parameter vector (same indices in every run with the same model)."""
+    params = [p.detach() for p in model.parameters()]
+    total = sum(p.numel() for p in params)
+    if total <= DUMP_PARAM_SAMPLES:
+        flat = torch.cat([p.float().flatten() for p in params])
+    else:       # gather the sample parameter by parameter (no flattened copy of the whole model)
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randint(0, total, (DUMP_PARAM_SAMPLES,), generator=g).sort().values
+        flat = torch.empty(DUMP_PARAM_SAMPLES, dtype=torch.float32, device=params[0].device)
+        off = 0
+        for p in params:
+            lo, hi = (int(torch.searchsorted(idx, v)) for v in (off, off + p.numel()))
+            if hi > lo:
+                flat[lo:hi] = p.reshape(-1)[(idx[lo:hi] - off).to(p.device)].float()
+            off += p.numel()
+    return {'loss': loss.detach().double().reshape(1).cpu().numpy(), 'params_sample': flat.cpu().numpy()}
+
+
+def write_outputs(out_dir, arrays):
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f'{name}.npy'), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
@@ -265,6 +314,10 @@ def main():
                     help='--impl reference: drop to 1 clip per step if (steps+warmup) x first-step time exceeds this')
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-graph', action='store_true', help='launch every kernel from Python instead of replaying the captured step')
+    ap.add_argument('--dump-outputs', metavar='DIR',
+                    help='after the timed steps, restore the seeded initial model and optimizer state, run the timed '
+                         'step once more on the benchmark batch and write what it computed (its loss and a fixed, seeded '
+                         'sample of the updated parameters) as DIR/<name>.npy, so that two builds can be compared')
     args = ap.parse_args()
     rank, world, local = env_int('RANK', 0), env_int('WORLD_SIZE', 1), env_int('LOCAL_RANK', 0)
 
@@ -277,10 +330,9 @@ def main():
     dev = torch.device('cuda', local)
     if world > 1:
         os.environ.setdefault('MASTER_ADDR', '127.0.0.1')
-        # Every CTA NCCL occupies takes a whole SM away from the persistent one-CTA-per-SM GEMM kernels (227 KB of shared
-        # memory each: nothing co-resides); capping NCCL's CTAs was measured and is WORSE (N = 2, profiles/r02j_*: 8 CTAs
-        # 66.3 ms = default, 4 CTAs 69.7, 2 CTAs 81.3 — the all-reduce then no longer hides behind backward). The GEMM
-        # kernels instead draw their tiles dynamically, so CTAs that cannot be resident cost nothing (conv3d_igemm.cu).
+        # Every CTA NCCL occupies takes a whole SM away from the persistent one-CTA-per-SM GEMM kernels (most of the shared
+        # memory each: nothing co-resides). OG_NCCL_MAX_CTAS caps NCCL's CTAs for experiments; capping can also keep the
+        # all-reduce from hiding behind backward.
         if os.environ.get('OG_NCCL_MAX_CTAS'):
             os.environ.setdefault('NCCL_MAX_CTAS', os.environ['OG_NCCL_MAX_CTAS'])
         dist.init_process_group('nccl', device_id=dev)
@@ -294,6 +346,8 @@ def main():
                               perc_loss_weight=0).to(dev)
     n_params = sum(p.numel() for p in model.parameters())
     opt = model.configure_optimizers()                      # FusedAdamW, AdamW defaults
+    init_state = [(t, t.detach().clone()) for t in list(model.parameters()) + list(model.buffers())] \
+        if args.dump_outputs else None
     og.enable_zero_arena(True)   # every step below ends with zero_grad(set_to_none=True): the arena contract holds
     # N > 1: ONE gradient exchange per step, all-reduced in place on the step's zero arena (no bucket copies)
     bucket_mb = int(os.environ.get('OG_BUCKET_MB', '64'))
@@ -411,6 +465,17 @@ def main():
     timing, _lib.TIMING = _lib.TIMING, None
     if use_graph:
         launches = int(round(launches_per_step * args.steps))   # kernels executed by the replays of the timed region
+    # --dump-outputs: one more step of the timed path (the captured step) from the seeded initial state. The gradient
+    # reductions of a step sum in a fixed order, so this step is the same in every run. The timed steps themselves are
+    # not: after tens of steps their parameters still differ between runs (a last-bit difference that is not yet traced
+    # to its reduction, amplified by training), so they cannot serve as the comparison.
+    dump = None
+    if args.dump_outputs:
+        model.zero_grad(set_to_none=True)
+        restore_initial_state(model, opt, init_state)
+        loss = train_step(dev_video)
+        barrier()
+        dump = snapshot_outputs(model, loss) if rank == 0 else None
 
     if rank == 0:
         peaks, peak_src = load_peaks()
@@ -479,14 +544,7 @@ def main():
         dom = max(kinds, key=lambda k: kern[k]['ms_per_step']) if kinds else None
         roofline = None
         if dom:
-            traffic, traffic_note = None, None
-            try:    # DRAM bytes of one launch of the dominant kernel, from the committed ncu --set full capture
-                tj = json.load(open(os.path.join(ROOT, 'profiles', 'r02_ncu_traffic.json')))[dom]
-                traffic = tj['traffic_bytes']
-                traffic_note = (f"ncu --set full, one launch of {tj['shape']}: dram read {tj['dram_read_bytes']} + "
-                                f"write {tj['dram_write_bytes']} B; algorithmic {tj['algorithmic_bytes']} B")
-            except Exception:
-                pass
+            traffic, traffic_note = None, 'not measured'
             conv_flop = sum(d['flop'] for d in kinds.values()) / prof_steps
             roofline = {'kernel': dom, 'bound': 'tensor', 'achieved': kern[dom]['tflops'], 'peak': peak_tf,
                         'unit': 'TFLOP/s', 'frac': kern[dom]['tflops'] / peak_tf, 'traffic': traffic,
@@ -509,7 +567,7 @@ def main():
                        'grad_exchange': None if reducer is None else
                        f'NCCL all-reduce (AVG) in place on the zero arena, {reducer.bucket >> 20} MB ranges overlapped with '
                        f'backward, {reducer.grad_bytes()} B per step, NCCL_MAX_CTAS={os.environ.get("NCCL_MAX_CTAS")}',
-                       'l2': 'no flush: every step streams several GB of activations (>> 126 MB L2)'},
+                       'l2': 'no flush: every step streams several GB of activations (>> 50 MB L2)'},
             'e2e': {'value': fps_e2e, 'unit': 'frames/s', 'h2d_bytes_per_step': h2d_bytes * world,
                     'd2h_bytes_per_step': 4 * world,
                     'legs_ms': [ms_e2e_a / args.steps, ms_e2e_b / args.steps],
@@ -528,10 +586,12 @@ def main():
                 'value': args.cpu_batch * FRAMES / dt, 'unit': 'frames/s', 'cores': threads, 'cores_usable': avail,
                 'kind': kind, 'thread_probe_ms': probe,
                 'sample': f'one training step ({dt:.1f} s): ' + cpu_sample_text(args.cpu_batch, threads, avail, kind)}
+        if dump is not None:
+            write_outputs(args.dump_outputs, dump)
         print(json.dumps(line), flush=True)
     if world > 1:
         # Tearing the process group down while a CUDA graph that captured NCCL collectives is still alive hung in
-        # ProcessGroupNCCL's destructor (2xB200, torch 2.11 / NCCL 2.28): finish all work, agree that everybody is done,
+        # ProcessGroupNCCL's destructor (torch 2.11 / NCCL 2.28): finish all work, agree that everybody is done,
         # then leave without running the destructors.
         barrier()
         sys.stdout.flush()

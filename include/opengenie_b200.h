@@ -1,4 +1,4 @@
-/* opengenie_b200.h — C ABI of libopengenie_b200.so (sm_100a only).
+/* opengenie_b200.h — C ABI of libopengenie_b200.so (sm_90a only).
  *
  * The drop-in boundary for open-genie's data-parallel hot path. The reference has no FFI of its own:
  * every entry point below replaces one ATen call site (or a fused run of them) in the reference's
@@ -12,7 +12,7 @@
  *     is exactly the memory order of a torch (Cout,Cin,kt,kh,kw) tensor in channels_last_3d format.
  *   - every function returns OG_OK (0) or a negative og_status; og_last_error() gives the message.
  *     Nothing throws, nothing allocates device memory, nothing synchronises the stream.
- *   - there is NO CPU or library fallback: on a non-sm_100 device the launch fails with OG_ERR_CUDA.
+ *   - there is NO CPU or library fallback: on a non-sm_90 device the launch fails with OG_ERR_CUDA.
  */
 #ifndef OPENGENIE_B200_H_
 #define OPENGENIE_B200_H_
@@ -42,7 +42,7 @@ int og_compiled_sm(void);
 uint64_t og_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------
- * conv3d — implicit GEMM on tcgen05 tensor cores (TMA-staged NDHWC tiles, fp32 accumulate in TMEM)
+ * conv3d — implicit GEMM on wgmma tensor cores (TMA-staged NDHWC tiles, fp32 accumulate in registers)
  * ---------------------------------------------------------------------------------------------- */
 
 /* Forward 3-D convolution, stride 1, "same" output size, zero padding.
@@ -63,7 +63,7 @@ uint64_t og_launch_count(void);
  * SpaceTimeAttention, attention.py:472).
  * Reads outside [0,T)x[0,H)x[0,W) are zero (pad_mode='constant').
  * workspace (optional, may be NULL): N*T*H*W*cout fp32 of scratch enables split-K for problems whose tiles
- * cannot fill the 148 SMs (small T*H*W, deep K); without it the same result is computed unsplit. With room for one
+ * cannot fill the 132 SMs (small T*H*W, deep K); without it the same result is computed unsplit. With room for one
  * such slab per split (20 MB always suffices) every split stores its partial tile with plain stores and the finish pass
  * adds the slabs (and emits gn_sums); a smaller workspace is zeroed and reduced into with red.global.add.
  * gn_sums (optional): fp64 [N][2] += (sum, sum of squares) of the bf16 output per sample — the og_gn_stats
@@ -101,17 +101,19 @@ int og_conv3d_dgrad(const void* dy, int cout, int w_rows, const void* w, int ldw
 /* Weight gradient (autograd's conv3d backward-weight). ACCUMULATES into dw (caller zeroes it):
  *   dw[co][tap][ci] += sum_{n,t,h,w} dy[n,t,h,w,co] * x[n, t+it-pt, h+ih-ph, w+iw-pw, ci]
  * dy: bf16 [N,T,H,W,cout]; x: bf16 [N,T,H,W,cin] (cin % 64 == 0); dw: fp32, row stride ld_dw elements,
- * tap-major / channel-minor inside a row (the channels_last_3d order of the torch weight). */
+ * tap-major / channel-minor inside a row (the channels_last_3d order of the torch weight).
+ * workspace (may be NULL): fp32 scratch for split-K — one [cout][taps*cin] (+ bias) partial per split, added in split
+ * order, so the result is the same every run; the split count shrinks to what fits (none without a workspace). */
 int og_conv3d_wgrad(const void* dy, int cout, const void* x, int cin, float* dw, int64_t ld_dw, int kt, int kh,
-                    int kw, int pt, int ph, int pw, int N, int T, int H, int W, og_stream_t stream);
+                    int kw, int pt, int ph, int pw, int N, int T, int H, int W, void* workspace,
+                    size_t workspace_bytes, og_stream_t stream);
 /* og_conv3d_wgrad + the bias gradient of the same nn.Conv3d in one launch: dbias[c] += sum over voxels of dy[v][c] for
  * c < n_bias (1 <= n_bias <= cout; caller zeroes dbias). The sums come out of the same tensor-core pass (an extra N = 16
- * product against a tile of ones in the last filter-tap group); when the tiling leaves no spare accumulator columns the
- * call runs og_colsum afterwards — same result either way. Replaces the bias half of autograd's conv3d backward
+ * product against a tile of ones in the last filter-tap group). Replaces the bias half of autograd's conv3d backward
  * (genie/module/video.py:178-192, 609-629). */
 int og_conv3d_wgrad_bias(const void* dy, int cout, const void* x, int cin, float* dw, int64_t ld_dw, int kt, int kh,
                          int kw, int pt, int ph, int pw, int N, int T, int H, int W, float* dbias, int n_bias,
-                         og_stream_t stream);
+                         void* workspace, size_t workspace_bytes, og_stream_t stream);
 
 /* Strided CausalConv3d — SpaceTimeDownsample (genie/module/video.py:457-483) — as the SAME implicit GEMM, no im2col:
  * geometry of video.py:154-164 (time padded at the FRONT only by pt = (kt-1) + (1-st); space symmetrically by
@@ -131,7 +133,7 @@ int og_conv3d_strided_dgrad(const void* dy, int cout, int w_rows, const void* w,
                             og_stream_t stream);
 int og_conv3d_strided_wgrad(const void* dy, int cout, const void* x, int cin, float* dw, int64_t ld_dw, int kt, int kh,
                             int kw, int st, int sh, int sw, int pt, int ph, int pw, int N, int T, int H, int W,
-                            og_stream_t stream);
+                            void* workspace, size_t workspace_bytes, og_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * GroupNorm / AdaptiveGroupNorm (+SiLU), NDHWC bf16, HBM-bound passes
@@ -157,9 +159,11 @@ int og_gn_finalize(const double* sums, int N, int C, int G, int64_t V, float eps
 int og_affine_act_fwd(const void* x, const float* A, const float* B, void* y, int N, int64_t V, int C, int act,
                       og_stream_t stream);
 
-/* S[n][c] = (sum_v dpre, sum_v dpre*x), dpre = dy * act'(x*A+B). Caller zeroes S (N*C*2 floats). */
+/* S[n][c] = (sum_v dpre, sum_v dpre*x), dpre = dy * act'(x*A+B). Caller zeroes S (N*C*2 floats).
+ * workspace (may be NULL): fp32 scratch for per-block partial sums, added in block order (reproducible); the number of
+ * blocks per sample shrinks to what fits (one per sample without a workspace). */
 int og_affine_act_bwd_reduce(const void* dy, const void* x, const float* A, const float* B, int act, float* S,
-                             int N, int64_t V, int C, og_stream_t stream);
+                             int N, int64_t V, int C, void* workspace, size_t workspace_bytes, og_stream_t stream);
 
 /* Turns S into the per-(n,c) coefficients of dx = A*dpre + Q*x + R and the parameter gradients:
  * dgamma/dbeta [C] are ACCUMULATED (+=); dcond_scale/dcond_shift [N,C] are written. Any of the four may
@@ -188,7 +192,8 @@ int og_adagn_cond_bwd(const float* dscale, const float* dshift, const float* cba
  * og_gn_act_fwd  = og_gn_finalize + og_affine_act_fwd  (A, B, mean_rstd are still written for backward);
  * og_gn_act_bwd  = og_gn_bwd_finalize + og_affine_act_bwd_apply, S/mean_rstd NULL => pure activation backward.
  * dx_colsum (optional, float[C], ACCUMULATED) receives sum over rows of dx — the bias gradient of the
- * convolution that produced x (nn.Conv3d bias of ResidualBlock conv #1, genie/module/video.py:609-615).
+ * convolution that produced x (nn.Conv3d bias of ResidualBlock conv #1, genie/module/video.py:609-615); its per-block
+ * partials go to the fp32 workspace (at least N*C floats when N > 1) and are added in block order (reproducible).
  * Both need (C/G) % 8 == 0. */
 int og_gn_act_fwd(const void* x, const double* sums, const float* gamma, const float* beta, const float* cond_scale,
                   const float* cond_shift, float eps, int G, int act, void* y, float* A, float* B, float* mean_rstd,
@@ -196,7 +201,8 @@ int og_gn_act_fwd(const void* x, const double* sums, const float* gamma, const f
 int og_gn_act_bwd(const void* dy, const void* x, const float* A, const float* B, const float* S,
                   const float* mean_rstd, const float* gamma, const float* beta, const float* cond_scale, int G, int act,
                   const void* add, void* dx, float* dgamma, float* dbeta, float* dcond_scale, float* dcond_shift,
-                  float* dx_colsum, int N, int64_t V, int C, og_stream_t stream);
+                  float* dx_colsum, int N, int64_t V, int C, void* workspace, size_t workspace_bytes,
+                  og_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * layout / data movement
@@ -312,7 +318,7 @@ int og_rope_ln_bwd(const void* x, const float* freq, const float* gamma, float e
                    int64_t pos_div, int pos_mod, const float* cos_sin, og_stream_t stream);
 
 /* Spatial attention: F.scaled_dot_product_attention(q,k,v, scale) non-causal (attention.py:229-234) on
- * tcgen05 tensor cores. q,k,v,out: [nseq][S][C], C = n_head*64. lse: fp32 [nseq][n_head][S] (saved for backward).
+ * wgmma tensor cores. q,k,v,out: [nseq][S][C], C = n_head*64. lse: fp32 [nseq][n_head][S] (saved for backward).
  * residual / out_res (optional, bf16 like out): out_res = out + residual, i.e. `attn(x) + skip(x)`
  * (attention.py:470-471), added in fp32; `out` itself is still written (the backward pass needs it). */
 int og_flash_attn_fwd(const void* q, const void* k, const void* v, void* out, const void* residual, void* out_res,

@@ -1,4 +1,4 @@
-"""open_genie_b200 — B200-native (sm_100a) implementation of open-genie's data-parallel hot path behind the
+"""open_genie_b200 — H100-native (sm_90a) implementation of open-genie's data-parallel hot path behind the
 reference's own Python surface (myscience/open-genie: genie/__init__.py).
 
 Importing this package never touches the GPU; the CUDA library (csrc/libopengenie_b200.so) is loaded on

@@ -1,5 +1,5 @@
 """LatentAction — mirrors genie/action.py:31-176 (same constructor, encode/decode/forward/sample, return tuples,
-state_dict keys) on the B200 kernels.
+state_dict keys) on the CUDA kernels.
 
 Pinned to the HEAD-valid behaviour (SURVEY.md §8): the reference constructor forgets `input_dim` when it builds
 the quantizer (action.py:93-101), which makes LookupFreeQuantization project from 2^d inputs and crash in

@@ -719,9 +719,8 @@ __global__ void __launch_bounds__(128)
   if (kv_bcast) flush();
 }
 
-// mma.sync m16n8k16 path (temporal_attn_mma.cu) for d_head = 64, T <= 16 — the default since round 2 (it passed the
-// parity suite on a B200 and took the LatentAction step from 246.9 to 220.1 ms, the Dynamics step from 20.5 to 16.5 ms:
-// profiles/r02f_configs*.jsonl); OG_TEMPORAL_MMA=0 selects the per-lane kernels below, which also cover T in (16, 32].
+// mma.sync m16n8k16 path (temporal_attn_mma.cu) for d_head = 64, T <= 16 — the default; OG_TEMPORAL_MMA=0 selects the
+// per-lane kernels below, which also cover T in (16, 32].
 int launch_temporal_fwd_mma(const void* q, const void* k, const void* v, const void* residual, void* out, int B, int T,
                             long long P, int C, int n_head, float scale, int kv_bcast, cudaStream_t stream);
 int launch_temporal_bwd_mma(const void* q, const void* k, const void* v, const void* dout, void* dq, void* dk, void* dv,

@@ -1,5 +1,5 @@
 // conv3d_igemm.cu — stride-1 3-D convolution forward and data-gradient as an implicit GEMM on the
-// 5th-gen tensor cores (tcgen05.mma, accumulators in TMEM), operands staged by TMA.
+// Hopper tensor cores (wgmma.mma_async, fp32 accumulators in registers), operands staged by TMA.
 //
 //   D[m][n] = sum_k A[m][k] * B[n][k]      m = output voxel (n,t,h,w), n = output channel,
 //                                           k = (segment, tap, input channel)
@@ -15,10 +15,12 @@
 // MN-major B operand (k = cout rows of 64, n = cin contiguous) with mirrored taps, so no transposed
 // weight copy ever exists.
 //
-// Warp roles (192 threads, 1 CTA / SM, persistent over tiles):
+// Warp roles (256 threads, 1 CTA / SM, persistent over tiles):
 //   warp 0    TMA producer (one elected lane)
-//   warp 1    TMEM allocator + MMA issuer (one elected lane)
-//   warps 2-5 epilogue: TMEM -> registers -> (+bias) -> global, double-buffered against the next tile's MMAs
+//   warps 1-3 idle (they only complete the first warpgroup: wgmma needs an aligned one)
+//   warps 4-7 one warpgroup: wgmma main loop (128 x BN accumulator = two m64 halves in registers, BN <= 128),
+//             then the epilogue: registers -> fp32 tile in shared memory -> one row per thread -> (+bias) -> global.
+//             The producer keeps filling the stage ring with the next tile's operands meanwhile.
 #include <stdlib.h>
 
 #include <utility>
@@ -51,7 +53,7 @@ struct IgemmParams {
   int OT, OH, OW;  // extents of the OUTPUT tensor; M-tile voxel (t,h,w) is stored at (t*om[0]+oo[0], h*om[1]+oo[1], ...)
   int om[3], oo[3];
   int b_mn_major;  // 0: B tile is [n rows][64 k] (K-major); 1: B tile is [k rows][n] in 64-wide panels (MN-major)
-  int block_n;     // UMMA N (16..256)
+  int block_n;     // wgmma N (16..128)
   int num_n_tiles, num_m_tiles;
   int bw_log2, bh_log2, bt_log2, bn_log2;  // M tile = 2^bw x 2^bh x 2^bt x 2^bn voxels (product 128)
   int tiles_w, tiles_h, tiles_t;           // M tiles along each axis (ceil)
@@ -65,7 +67,6 @@ struct IgemmParams {
   const float* bias1;
   int num_stages;
   int num_kb;  // k-blocks per tile
-  int m_sub;   // M sub-tiles (of 128 rows) per CTA tile sharing one B stage: 1 or 2
   int fast_store;  // bf16 output, n_out % 64 == 0, block_n % 64 == 0: coalesced staged stores
   const __nv_bfloat16* residual;  // optional bf16 [voxels][n_out] added to the output (out = conv + bias + residual)
   // fused epilogue reductions (fast_store path, one sample per CTA tile):
@@ -75,7 +76,6 @@ struct IgemmParams {
   const float* red_B;
   float* red_S;                // ... S[n][c] += (sum dpre, sum dpre*x), dpre = d * act'(x*A+B)   (og_affine_act_bwd_reduce)
   int red_act;
-  int swap;        // operand swap (see below): D^T[cout][256 voxels] = W . X^T, used when Cout tiles are 128 wide
   unsigned int* sched;  // dynamic tile scheduler state {magic, next item, CTAs done} in the caller's workspace, or NULL
   int splits;      // split-K factor (1 = none): each work item covers a k-block range and reduces into `ws`
   float* ws;       // fp32 [voxels][n_out] partial-sum workspace (zero on entry) when splits > 1
@@ -86,15 +86,31 @@ struct IgemmParams {
                            // (bias, cast, store, GroupNorm sums) and re-zeroes its part of `ws` — no memset, no finish launch
 };
 
+
 static constexpr int kBlockM = 128;
 static constexpr int kBlockK = 64;                       // 64 bf16 = one 128-byte swizzle row
 static constexpr int kABytes = kBlockM * kBlockK * 2;    // 16 KiB
-static constexpr int kTmemCols = 512;
-static constexpr int kAccStride = 256;                   // columns between the two accumulator buffers
 static constexpr int kMaxStages = 8;
-static constexpr int kThreads = 192;
+static constexpr int kThreads = 256;
 static constexpr int kSchedDepth = 4;
 static constexpr unsigned int kSchedMagic = 0x0695CED0u;   // written by og_workspace_init
+// barriers (256) + bias (1024) + 4 warps x 4 KiB store staging + fused reductions (4352); the fp32 accumulator tile follows
+static constexpr int kTailBytes = 256 + 1024 + 4 * 4096 + 4352;
+__host__ __device__ constexpr int acc_ld(int bn) { return bn + 4; }   // fp32 row stride: conflict-free float4 row reads
+
+template <int NV>
+__device__ __forceinline__ void ld_acc_row(const float* src, uint32_t (&v)[32]) {
+#pragma unroll
+  for (int i = 0; i < NV / 4; ++i) {
+    const float4 f = reinterpret_cast<const float4*>(src)[i];
+    v[4 * i] = __float_as_uint(f.x);
+    v[4 * i + 1] = __float_as_uint(f.y);
+    v[4 * i + 2] = __float_as_uint(f.z);
+    v[4 * i + 3] = __float_as_uint(f.w);
+  }
+#pragma unroll
+  for (int i = NV; i < 32; ++i) v[i] = 0u;
+}
 
 struct TileCoord {
   int n0, t0, h0, w0;
@@ -116,26 +132,24 @@ __device__ __forceinline__ TileCoord decode_m_tile(const IgemmParams& p, int m_t
   return c;
 }
 
+template <int BN, int BMN>
 __global__ void __launch_bounds__(kThreads, 1)
     og_conv_igemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
                          const __grid_constant__ CUtensorMap mapB, const IgemmParams p) {
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment: required by the 128-byte swizzle pattern shared by TMA and the UMMA descriptors
+  // 1024-byte alignment: required by the 128-byte swizzle pattern shared by TMA and the wgmma descriptors
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int b_bytes = p.block_n * kBlockK * 2;
-  const int a_bytes = p.m_sub * kABytes;
+  const int a_bytes = kABytes;
   const int stage_bytes = a_bytes + b_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.num_stages * stage_bytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + kMaxStages;
-  uint64_t* tmem_full = bars + 2 * kMaxStages;
-  uint64_t* tmem_empty = bars + 2 * kMaxStages + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 4);
-  // Dynamic tile scheduler (round 2). With the static `item = blockIdx.x + i * gridDim.x` assignment a CTA that cannot be
+  // Dynamic tile scheduler. With the static `item = blockIdx.x + i * gridDim.x` assignment a CTA that cannot be
   // resident (another kernel — the NCCL all-reduce of the data-parallel step — holds its SM; this kernel's 227 KB of
   // shared memory exclude co-residency) starts only when a sibling CTA finishes and then still owns its full share of
   // tiles: the launch takes ~2x as long. Here the producer warp draws work items from a global counter and hands them to
-  // the MMA / epilogue warps through a 4-deep shared-memory ring, so late CTAs simply find no work left.
+  // the MMA / epilogue warpgroup through a 4-deep shared-memory ring, so late CTAs simply find no work left.
   uint64_t* sched_full = bars + 2 * kMaxStages + 5;    // [4]
   uint64_t* sched_empty = bars + 2 * kMaxStages + 9;   // [4]
   int* sched_item = reinterpret_cast<int*>(bars + 2 * kMaxStages + 13);  // [4]
@@ -146,11 +160,11 @@ __global__ void __launch_bounds__(kThreads, 1)
   float* red_s = coef_s + 512;                                            // [256][2] column sums of the current tile
   double* stat_s = reinterpret_cast<double*>(red_s + 512);                // [2]
   int* flag_s = reinterpret_cast<int*>(stat_s + 2);                       // [1] "this CTA finishes the tile" (fused split-K)
+  float* acc_s = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + kTailBytes);  // [128][acc_ld(BN)] fp32
 
   const int warp = warp_idx_uniform();
   const int lane = threadIdx.x & 31;
-  const int num_m_super = (p.num_m_tiles + p.m_sub - 1) / p.m_sub;
-  const int total_tiles = num_m_super * p.num_n_tiles * p.splits;  // work items
+  const int total_tiles = p.num_m_tiles * p.num_n_tiles * p.splits;  // work items
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&mapA0);
@@ -158,23 +172,15 @@ __global__ void __launch_bounds__(kThreads, 1)
     tma_prefetch_desc(&mapB);
     for (int s = 0; s < p.num_stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 4);
+      mbar_init(&empty[s], 4);   // one arrival per consumer warp
     }
     for (int a = 0; a < kSchedDepth; ++a) {
       mbar_init(&sched_full[a], 1);
-      mbar_init(&sched_empty[a], 5);   // MMA warp + 4 epilogue warps
+      mbar_init(&sched_empty[a], 4);   // the 4 consumer warps
     }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ===================================== TMA producer =====================================
@@ -207,8 +213,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         const int tile = item / p.splits, split = item - tile * p.splits;
         const int m_super = tile / p.num_n_tiles;
         const int n_tile = tile - m_super * p.num_n_tiles;
-        const TileCoord tc = decode_m_tile(p, m_super * p.m_sub);
-        const TileCoord tc1 = decode_m_tile(p, m_super * p.m_sub + 1);  // second sub-tile (m_sub == 2)
+        const TileCoord tc = decode_m_tile(p, m_super);
         const int kb_begin = (int)(((long long)p.num_kb * split) / p.splits);
         const int kb_end = (int)(((long long)p.num_kb * (split + 1)) / p.splits);
         // position (segment, tap = (jt, jh, jw), channel block) of kb_begin: divisions once per work item,
@@ -224,7 +229,6 @@ __global__ void __launch_bounds__(kThreads, 1)
         int jh = (tapc / sg.n[2]) % sg.n[1];
         int jw = tapc % sg.n[2];
         const int aw0 = tc.w0 * p.sx[2], ah0 = tc.h0 * p.sx[1], at0 = tc.t0 * p.sx[0];
-        const int bw0 = tc1.w0 * p.sx[2], bh0 = tc1.h0 * p.sx[1], bt0 = tc1.t0 * p.sx[0];
         for (int kb = kb_begin; kb < kb_end; ++kb) {
           const CUtensorMap* mapA = (sidx == 0) ? &mapA0 : &mapA1;
           const int dt = sg.sh0[0] + jt * sg.shstep[0], dh = sg.sh0[1] + jh * sg.shstep[1],
@@ -235,9 +239,7 @@ __global__ void __launch_bounds__(kThreads, 1)
           if (elect_one()) {
             mbar_expect_tx(&full[stage], (uint32_t)stage_bytes);
             tma_load_5d(sa, mapA, &full[stage], cb * kBlockK, aw0 + dw, ah0 + dh, at0 + dt, tc.n0);
-            if (p.m_sub == 2)
-              tma_load_5d(sa + kABytes, mapA, &full[stage], cb * kBlockK, bw0 + dw, bh0 + dh, bt0 + dt, tc1.n0);
-            if (!p.b_mn_major) {
+            if (!BMN) {
               tma_load_2d(sb, &mapB, &full[stage], kb * kBlockK, n_tile * p.block_n);
             } else {
               // w[co][tap][ci] as (ci, tap, co): one (64 ci, 1 tap, 64 co) box per 64-wide N panel
@@ -281,106 +283,23 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ===================================== MMA issuer =====================================
-    {
-      const uint32_t idesc = umma_idesc_bf16(kBlockM, (uint32_t)p.block_n, 0u, (uint32_t)p.b_mn_major);
-      const uint32_t idesc_swap = umma_idesc_bf16(kBlockM, 256u, (uint32_t)p.b_mn_major, 0u);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      int sslot = 0;
-      uint32_t sphase = 0;
-      for (int iter = 0;; ++iter) {
-        int item;
-        if (dyn) {
-          mbar_wait(&sched_full[sslot], sphase);
-          item = sched_item[sslot];
-          __syncwarp();
-          if (elect_one()) mbar_arrive(&sched_empty[sslot]);
-          if (++sslot == kSchedDepth) {
-            sslot = 0;
-            sphase ^= 1;
-          }
-        } else {
-          item = blockIdx.x + iter * gridDim.x;
-        }
-        if (item >= total_tiles) break;
-        const int split = item % p.splits;
-        const int nkb = (int)(((long long)p.num_kb * (split + 1)) / p.splits) -
-                        (int)(((long long)p.num_kb * split) / p.splits);
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * kAccStride;
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
-          const uint32_t b_addr = a_addr + a_bytes;
-          if (p.swap) {
-            // Swapped operands: A = the 128 x 64 weight tile (M = output channels), B = the TWO voxel sub-tiles as one
-            // 256-row K-major operand (they sit back to back in the stage). One 128x256x16 MMA replaces two
-            // 128x128x16 ones: the same bytes per stage, but 96 instead of 128 B/clk of shared-memory operand reads,
-            // which is what capped the Cout = 128 layers at ~78 % of the Cout = 256 rate.
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < kBlockK / 16; ++k) {
-                const uint64_t wdesc = p.b_mn_major ? umma_smem_desc_sw128(b_addr + k * 2048, 64 * 128, 1024)
-                                                    : umma_smem_desc_sw128(b_addr + k * 32, 16, 1024);
-                const uint64_t xdesc = umma_smem_desc_sw128(a_addr + k * 32, 16, 1024);
-                umma_bf16_ss(d_tmem, wdesc, xdesc, idesc_swap, (kb | k) != 0 ? 1u : 0u);
-              }
-              umma_commit(&empty[stage]);
-            }
-            __syncwarp();
-          } else if (elect_one()) {
-            for (int ms = 0; ms < p.m_sub; ++ms) {
-#pragma unroll
-              for (int k = 0; k < kBlockK / 16; ++k) {
-                // A: K-major, 128-byte rows, 8-row groups 1024 B apart; advance 16 elements = 32 B inside the row
-                const uint64_t adesc = umma_smem_desc_sw128(a_addr + ms * kABytes + k * 32, 16, 1024);
-                uint64_t bdesc;
-                if (!p.b_mn_major) {
-                  bdesc = umma_smem_desc_sw128(b_addr + k * 32, 16, 1024);
-                } else {
-                  // B: MN-major panels [block_n/64][64 k-rows][128 B]; 16 k-rows = 2048 B; panel stride 8192 B
-                  bdesc = umma_smem_desc_sw128(b_addr + k * 2048, 64 * 128, 1024);
-                }
-                umma_bf16_ss(d_tmem + ms * p.block_n, adesc, bdesc, idesc, (kb | k) != 0 ? 1u : 0u);
-              }
-            }
-            umma_commit(&empty[stage]);  // frees the smem slot once these MMAs have read it
-          }
-          if (!p.swap) __syncwarp();
-          if (++stage == p.num_stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (elect_one()) umma_commit(&tmem_full[acc]);  // accumulator complete -> epilogue
-        __syncwarp();
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================================== epilogue =====================================
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
+  } else if (warp >= 4) {
+    // ============================ wgmma main loop + epilogue (one warpgroup) ============================
+    const int q = warp & 3;  // warp of the warpgroup: wgmma rows 16q..16q+15 of each m64 half; epilogue rows 32q..32q+31
     const int row = q * 32 + lane;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    const int et = threadIdx.x - 128;
+    int stage = 0;
+    uint32_t phase = 0;
     float fl_s = 0.f, fl_ss = 0.f;
-    for (int j = threadIdx.x - 64; j < 512; j += 128) red_s[j] = 0.f;
-    if (threadIdx.x == 64) stat_s[0] = stat_s[1] = 0.0;
+    for (int j = et; j < 512; j += 128) red_s[j] = 0.f;
+    if (et == 0) stat_s[0] = stat_s[1] = 0.0;
     asm volatile("bar.sync 1, 128;" ::: "memory");
     int sslot = 0;
     uint32_t sphase = 0;
     for (int iter = 0;; ++iter) {
       int item;
       if (dyn) {
-        mbar_wait_relaxed(&sched_full[sslot], sphase);
+        mbar_wait(&sched_full[sslot], sphase);
         item = sched_item[sslot];
         __syncwarp();
         if (lane == 0) mbar_arrive(&sched_empty[sslot]);
@@ -393,59 +312,63 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
       if (item >= total_tiles) break;
       const int tile = item / p.splits;
+      const int split = item - tile * p.splits;
       const int m_super = tile / p.num_n_tiles;
       const int n_tile = tile - m_super * p.num_n_tiles;
-      mbar_wait_relaxed(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      if (p.swap) {
-        // accumulator is D^T: TMEM lane = output channel (this thread owns channel `co`), column = voxel of the
-        // 256-voxel super tile. 32-voxel chunks are transposed through a [32 voxels][128 channels] bf16 staging tile
-        // shared by the four epilogue warps (double-buffered, one named barrier per chunk), then stored as full
-        // 256-byte voxel rows. Host guarantees: whole boxes, n_out % 128 == 0, no residual / split-K.
-        const TileCoord tcs0 = decode_m_tile(p, m_super * 2), tcs1 = decode_m_tile(p, m_super * 2 + 1);
-        const int co = n_tile * 128 + row;
-        float bsum = 0.f;
-        if (p.bias0) bsum += __ldg(p.bias0 + co);
-        if (p.bias1) bsum += __ldg(p.bias1 + co);
-        const uint32_t t_addr = tmem_base + acc * kAccStride + ((uint32_t)(q * 32) << 16);
-        __nv_bfloat16* outp = reinterpret_cast<__nv_bfloat16*>(p.out);
-        float st_s = 0.f, st_ss = 0.f;
-        for (int c = 0; c < 256; c += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32(t_addr + c, v);
-          tmem_ld_wait();
-          uint8_t* buf = stage_s + ((c >> 5) & 1) * 8192;
+      const int nkb = (int)(((long long)p.num_kb * (split + 1)) / p.splits) -
+                      (int)(((long long)p.num_kb * split) / p.splits);
+      float acc[2][BN / 2];
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const __nv_bfloat16 hb = __float2bfloat16_rn(__uint_as_float(v[j]) + bsum);
-            if (p.gn_sums) {
-              const float r = __bfloat162float(hb);
-              st_s += r;
-              st_ss = fmaf(r, r, st_ss);
-            }
-            *reinterpret_cast<__nv_bfloat16*>(buf + j * 256 + row * 2) = hb;
-          }
-          asm volatile("bar.sync 1, 128;" ::: "memory");
+      for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int j = (warp - 2) * 8 + i * 2 + (lane >> 4);
-            const int vv = c + j;
-            const TileCoord tc = (vv >> 7) ? tcs1 : tcs0;
-            const int r = vv & 127;
-            const int dw = r & ((1 << p.bw_log2) - 1);
-            const int dh = (r >> p.bw_log2) & ((1 << p.bh_log2) - 1);
-            const int dt = (r >> (p.bw_log2 + p.bh_log2)) & ((1 << p.bt_log2) - 1);
-            const int dn = r >> (p.bw_log2 + p.bh_log2 + p.bt_log2);
-            const long long vox = (((long long)(tc.n0 + dn) * p.OT + tc.t0 + dt) * p.OH + tc.h0 + dh) * p.OW + tc.w0 + dw;
-            const uint4 u = *reinterpret_cast<const uint4*>(buf + j * 256 + (lane & 15) * 16);
-            *reinterpret_cast<uint4*>(outp + vox * p.ldo + n_tile * 128 + (lane & 15) * 8) = u;
-          }
+        for (int i = 0; i < BN / 2; ++i) acc[hh][i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
+        const uint32_t b_addr = a_addr + a_bytes;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) {
+          // A: K-major, 128-byte rows, 8-row groups 1024 B apart; advance 16 elements = 32 B inside the row.
+          // B: K-major [BN rows][64 k], or MN-major panels [BN/64][64 k-rows][128 B] (16 k-rows = 2048 B, panels 8 KiB apart)
+          const uint64_t bdesc = BMN ? gmma_desc_sw128(b_addr + k * 2048, 64 * 128, 1024)
+                                     : gmma_desc_sw128(b_addr + k * 32, 16, 1024);
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh)
+            wgmma_ss<BN, 0, BMN>(acc[hh], gmma_desc_sw128(a_addr + hh * 8192 + k * 32, 16, 1024), bdesc, 1);
         }
-        fl_s += st_s;
-        fl_ss += st_ss;
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous k-block's MMAs are done: its stage goes back to the producer
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == p.num_stages) {
+          stage = 0;
+          phase ^= 1;
+        }
       }
-      for (int ms = 0; ms < (p.swap ? 0 : p.m_sub); ++ms) {
-      const TileCoord tc = decode_m_tile(p, m_super * p.m_sub + ms);
+      wgmma_wait<0>();
+      reg_fence(acc[0]);
+      reg_fence(acc[1]);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+      // accumulator fragments -> fp32 tile in shared memory; the epilogue below reads one row per thread
+      asm volatile("bar.sync 1, 128;" ::: "memory");   // the previous tile's epilogue is done with acc_s
+      {
+        const int r0 = q * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            float* d0 = acc_s + (hh * 64 + r0) * acc_ld(BN) + j * 8 + c0;
+            *reinterpret_cast<float2*>(d0) = make_float2(acc[hh][4 * j], acc[hh][4 * j + 1]);
+            *reinterpret_cast<float2*>(d0 + 8 * acc_ld(BN)) = make_float2(acc[hh][4 * j + 2], acc[hh][4 * j + 3]);
+          }
+      }
+      asm volatile("bar.sync 1, 128;" ::: "memory");
+      const float* acc_row = acc_s + row * acc_ld(BN);
+
+      do {  // one pass; `continue` below leaves it for the tile's common tail
+      const TileCoord tc = decode_m_tile(p, m_super);
       const int dw = row & ((1 << p.bw_log2) - 1);
       const int dh = (row >> p.bw_log2) & ((1 << p.bh_log2) - 1);
       const int dt = (row >> (p.bw_log2 + p.bh_log2)) & ((1 << p.bt_log2) - 1);
@@ -457,15 +380,12 @@ __global__ void __launch_bounds__(kThreads, 1)
                             vw * p.om[2] + p.oo[2];
       const int col0 = n_tile * p.block_n;
 
-      const uint32_t t_addr = tmem_base + acc * kAccStride + ms * p.block_n + ((uint32_t)(q * 32) << 16);
-
       if (p.splits > 1) {
         // split-K: add this item's partial sums into the fp32 workspace (bias / cast happen in the finish pass)
         for (int c = 0; c < p.block_n; c += 32) {
           if (col0 + c >= p.n_out) break;
           uint32_t v[32];
-          tmem_ld_32x32(t_addr + c, v);
-          tmem_ld_wait();
+          ld_acc_row<32>(acc_row + c, v);
           if (row_ok && p.dbg != 1) {
             if (p.ws_slab) {
               // own slab: plain stores (each thread fills one 128-byte line of its row per chunk)
@@ -501,11 +421,11 @@ __global__ void __launch_bounds__(kThreads, 1)
 
       if (p.fast_store) {
         // bf16 output, whole 64-column chunks: registers -> (bias) -> bf16 -> swizzled smem staging -> the warp
-        // writes 4 full 128-byte row segments per instruction (the row-per-thread TMEM layout would otherwise
+        // writes 4 full 128-byte row segments per instruction (the row-per-thread accumulator layout would otherwise
         // scatter 16-byte pieces over 32 different lines per store).
-        if (ms == 0) {
+        {
           asm volatile("bar.sync 1, 128;" ::: "memory");  // previous tile's bias readers are done
-          for (int j = threadIdx.x - 64; j < p.block_n; j += 128) {
+          for (int j = et; j < p.block_n; j += 128) {
             const int col = col0 + j;
             float b = 0.f;
             if (col < p.n_out) {
@@ -521,14 +441,13 @@ __global__ void __launch_bounds__(kThreads, 1)
           asm volatile("bar.sync 1, 128;" ::: "memory");
         }
         float st_s = 0.f, st_ss = 0.f;
-        uint8_t* my_stage = stage_s + (warp - 2) * 4096;
+        uint8_t* my_stage = stage_s + q * 4096;
         __nv_bfloat16* outp = reinterpret_cast<__nv_bfloat16*>(p.out);
         for (int c = 0; c < p.block_n; c += 64) {
           if (col0 + c >= p.n_out) break;  // partial last N tile (n_out % 64 == 0, so chunks are all-or-nothing)
           uint32_t v0[32], v1[32];
-          tmem_ld_32x32(t_addr + c, v0);
-          tmem_ld_32x32(t_addr + c + 32, v1);
-          tmem_ld_wait();
+          ld_acc_row<32>(acc_row + c, v0);
+          ld_acc_row<32>(acc_row + c + 32, v1);
           if (p.residual && row_ok) {  // fp32 add before the single bf16 rounding
             const uint4* rp = reinterpret_cast<const uint4*>(p.residual + vox * p.ldo + col0 + c);
 #pragma unroll
@@ -652,17 +571,10 @@ __global__ void __launch_bounds__(kThreads, 1)
 
       for (int c = 0; c < p.block_n; c += 32) {
         uint32_t v[32];
-        if (p.block_n >= 32) {
-          tmem_ld_32x32(t_addr + c, v);
-        } else {
-          uint32_t v16[16];
-          tmem_ld_32x16(t_addr + c, v16);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = v16[j];
-#pragma unroll
-          for (int j = 16; j < 32; ++j) v[j] = 0;
-        }
-        tmem_ld_wait();
+        if (BN >= 32)
+          ld_acc_row<32>(acc_row + c, v);
+        else
+          ld_acc_row<16>(acc_row + c, v);
         const int cbase = col0 + c;
         if (cbase >= p.n_out || !row_ok) continue;
         float f[32];
@@ -705,18 +617,14 @@ __global__ void __launch_bounds__(kThreads, 1)
           }
         }
       }
-      }  // m_sub
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
+      } while (0);
       if (p.splits > 1 && p.tile_ctr) {
         // ---- fused split-K finish: the last of the `splits` items of this tile to arrive reduces nothing more — all
         // partial sums are already in `ws` (L2 reductions) — it reads the tile back, adds the bias, rounds, stores, emits
         // the GroupNorm sums and zeroes the tile for the next launch. Replaces a memset, a finish launch and a stats pass.
         __threadfence();
         asm volatile("bar.sync 1, 128;" ::: "memory");
-        const int et0 = threadIdx.x - 64;
-        if (et0 == 0) {
+        if (et == 0) {
           const unsigned int old = atomicAdd(p.tile_ctr + tile, 1u);
           const int last = old == (unsigned int)(p.splits - 1);
           if (last) p.tile_ctr[tile] = 0u;
@@ -730,8 +638,8 @@ __global__ void __launch_bounds__(kThreads, 1)
           // a warp walks its 32 rows one at a time, its lanes spread over the row's columns (8 per lane): every access is a
           // coalesced 1 KB row segment (the first version gave each thread a whole row: 32 scattered 32-byte pieces per
           // warp instruction made the finishing CTA 50 us slower than the separate finish launch it replaced)
-          for (int ms = 0; ms < p.m_sub; ++ms) {
-            const TileCoord tc = decode_m_tile(p, m_super * p.m_sub + ms);
+          {
+            const TileCoord tc = decode_m_tile(p, m_super);
             n_of_tile = tc.n0;
             const int col0 = n_tile * p.block_n;
 #pragma unroll 4
@@ -817,7 +725,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
       if (p.fast_store && p.splits == 1 && (p.gn_sums || p.red_S)) {
         // flush this tile's fused reductions (all rows of a CTA tile belong to one sample: host-checked)
-        const TileCoord tcf = decode_m_tile(p, m_super * p.m_sub);
+        const TileCoord tcf = decode_m_tile(p, m_super);
         if (p.gn_sums) {
           for (int o = 16; o > 0; o >>= 1) {
             fl_s += __shfl_xor_sync(0xffffffffu, fl_s, o);
@@ -829,7 +737,6 @@ __global__ void __launch_bounds__(kThreads, 1)
           }
         }
         asm volatile("bar.sync 1, 128;" ::: "memory");
-        const int et = threadIdx.x - 64;
         if (p.red_S) {
           const int col0f = n_tile * p.block_n;
           for (int j = et; j < 2 * p.block_n; j += 128) {
@@ -846,16 +753,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
         fl_s = fl_ss = 0.f;
       }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 
@@ -936,15 +834,27 @@ __global__ void __launch_bounds__(256)
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static int pick_block_n(int n_out, int num_m_tiles, bool mn_major) {
-  // The widest N tile that covers n_out (<= 256). Measured on B200: fewer, fatter tiles beat more, thinner ones
-  // even when they leave SMs idle (a 128x256 tile streams 96 B/MMA-clk, a 128x64 one 192 B/MMA-clk, and the
-  // TMA-latency x smem-capacity product caps what one SM can stream); low tile counts are handled by split-K.
+static int pick_block_n(int n_out, bool mn_major) {
+  // The widest N tile that covers n_out, up to 128: the 128 x 128 fp32 accumulator is 128 registers per thread of the
+  // one MMA warpgroup, the most that leaves room for addressing. Low tile counts are handled by split-K.
   int bn = 16;
-  while (bn < n_out && bn < 256) bn *= 2;
+  while (bn < n_out && bn < 128) bn *= 2;
   if (mn_major && bn < 64) bn = 64;
-  (void)num_m_tiles;
   return bn;
+}
+
+template <int BN, int BMN>
+static int launch_igemm_kernel(int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& mapA0,
+                               const CUtensorMap& mapA1, const CUtensorMap& mapB, const IgemmParams& p) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_conv_igemm_kernel<BN, BMN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       227 * 1024));
+    attr_set = true;
+  }
+  og_conv_igemm_kernel<BN, BMN><<<grid, kThreads, smem_bytes, stream>>>(mapA0, mapA1, mapB, p);
+  OG_CHECK_CUDA(cudaGetLastError());
+  return OG_OK;
 }
 
 struct IgemmLaunch {
@@ -1040,10 +950,10 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   p.H = H;
   p.W = W;
   p.num_m_tiles = ((N + bn - 1) / bn) * p.tiles_w * p.tiles_h * p.tiles_t;
-  p.block_n = pick_block_n(n_out, p.num_m_tiles, L.b_mn_major != 0);
+  p.block_n = pick_block_n(n_out, L.b_mn_major != 0);
   if (const char* e = getenv("OG_IGEMM_BN")) {  // tuning experiments only
     const int v = atoi(e);
-    if (v >= 16 && v <= 256 && (!L.b_mn_major || v >= 64)) p.block_n = v;
+    if ((v == 16 || v == 32 || v == 64 || v == 128) && (!L.b_mn_major || v >= 64)) p.block_n = v;
   }
   p.num_n_tiles = (n_out + p.block_n - 1) / p.block_n;
   p.n_out = n_out;
@@ -1054,14 +964,7 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   p.bias0 = L.bias0;
   p.bias1 = L.bias1;
   p.residual = reinterpret_cast<const __nv_bfloat16*>(L.residual);
-  // TMA latency x smem capacity bounds the bytes/clk one SM can stream; sharing each B stage between two
-  // 128-row M sub-tiles keeps the demand at (32+16) KB per 512 MMA-clk (same as a 128x256 tile).
-  p.m_sub = (p.block_n <= 128 && p.num_m_tiles >= 2 * num_sms()) ? 2 : 1;
-  if (const char* e = getenv("OG_IGEMM_MSUB")) {
-    const int v = atoi(e);
-    if ((v == 1 || v == 2) && v * p.block_n <= 256) p.m_sub = v;
-  }
-  const int stage_bytes = p.m_sub * kABytes + p.block_n * kBlockK * 2;
+  const int stage_bytes = kABytes + p.block_n * kBlockK * 2;
   p.fast_store = (!L.out_f32 && n_out % 64 == 0 && p.block_n % 64 == 0) ? 1 : 0;
   // dynamic tile scheduling: state lives in the last 256 bytes of the caller's workspace (og_workspace_init)
   p.sched = nullptr;
@@ -1070,19 +973,16 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   if (L.workspace && L.workspace_bytes >= 2 * kWsTail) {
     const size_t off = (L.workspace_bytes - kWsTail) & ~(size_t)255;
     ws_usable = off;
-    // in-kernel split-K finish: OFF by default. Measured on one B200 (profiles/r02p_*): it removes 98 launches per step
-    // (memset + finish + statistics pass) yet the graphed step is 64.0-64.7 ms with it and 62.95 ms without — the last
-    // arriver's fence + read-back sits on the tail of every split launch, while the three small launches it replaces cost
-    // ~3 us each inside a graph. OG_SPLITK_FUSED=1 enables it.
+    // in-kernel split-K finish: OFF by default. It removes the memset, finish and statistics launches of every split
+    // launch, but the last arriver's fence + read-back sits on the tail of the launch instead. OG_SPLITK_FUSED=1 enables it.
     static const bool fused_finish_on = [] {
       const char* e = getenv("OG_SPLITK_FUSED");
       return e && atoi(e) == 1;
     }();
     if (fused_finish_on && ws_prepared(L.workspace, L.workspace_bytes))
       tile_ctr = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(L.workspace) + off + 256);
-    // OFF by default: measured on 2 x B200 (profiles/r02k_*), the graphed data-parallel step takes 68.7 ms with either
-    // assignment and the single-GPU step is within noise (64.9 dynamic vs 64.6 static) — the cost of overlapping the
-    // all-reduce turned out to be power, not SM residency (DESIGN.md §5). OG_IGEMM_DYNAMIC=1 enables it.
+    // Dynamic tile assignment, OFF by default: it only helps when another kernel (a data-parallel all-reduce) holds SMs
+    // while this one launches. OG_IGEMM_DYNAMIC=1 enables it.
     static const bool dyn_on = [] {
       const char* e = getenv("OG_IGEMM_DYNAMIC");
       return e && atoi(e) == 1;
@@ -1096,7 +996,7 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   p.dbg = 0;
   if (const char* e = getenv("OG_IGEMM_DBG")) p.dbg = atoi(e);
   if (plain) {
-    const long long tiles = (long long)((p.num_m_tiles + p.m_sub - 1) / p.m_sub) * p.num_n_tiles;
+    const long long tiles = (long long)p.num_m_tiles * p.num_n_tiles;
     const size_t need = (size_t)N * T * H * W * n_out * sizeof(float);
     if (tiles * 2 <= num_sms() && p.num_kb >= 32 && L.workspace && ws_usable >= need && !L.residual) {
       int sp = (int)(num_sms() / tiles);
@@ -1120,7 +1020,7 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
       }
     }
   }
-  const int tail_bytes = 256 /*barriers*/ + 1024 /*bias*/ + 4 * 4096 /*store staging*/ + 4352 /*fused reductions*/;
+  const int tail_bytes = kTailBytes + kBlockM * acc_ld(p.block_n) * 4 /*fp32 accumulator tile*/;
   int stages = (227 * 1024 - 1024 /*align slack*/ - tail_bytes) / stage_bytes;
   if (stages > kMaxStages) stages = kMaxStages;
   p.num_stages = stages;
@@ -1169,33 +1069,29 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
     if (r != OG_OK) return r;
   }
 
-  static bool attr_set = false;
-  if (!attr_set) {
-    OG_CHECK_CUDA(cudaFuncSetAttribute(og_conv_igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  // operand swap for 128-wide Cout tiles (two voxel sub-tiles form the N = 256 operand): whole boxes only
-  p.swap = (plain && p.block_n == 128 && p.m_sub == 2 && p.fast_store && p.splits == 1 && !L.residual && !L.red_S &&
-            n_out % 128 == 0 && (p.num_m_tiles % 2 == 0) && W % bw == 0 && H % bh == 0 && T % bt == 0 && N % bn == 0)
-               ? 1 : 0;
-  if (const char* e = getenv("OG_IGEMM_SWAP")) {
-    if (atoi(e) == 0) p.swap = 0;
-  }
   // fused epilogue reductions need: staged bf16 stores, no split-K, every CTA tile inside one sample
-  const int tiles_per_sample = p.tiles_w * p.tiles_h * p.tiles_t;
-  const bool can_fuse = plain && p.fast_store && p.splits == 1 && bn == 1 && (tiles_per_sample % p.m_sub == 0) && n_out <= 65536;
-  const bool can_fuse_splitk = plain && p.splits > 1 && p.tile_ctr && bn == 1 && !L.out_f32 && (tiles_per_sample % p.m_sub == 0);
+  const bool can_fuse = plain && p.fast_store && p.splits == 1 && bn == 1 && n_out <= 65536;
+  const bool can_fuse_splitk = plain && p.splits > 1 && p.tile_ctr && bn == 1 && !L.out_f32;
   p.gn_sums = (L.gn_sums && (can_fuse || can_fuse_splitk)) ? L.gn_sums : nullptr;
   p.red_S = (L.red_S && can_fuse) ? L.red_S : nullptr;
   p.red_x = reinterpret_cast<const __nv_bfloat16*>(L.red_x);
   p.red_A = L.red_A;
   p.red_B = L.red_B;
   p.red_act = L.red_act;
-  const int total_tiles = ((p.num_m_tiles + p.m_sub - 1) / p.m_sub) * p.num_n_tiles * p.splits;
+  const int total_tiles = p.num_m_tiles * p.num_n_tiles * p.splits;
   int grid = num_sms();
   if (grid > total_tiles) grid = total_tiles;
-  og_conv_igemm_kernel<<<grid, kThreads, smem_bytes, stream>>>(mapA0, mapA1, mapB, p);
-  OG_CHECK_CUDA(cudaGetLastError());
+  int rc;
+  switch (p.block_n * 2 + p.b_mn_major) {
+    case 16 * 2: rc = launch_igemm_kernel<16, 0>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p); break;
+    case 32 * 2: rc = launch_igemm_kernel<32, 0>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p); break;
+    case 64 * 2: rc = launch_igemm_kernel<64, 0>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p); break;
+    case 128 * 2: rc = launch_igemm_kernel<128, 0>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p); break;
+    case 64 * 2 + 1: rc = launch_igemm_kernel<64, 1>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p); break;
+    case 128 * 2 + 1: rc = launch_igemm_kernel<128, 1>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p); break;
+    default: OG_REQUIRE(false, "conv3d: no kernel for block_n=%d", p.block_n);
+  }
+  if (rc != OG_OK) return rc;
   g_launches.fetch_add(1);
   bool finish_did_stats = false;
   if (p.splits > 1 && !p.tile_ctr) {
@@ -1226,7 +1122,7 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   }
   if (L.red_S && !p.red_S) {
     OG_REQUIRE(!L.out_f32 && plain, "conv3d: fused backward reduction needs a plain bf16 output");
-    int r = og_affine_act_bwd_reduce(L.out, L.red_x, L.red_A, L.red_B, L.red_act, L.red_S, N, (int64_t)T * H * W, n_out,
+    int r = og_affine_act_bwd_reduce(L.out, L.red_x, L.red_A, L.red_B, L.red_act, L.red_S, N, (int64_t)T * H * W, n_out, nullptr, 0,
                                      (og_stream_t)stream);
     if (r != OG_OK) return r;
   }

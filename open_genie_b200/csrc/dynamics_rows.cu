@@ -126,7 +126,7 @@ __global__ void og_masked_ce_bwd_kernel(const __nv_bfloat16* __restrict__ logits
 // MaskGIT sampling (DynamicsModel.generate, genie/dynamics.py:101-165)
 //
 // In the reference loop the transformer input `tok_id` is packed ONCE before the loop and never updated (lines
-// 128-134), so every iteration sees the same logits; only the multinomial draws differ. The B200 form therefore
+// 128-134), so every iteration sees the same logits; only the multinomial draws differ. The GPU form therefore
 // evaluates the transformer once, turns the last frame's logits into per-position CDFs once (og_softmax_cdf), and runs
 // ALL sampling iterations in one launch (og_maskgit_sample: one CTA per batch row; per iteration inverse-CDF draw ->
 // confidence -> mask already-predicted positions to -inf -> top-k -> scatter into code / mask).

@@ -1,29 +1,25 @@
-// flash_attn.cu — spatial (non-causal) multi-head attention, FlashAttention-style, on tcgen05 tensor cores.
+// flash_attn.cu — spatial (non-causal) multi-head attention, FlashAttention-style, on the Hopper tensor cores (wgmma).
 //
 // Reference: F.scaled_dot_product_attention(q, k, v, scale = n_head * d_head**-0.5) reached from
 // SpatialAttention.forward -> Attention.forward (genie/module/attention.py:279-307, 199-239), with
 // q = k = v = LayerNorm(RoPE(x)) in the HEAD-valid configuration. Layout: [nseq][S][C] bf16 rows
 // (one sequence = the H*W tokens of one frame, contiguous in NDHWC), head h = columns [h*64, h*64+64).
 //
-// Forward, one CTA per (sequence, head, 128-query tile), loop over 128-key tiles:
-//   S  = Q K^T           tcgen05.mma, A = Q tile (K-major), B = K tile (K-major)      -> TMEM [128][128] fp32
-//   P  = exp(S*scale - m) softmax warps: one TMEM lane (= query row) per thread, online max / sum in registers,
-//                         P written as bf16 into a 128-byte-swizzled smem tile (the A operand of the next MMA)
-//   PV = P V             tcgen05.mma, A = P (K-major, smem), B = V tile (MN-major: keys are the K dim)
-//   O += PV              accumulated in TMEM by the MMA; rescaled in place only when a row maximum jumps (lazy rescale)
-// Q/K/V tiles arrive by 3-D TMA (rows beyond S are zero-filled and masked to -inf).
-// Backward recomputes P from the saved log-sum-exp in two passes: dV / dK accumulate in TMEM per key tile, dQ per query
-// tile (no atomics, no fp32 gradient buffers).
+// Every kernel is one warpgroup (128 threads) owning a 64-row tile; thread 0 streams the other operand's 64-row tiles
+// through a two-stage TMA ring (rows beyond S are zero-filled by TMA and masked). Accumulators live in registers in the
+// wgmma fragment layout (og_ptx.cuh): a thread holds two rows, r0 = 16*warp + lane/4 and r0 + 8.
 //
-// Kernels in this file (the host entry points pick; DESIGN.md section 6 has the measurements behind each step):
-//   og_flash_attn_fwd_kernel    one CTA per work item, two CTAs per SM                          (S > 1024)
-//   og_flash_attn_fwd2_kernel   persistent form of it                                           (S <= 1024)
-//   og_flash_attn_bwd3_kernel   backward, software-pipelined AND persistent                     (default)
-//   og_flash_attn_bwd2_kernel   backward, software-pipelined, one CTA per work item             (OG_FLASH_BWD_PERSISTENT=0,
-//                               16-warp / non-interleaved variants, knock-out timing switches)
-//   og_flash_attn_bwd_kernel    backward, first version: S,dP -> softmax -> gradients in turn   (OG_FLASH_BWD_V1=1)
-#include <type_traits>
-
+// Forward, one CTA per (sequence, head, 64-query tile), loop over 64-key tiles:
+//   S  = Q K^T           wgmma, A = Q tile (K-major smem), B = K tile (K-major smem)
+//   P  = exp(S*scale - m) online max / sum in registers (base 2 with the scale folded in)
+//   O  = O*alpha + P V    wgmma, A = P straight from the S registers (bf16), B = V tile (MN-major: keys are the K dim)
+// Backward recomputes P from the saved log-sum-exp in two passes, both recomputing S and dP = dO V^T:
+//   MODE 0: one CTA per key tile j, streams the query tiles i, computes the transposed scores S^T = K Q^T and
+//             dV_j += P^T dO_i,  dK_j += dS^T Q_i        (A = P^T / dS^T from registers, B = dO_i / Q_i MN-major)
+//   MODE 1: one CTA per query tile i, streams the key tiles j:
+//             dQ_i += dS K_j                             (A = dS from registers, B = K_j MN-major)
+// with P = exp(S*scale - lse), dS = P * (dP - delta) * scale, delta = rowsum(dO * O).
+// No atomics, no fp32 gradient buffers; outputs are bf16 in the activation layout.
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 
@@ -31,10 +27,9 @@ namespace og {
 extern std::atomic<uint64_t> g_launches;
 
 static constexpr int kD = 64;            // head dim
-static constexpr int kTile = 128;        // queries / keys per tile
-static constexpr int kTileBytes = kTile * kD * 2;  // 16 KiB
-static constexpr int kFaThreads = 192;
-static constexpr int kFaBwdThreads = 320;  // warp 0 TMA, warp 1 MMA, 8 softmax warps (two per TMEM lane quarter)
+static constexpr int kTile = 64;         // rows per tile (queries or keys)
+static constexpr int kTileBytes = kTile * kD * 2;  // 8 KiB
+static constexpr int kFaThreads = 128;
 
 struct FaParams {
   int S, C, nh, nseq;
@@ -46,623 +41,8 @@ struct FaParams {
   __nv_bfloat16* out_res;
 };
 
-// write 8 consecutive bf16 (one 16-byte chunk) of row `row`, chunk index `chunk` (0..7) into a
-// [rows][128 B] tile with the 128-byte swizzle TMA / UMMA use (chunk ^= row & 7)
-__device__ __forceinline__ void st_swizzled_chunk(uint8_t* tile, int row, int chunk, uint4 v) {
-  *reinterpret_cast<uint4*>(tile + row * 128 + ((chunk ^ (row & 7)) << 4)) = v;
-}
-
-// Ordered variants (volatile asm keeps their relative program order): used to INTERLEAVE the MUFU exponentials of one
-// column chunk with the FMA / ALU / store work of the previous one — left alone, ptxas emits 32 MUFU.EX2 back to back
-// (8 clk each on the 4-lane XU pipe) and the other pipes idle meanwhile.
-__device__ __forceinline__ float ex2_ordered(float x) {
-  float y;
-  asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ void st_swizzled_chunk_ordered(uint8_t* tile, int row, int chunk, uint4 v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(smem_u32(tile + row * 128 + ((chunk ^ (row & 7)) << 4))),
-               "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
-               : "memory");
-}
-
-__global__ void __launch_bounds__(kFaThreads, 2)
-    og_flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                             const __grid_constant__ CUtensorMap mapV, const FaParams p) {
-  // Two CTAs per SM (their softmax / MMA phases interleave), so every byte counts: 7 tiles + barriers =
-  // 114.8 KB; the 1024-byte alignment the swizzled TMA tiles need is requested from the declaration instead
-  // of reserving slack for a manual round-up (checked below).
-  extern __shared__ __align__(1024) uint8_t smem_fwd[];
-  uint8_t* smem = smem_fwd;
-  if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint8_t* sQ = smem;                         // 16 KiB
-  uint8_t* sKV = smem + kTileBytes;           // 2 stages x (K 16 KiB + V 16 KiB)
-  uint8_t* sP = sKV + 4 * kTileBytes;         // 2 k-blocks x 16 KiB
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * kTileBytes);
-  uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;   // [2]
-  uint64_t* kv_empty = bars + 3;  // [2]
-  uint64_t* s_ready = bars + 5;
-  uint64_t* p_ready = bars + 6;
-  uint64_t* pv_ready = bars + 7;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-
-  const int warp = warp_idx_uniform(), lane = threadIdx.x & 31;
-  int id = blockIdx.x;
-  const int qt = id % p.q_tiles;
-  id /= p.q_tiles;
-  const int h = id % p.nh;
-  const int seq = id / p.nh;
-  const int q0 = qt * kTile;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&mapQ);
-    tma_prefetch_desc(&mapK);
-    tma_prefetch_desc(&mapV);
-    mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
-    }
-    mbar_init(s_ready, 1);
-    mbar_init(p_ready, 4);
-    mbar_init(pv_ready, 1);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base;         // 128 columns
-  const uint32_t tPV = tmem_base + 128;  // 64 columns
-
-  if (warp == 0) {
-    {  // converged warp, one elected lane issues (og_ptx.cuh: elect_one)
-      if (elect_one()) {
-        mbar_expect_tx(q_full, kTileBytes);
-        tma_load_3d(sQ, &mapQ, q_full, h * kD, q0, seq);
-      }
-      __syncwarp();
-      for (int j = 0; j < p.kv_tiles; ++j) {
-        const int st = j & 1;
-        const uint32_t ph = (j >> 1) & 1;
-        mbar_wait(&kv_empty[st], ph ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(&kv_full[st], 2 * kTileBytes);
-          tma_load_3d(sKV + st * 2 * kTileBytes, &mapK, &kv_full[st], h * kD, j * kTile, seq);
-          tma_load_3d(sKV + st * 2 * kTileBytes + kTileBytes, &mapV, &kv_full[st], h * kD, j * kTile, seq);
-        }
-        __syncwarp();
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    {
-      const uint32_t idesc_s = umma_idesc_bf16(128, 128, 0u, 0u);   // S = Q K^T : both K-major
-      const uint32_t idesc_pv = umma_idesc_bf16(128, 64, 0u, 1u);   // PV = P V  : A K-major, B MN-major
-      const uint32_t q_addr = smem_u32(sQ), p_addr = smem_u32(sP);
-      mbar_wait(q_full, 0);
-      for (int j = 0; j <= p.kv_tiles; ++j) {
-        if (j < p.kv_tiles) {
-          // S_j = Q K_j^T (issued before PV_{j-1} completes its consumer side: overlaps the softmax warps' O update)
-          const int st = j & 1;
-          mbar_wait(&kv_full[st], (j >> 1) & 1);
-          tc_fence_after();
-          if (j > 0) {
-            // S buffer is free once P_{j-1} has been written (the softmax warps are done reading S_{j-1})
-            mbar_wait(p_ready, (j - 1) & 1);
-            tc_fence_after();
-          }
-          const uint32_t k_addr = smem_u32(sKV + st * 2 * kTileBytes);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < kD / 16; ++k)
-              umma_bf16_ss(tS, umma_smem_desc_sw128(q_addr + k * 32, 16, 1024),
-                           umma_smem_desc_sw128(k_addr + k * 32, 16, 1024), idesc_s, k > 0 ? 1u : 0u);
-            umma_commit(s_ready);
-          }
-          __syncwarp();
-        }
-        if (j > 0) {
-          // PV_{j-1} = P_{j-1} V_{j-1}
-          const int jj = j - 1, st = jj & 1;
-          if (j == p.kv_tiles) {  // otherwise already waited above
-            mbar_wait(p_ready, jj & 1);
-            tc_fence_after();
-          }
-          const uint32_t v_addr = smem_u32(sKV + st * 2 * kTileBytes + kTileBytes);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < kTile / 16; ++k)
-              umma_bf16_ss(tPV, umma_smem_desc_sw128(p_addr + (k >> 2) * kTileBytes + (k & 3) * 32, 16, 1024),
-                           umma_smem_desc_sw128(v_addr + k * 2048, 8192, 1024), idesc_pv, (jj > 0 || k > 0) ? 1u : 0u);
-            umma_commit(pv_ready);
-            umma_commit(&kv_empty[st]);
-          }
-          __syncwarp();
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ============================ softmax / output warps: thread = query row ============================
-    // Online softmax in base 2 with the scale folded in: p = 2^(s*c - m), c = scale*log2(e)  (one FFMA + one
-    // MUFU.EX2 per element). O stays in TMEM and is accumulated by the PV MMAs; it is only rescaled (TMEM ->
-    // registers -> TMEM) when some row of the warp raised its running maximum by more than 2^8 — until then the
-    // stale maximum is kept, P and l stay mutually consistent and the final O/l is exact (FA-4's lazy rescale).
-    const int qd = warp & 3;
-    const int row = qd * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(qd * 32) << 16;
-    const float cl2 = p.scale * 1.4426950408889634f;
-    float m = -INFINITY, l = 0.f;
-    for (int j = 0; j < p.kv_tiles; ++j) {
-      mbar_wait(s_ready, j & 1);
-      tc_fence_after();
-      const int kv_valid = p.S - j * kTile;  // keys of this tile that exist (>= 128 except for the last tile)
-      // pass 1: row max of the raw scores
-      float mt = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < kTile; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(tS + lane_addr + c, v);
-        tmem_ld_wait();
-        if (kv_valid >= kTile) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) mt = fmaxf(mt, __uint_as_float(v[i]));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (c + i < kv_valid) mt = fmaxf(mt, __uint_as_float(v[i]));
-        }
-      }
-      mt *= cl2;  // scale > 0
-      float mn = m, alpha = 1.f;
-      if (mt > m + 8.f) {  // (first tile: m = -inf)
-        mn = mt;
-        alpha = ex2_approx(m - mn);
-      }
-      if (j > 0) {
-        // O (TMEM) holds sum_{j' < j} P V once PV_{j-1} has completed
-        mbar_wait(pv_ready, (j - 1) & 1);
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, alpha != 1.f)) {
-#pragma unroll
-          for (int c = 0; c < kD; c += 32) {
-            uint32_t v[32];
-            tmem_ld_32x32(tPV + lane_addr + c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-            tmem_st_32x32(tPV + lane_addr + c, v);
-          }
-          tmem_st_wait();
-        }
-      }
-      // pass 2: P = 2^(s*c - m), row sum, bf16 P -> swizzled smem
-      float ls = 0.f;
-#pragma unroll
-      for (int c = 0; c < kTile; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(tS + lane_addr + c, v);
-        tmem_ld_wait();
-        float pf[32];
-        if (kv_valid >= kTile) {  // whole key tile (every tile but possibly the last): no per-element select / compare
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            pf[i] = ex2_approx(fmaf(__uint_as_float(v[i]), cl2, -mn));
-            ls += pf[i];
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float e = ex2_approx(fmaf(__uint_as_float(v[i]), cl2, -mn));
-            pf[i] = (c + i < kv_valid) ? e : 0.f;
-            ls += pf[i];
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          uint4 u;
-          u.x = pack_bf16x2(pf[i], pf[i + 1]);
-          u.y = pack_bf16x2(pf[i + 2], pf[i + 3]);
-          u.z = pack_bf16x2(pf[i + 4], pf[i + 5]);
-          u.w = pack_bf16x2(pf[i + 6], pf[i + 7]);
-          const int col = c + i;
-          st_swizzled_chunk(sP + (col >> 6) * kTileBytes, row, (col & 63) >> 3, u);
-        }
-      }
-      l = l * alpha + ls;
-      m = mn;
-      // make the generic-proxy smem writes (and the TMEM rescale) visible to the tensor core, then signal
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_ready);
-    }
-    // final O: wait for the last PV, normalise
-    mbar_wait(pv_ready, (p.kv_tiles - 1) & 1);
-    tc_fence_after();
-    float o[kD];
-#pragma unroll
-    for (int c = 0; c < kD; c += 32) {
-      uint32_t v[32];
-      tmem_ld_32x32(tPV + lane_addr + c, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) o[c + i] = __uint_as_float(v[i]);
-    }
-    tc_fence_before();
-    const int qrow = q0 + row;
-    if (qrow < p.S) {
-      const float inv = 1.f / l;
-      __nv_bfloat16* dst = p.out + ((long long)seq * p.S + qrow) * p.C + h * kD;
-#pragma unroll
-      for (int i = 0; i < kD; ++i) o[i] *= inv;
-#pragma unroll
-      for (int i = 0; i < kD; i += 8) {
-        uint4 u;
-        u.x = pack_bf16x2(o[i], o[i + 1]);
-        u.y = pack_bf16x2(o[i + 2], o[i + 3]);
-        u.z = pack_bf16x2(o[i + 4], o[i + 5]);
-        u.w = pack_bf16x2(o[i + 6], o[i + 7]);
-        *reinterpret_cast<uint4*>(dst + i) = u;
-      }
-      if (p.res) {  // second output: attention + residual, added in fp32 before the rounding
-        const long long off = ((long long)seq * p.S + qrow) * p.C + h * kD;
-        const uint4* rp = reinterpret_cast<const uint4*>(p.res + off);
-        __nv_bfloat16* dst2 = p.out_res + off;
-#pragma unroll
-        for (int i = 0; i < kD; i += 8) {
-          const uint4 ur = __ldg(rp + (i >> 3));
-          const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&ur);
-          float f[8];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 t = __bfloat1622float2(hh[e]);
-            f[2 * e] = o[i + 2 * e] + t.x;
-            f[2 * e + 1] = o[i + 2 * e + 1] + t.y;
-          }
-          uint4 u;
-          u.x = pack_bf16x2(f[0], f[1]);
-          u.y = pack_bf16x2(f[2], f[3]);
-          u.z = pack_bf16x2(f[4], f[5]);
-          u.w = pack_bf16x2(f[6], f[7]);
-          *reinterpret_cast<uint4*>(dst2 + i) = u;
-        }
-      }
-      if (p.lse) p.lse[((long long)seq * p.nh + h) * p.S + qrow] = (m + __log2f(l)) * 0.6931471805599453f;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// forward, persistent form of og_flash_attn_fwd_kernel: two CTAs per SM walk the (frame, head, query tile) work items;
-// TMEM, barriers and tensor maps are set up once, barrier parities derive from running counters (J = global K/V tile
-// index, wi = work item index), and the next item's Q / first K/V tiles and S_0 are in flight while the softmax warps
-// normalise and store the current item's output (see og_flash_attn_bwd3_kernel for the measured motivation).
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kFaThreads, 2)
-    og_flash_attn_fwd2_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                              const __grid_constant__ CUtensorMap mapV, const FaParams p, const int total_items) {
-  // Two CTAs per SM (their softmax / MMA phases interleave), so every byte counts: 7 tiles + barriers =
-  // 114.8 KB; the 1024-byte alignment the swizzled TMA tiles need is requested from the declaration instead
-  // of reserving slack for a manual round-up (checked below).
-  extern __shared__ __align__(1024) uint8_t smem_fwd[];
-  uint8_t* smem = smem_fwd;
-  if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint8_t* sQ = smem;                         // 16 KiB
-  uint8_t* sKV = smem + kTileBytes;           // 2 stages x (K 16 KiB + V 16 KiB)
-  uint8_t* sP = sKV + 4 * kTileBytes;         // 2 k-blocks x 16 KiB
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * kTileBytes);
-  uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;   // [2]
-  uint64_t* kv_empty = bars + 3;  // [2]
-  uint64_t* s_ready = bars + 5;
-  uint64_t* p_ready = bars + 6;
-  uint64_t* pv_ready = bars + 7;
-  uint64_t* q_empty = bars + 8;   // the item's last S MMA has read the Q tile
-  uint64_t* o_free = bars + 9;    // the softmax warps hold the item's O accumulator in registers
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 10);
-
-  const int warp = warp_idx_uniform(), lane = threadIdx.x & 31;
-  const int kvt = p.kv_tiles;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&mapQ);
-    tma_prefetch_desc(&mapK);
-    tma_prefetch_desc(&mapV);
-    mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
-    }
-    mbar_init(s_ready, 1);
-    mbar_init(p_ready, 4);
-    mbar_init(pv_ready, 1);
-    mbar_init(q_empty, 1);
-    mbar_init(o_free, 4);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base;         // 128 columns
-  const uint32_t tPV = tmem_base + 128;  // 64 columns
-
-  if (warp == 0) {
-    int J = 0, wi = 0;
-    for (int w = blockIdx.x; w < total_items; w += gridDim.x, ++wi) {
-      int id = w;
-      const int qt = id % p.q_tiles;
-      id /= p.q_tiles;
-      const int h = id % p.nh, seq = id / p.nh;
-      mbar_wait(q_empty, (wi & 1) ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(q_full, kTileBytes);
-        tma_load_3d(sQ, &mapQ, q_full, h * kD, qt * kTile, seq);
-      }
-      __syncwarp();
-      for (int j = 0; j < kvt; ++j, ++J) {
-        const int st = J & 1;
-        mbar_wait(&kv_empty[st], ((J >> 1) & 1) ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(&kv_full[st], 2 * kTileBytes);
-          tma_load_3d(sKV + st * 2 * kTileBytes, &mapK, &kv_full[st], h * kD, j * kTile, seq);
-          tma_load_3d(sKV + st * 2 * kTileBytes + kTileBytes, &mapV, &kv_full[st], h * kD, j * kTile, seq);
-        }
-        __syncwarp();
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    const uint32_t idesc_s = umma_idesc_bf16(128, 128, 0u, 0u);   // S = Q K^T : both K-major
-    const uint32_t idesc_pv = umma_idesc_bf16(128, 64, 0u, 1u);   // PV = P V  : A K-major, B MN-major
-    const uint32_t q_addr = smem_u32(sQ), p_addr = smem_u32(sP);
-    int J0 = 0, wi = 0;
-    for (int w = blockIdx.x; w < total_items; w += gridDim.x, ++wi, J0 += kvt) {
-      mbar_wait(q_full, wi & 1);
-      tc_fence_after();
-      for (int j = 0; j <= kvt; ++j) {
-        const int J = J0 + j;
-        if (j < kvt) {
-          const int st = J & 1;
-          mbar_wait(&kv_full[st], (J >> 1) & 1);
-          tc_fence_after();
-          if (J > 0) {
-            // S buffer is free once P of the previous tile (of this or the previous item) has been written
-            mbar_wait(p_ready, (J - 1) & 1);
-            tc_fence_after();
-          }
-          const uint32_t k_addr = smem_u32(sKV + st * 2 * kTileBytes);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < kD / 16; ++k)
-              umma_bf16_ss(tS, umma_smem_desc_sw128(q_addr + k * 32, 16, 1024),
-                           umma_smem_desc_sw128(k_addr + k * 32, 16, 1024), idesc_s, k > 0 ? 1u : 0u);
-            umma_commit(s_ready);
-            if (j == kvt - 1) umma_commit(q_empty);
-          }
-          __syncwarp();
-        }
-        if (j > 0) {
-          const int jj = j - 1, Jj = J - 1, st = Jj & 1;
-          if (j == kvt) {  // otherwise already waited above
-            mbar_wait(p_ready, Jj & 1);
-            tc_fence_after();
-          }
-          if (jj == 0 && wi > 0) {   // PV_0 overwrites O: the previous item's must have been read
-            mbar_wait(o_free, (wi - 1) & 1);
-            tc_fence_after();
-          }
-          const uint32_t v_addr = smem_u32(sKV + st * 2 * kTileBytes + kTileBytes);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < kTile / 16; ++k)
-              umma_bf16_ss(tPV, umma_smem_desc_sw128(p_addr + (k >> 2) * kTileBytes + (k & 3) * 32, 16, 1024),
-                           umma_smem_desc_sw128(v_addr + k * 2048, 8192, 1024), idesc_pv, (jj > 0 || k > 0) ? 1u : 0u);
-            umma_commit(pv_ready);
-            umma_commit(&kv_empty[st]);
-          }
-          __syncwarp();
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ============================ softmax / output warps: thread = query row ============================
-    // Online softmax in base 2 with the scale folded in: p = 2^(s*c - m), c = scale*log2(e)  (one FFMA + one
-    // MUFU.EX2 per element). O stays in TMEM and is accumulated by the PV MMAs; it is only rescaled (TMEM ->
-    // registers -> TMEM) when some row of the warp raised its running maximum by more than 2^8 — until then the
-    // stale maximum is kept, P and l stay mutually consistent and the final O/l is exact (FA-4's lazy rescale).
-    const int qd = warp & 3;
-    const int row = qd * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(qd * 32) << 16;
-    const float cl2 = p.scale * 1.4426950408889634f;
-    int J0 = 0, wi = 0;
-    for (int w = blockIdx.x; w < total_items; w += gridDim.x, ++wi, J0 += kvt) {
-    int id = w;
-    const int qt = id % p.q_tiles;
-    id /= p.q_tiles;
-    const int h = id % p.nh, seq = id / p.nh;
-    const int q0 = qt * kTile;
-    float m = -INFINITY, l = 0.f;
-    for (int j = 0; j < kvt; ++j) {
-      mbar_wait(s_ready, (J0 + j) & 1);
-      tc_fence_after();
-      const int kv_valid = p.S - j * kTile;  // keys of this tile that exist (>= 128 except for the last tile)
-      // pass 1: row max of the raw scores
-      float mt = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < kTile; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(tS + lane_addr + c, v);
-        tmem_ld_wait();
-        if (kv_valid >= kTile) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) mt = fmaxf(mt, __uint_as_float(v[i]));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (c + i < kv_valid) mt = fmaxf(mt, __uint_as_float(v[i]));
-        }
-      }
-      mt *= cl2;  // scale > 0
-      float mn = m, alpha = 1.f;
-      if (mt > m + 8.f) {  // (first tile: m = -inf)
-        mn = mt;
-        alpha = ex2_approx(m - mn);
-      }
-      if (j > 0) {
-        // O (TMEM) holds sum_{j' < j} P V once PV_{j-1} has completed
-        mbar_wait(pv_ready, (J0 + j - 1) & 1);
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, alpha != 1.f)) {
-#pragma unroll
-          for (int c = 0; c < kD; c += 32) {
-            uint32_t v[32];
-            tmem_ld_32x32(tPV + lane_addr + c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-            tmem_st_32x32(tPV + lane_addr + c, v);
-          }
-          tmem_st_wait();
-        }
-      }
-      // pass 2: P = 2^(s*c - m), row sum, bf16 P -> swizzled smem
-      float ls = 0.f;
-#pragma unroll
-      for (int c = 0; c < kTile; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(tS + lane_addr + c, v);
-        tmem_ld_wait();
-        float pf[32];
-        if (kv_valid >= kTile) {  // whole key tile (every tile but possibly the last): no per-element select / compare
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            pf[i] = ex2_approx(fmaf(__uint_as_float(v[i]), cl2, -mn));
-            ls += pf[i];
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float e = ex2_approx(fmaf(__uint_as_float(v[i]), cl2, -mn));
-            pf[i] = (c + i < kv_valid) ? e : 0.f;
-            ls += pf[i];
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          uint4 u;
-          u.x = pack_bf16x2(pf[i], pf[i + 1]);
-          u.y = pack_bf16x2(pf[i + 2], pf[i + 3]);
-          u.z = pack_bf16x2(pf[i + 4], pf[i + 5]);
-          u.w = pack_bf16x2(pf[i + 6], pf[i + 7]);
-          const int col = c + i;
-          st_swizzled_chunk(sP + (col >> 6) * kTileBytes, row, (col & 63) >> 3, u);
-        }
-      }
-      l = l * alpha + ls;
-      m = mn;
-      // make the generic-proxy smem writes (and the TMEM rescale) visible to the tensor core, then signal
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_ready);
-    }
-    // final O: wait for the last PV, normalise
-    mbar_wait(pv_ready, (J0 + kvt - 1) & 1);
-    tc_fence_after();
-    float o[kD];
-#pragma unroll
-    for (int c = 0; c < kD; c += 32) {
-      uint32_t v[32];
-      tmem_ld_32x32(tPV + lane_addr + c, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) o[c + i] = __uint_as_float(v[i]);
-    }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(o_free);   // the next item's first PV MMA may overwrite O
-    const int qrow = q0 + row;
-    if (qrow < p.S) {
-      const float inv = 1.f / l;
-      __nv_bfloat16* dst = p.out + ((long long)seq * p.S + qrow) * p.C + h * kD;
-#pragma unroll
-      for (int i = 0; i < kD; ++i) o[i] *= inv;
-#pragma unroll
-      for (int i = 0; i < kD; i += 8) {
-        uint4 u;
-        u.x = pack_bf16x2(o[i], o[i + 1]);
-        u.y = pack_bf16x2(o[i + 2], o[i + 3]);
-        u.z = pack_bf16x2(o[i + 4], o[i + 5]);
-        u.w = pack_bf16x2(o[i + 6], o[i + 7]);
-        *reinterpret_cast<uint4*>(dst + i) = u;
-      }
-      if (p.res) {  // second output: attention + residual, added in fp32 before the rounding
-        const long long off = ((long long)seq * p.S + qrow) * p.C + h * kD;
-        const uint4* rp = reinterpret_cast<const uint4*>(p.res + off);
-        __nv_bfloat16* dst2 = p.out_res + off;
-#pragma unroll
-        for (int i = 0; i < kD; i += 8) {
-          const uint4 ur = __ldg(rp + (i >> 3));
-          const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&ur);
-          float f[8];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 t = __bfloat1622float2(hh[e]);
-            f[2 * e] = o[i + 2 * e] + t.x;
-            f[2 * e + 1] = o[i + 2 * e + 1] + t.y;
-          }
-          uint4 u;
-          u.x = pack_bf16x2(f[0], f[1]);
-          u.y = pack_bf16x2(f[2], f[3]);
-          u.z = pack_bf16x2(f[4], f[5]);
-          u.w = pack_bf16x2(f[6], f[7]);
-          *reinterpret_cast<uint4*>(dst2 + i) = u;
-        }
-      }
-      if (p.lse) p.lse[((long long)seq * p.nh + h) * p.S + qrow] = (m + __log2f(l)) * 0.6931471805599453f;
-    }
-    }   // work items
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// backward. Two passes over the (q tile, kv tile) pairs, both recomputing S = Q K^T and dP = dO V^T:
-//   MODE 0: one CTA per KV tile j, streams the query tiles i, accumulates in TMEM
-//             dV_j += P^T dO_i      (A = P   as MN-major operand, B = dO_i MN-major)
-//             dK_j += dS^T Q_i      (A = dS  as MN-major operand, B = Q_i  MN-major)
-//   MODE 1: one CTA per query tile i, streams the KV tiles j, accumulates
-//             dQ_i += dS K_j        (A = dS K-major, B = K_j MN-major)
-// with P = exp(S*scale - lse), dS = P * (dP - delta) * scale, delta = rowsum(dO * O).
-// No atomics, no fp32 gradient buffers; outputs are bf16 in the activation layout.
-// ------------------------------------------------------------------------------------------------
 struct FaBwdParams {
   int S, C, nh, nseq, tiles;
-  int interleave;  // bwd2, 8 softmax warps: interleave exponentials with the previous chunk's dS work
-  int dbg;         // timing experiments only (OG_FLASH_DBG; results are wrong): 1 = no MUFU.EX2, 2 = no P / dS smem stores,
-                   // 4 = no gradient MMAs, 8 = no S / dP MMAs, 32 = softmax warps run the barrier protocol only (+16: no TMEM loads), 64 = no TMA stream loads
   float scale;
   const float* lse;    // [nseq][nh][S]
   const float* delta;  // [nseq][nh][S]
@@ -671,1070 +51,312 @@ struct FaBwdParams {
   __nv_bfloat16* dv;
 };
 
+// S-fragment (m64n64 fp32) -> the bf16 A operand of the next wgmma, one k16 slice per kk (og_ptx.cuh layouts: the
+// accumulator columns 16kk..16kk+15 of a thread's two rows are exactly its A fragment of that slice)
+__device__ __forceinline__ void frag_to_a(const float (&x)[32], uint32_t (&a)[4][4]) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    a[kk][0] = pack_bf16x2(x[8 * kk], x[8 * kk + 1]);
+    a[kk][1] = pack_bf16x2(x[8 * kk + 2], x[8 * kk + 3]);
+    a[kk][2] = pack_bf16x2(x[8 * kk + 4], x[8 * kk + 5]);
+    a[kk][3] = pack_bf16x2(x[8 * kk + 6], x[8 * kk + 7]);
+  }
+}
+
+// D = X Y^T over the 64 head dims: both tiles K-major [64 rows][64 d] with the 128-byte swizzle
+__device__ __forceinline__ void gemm_rows(float (&d)[32], uint32_t x_addr, uint32_t y_addr) {
+#pragma unroll
+  for (int k = 0; k < kD / 16; ++k)
+    wgmma_ss<64, 0, 0>(d, gmma_desc_sw128(x_addr + k * 32, 16, 1024), gmma_desc_sw128(y_addr + k * 32, 16, 1024), k > 0);
+}
+
+// D += A Y: A from registers (64 rows x 64 k), Y a [64 k rows][64 d] tile read MN-major
+__device__ __forceinline__ void gemm_acc(float (&d)[32], const uint32_t (&a)[4][4], uint32_t y_addr) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) wgmma_rs_n64<1>(d, a[kk], gmma_desc_sw128(y_addr + kk * 2048, 8192, 1024), 1);
+}
+
+// 64 x 64 fragment (times `sc`) -> bf16 rows of [nseq][S][C] (rows >= S dropped)
+__device__ __forceinline__ void store_frag(const float (&d)[32], float sc, __nv_bfloat16* base, long long row0, int S,
+                                           int row_in_seq0, int C) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const int r = warp * 16 + (lane >> 2) + rr * 8;
+    if (row_in_seq0 + r >= S) continue;
+    __nv_bfloat16* dst = base + (row0 + r) * C + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16x2(d[4 * j + 2 * rr] * sc, d[4 * j + 2 * rr + 1] * sc);
+  }
+}
+
+__global__ void __launch_bounds__(kFaThreads)
+    og_flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                             const __grid_constant__ CUtensorMap mapV, const FaParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem;                   // 8 KiB
+  uint8_t* sKV = smem + kTileBytes;     // 2 stages x (K 8 KiB + V 8 KiB)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + 4 * kTileBytes);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;  // [2]
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  int id = blockIdx.x;
+  const int qt = id % p.q_tiles;
+  id /= p.q_tiles;
+  const int h = id % p.nh;
+  const int seq = id / p.nh;
+  const int q0 = qt * kTile;
+
+  if (tid == 0) {
+    tma_prefetch_desc(&mapQ);
+    tma_prefetch_desc(&mapK);
+    tma_prefetch_desc(&mapV);
+    mbar_init(q_full, 1);
+    mbar_init(&kv_full[0], 1);
+    mbar_init(&kv_full[1], 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    mbar_expect_tx(q_full, kTileBytes);
+    tma_load_3d(sQ, &mapQ, q_full, h * kD, q0, seq);
+    for (int j = 0; j < 2 && j < p.kv_tiles; ++j) {
+      mbar_expect_tx(&kv_full[j], 2 * kTileBytes);
+      tma_load_3d(sKV + j * 2 * kTileBytes, &mapK, &kv_full[j], h * kD, j * kTile, seq);
+      tma_load_3d(sKV + j * 2 * kTileBytes + kTileBytes, &mapV, &kv_full[j], h * kD, j * kTile, seq);
+    }
+  }
+  // Online softmax in base 2 with the scale folded in: p = 2^(s*c - m), c = scale*log2(e). l is a per-thread partial
+  // row sum (the quad's four partial sums are added once at the end).
+  const float cl2 = p.scale * 1.4426950408889634f;
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  const uint32_t q_addr = smem_u32(sQ);
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < p.kv_tiles; ++j) {
+    const int st = j & 1;
+    mbar_wait(&kv_full[st], (j >> 1) & 1);
+    const uint32_t k_addr = smem_u32(sKV + st * 2 * kTileBytes), v_addr = k_addr + kTileBytes;
+    float s[32];
+    wgmma_fence();
+    gemm_rows(s, q_addr, k_addr);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    const int kv_valid = p.S - j * kTile;  // keys of this tile that exist (>= 64 except for the last tile)
+    if (kv_valid < kTile) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if ((i >> 2) * 8 + 2 * (lane & 3) + (i & 1) >= kv_valid) s[i] = -INFINITY;
+    }
+    float alpha[2];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      float mt = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) mt = fmaxf(mt, fmaxf(s[4 * jj + 2 * rr], s[4 * jj + 2 * rr + 1]));
+      mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
+      mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+      const float mn = fmaxf(m[rr], mt * cl2);  // scale > 0; every tile has a valid key, so mn is finite
+      alpha[rr] = ex2_approx(m[rr] - mn);
+      m[rr] = mn;
+      float ls = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int i = 4 * jj + 2 * rr + e;
+          s[i] = ex2_approx(fmaf(s[i], cl2, -mn));
+          ls += s[i];
+        }
+      }
+      l[rr] = l[rr] * alpha[rr] + ls;
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+    uint32_t a[4][4];
+    frag_to_a(s, a);
+    wgmma_fence();
+    gemm_acc(o, a, v_addr);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    __syncthreads();  // every warp is done with stage st
+    if (tid == 0 && j + 2 < p.kv_tiles) {
+      mbar_expect_tx(&kv_full[st], 2 * kTileBytes);
+      tma_load_3d(sKV + st * 2 * kTileBytes, &mapK, &kv_full[st], h * kD, (j + 2) * kTile, seq);
+      tma_load_3d(sKV + st * 2 * kTileBytes + kTileBytes, &mapV, &kv_full[st], h * kD, (j + 2) * kTile, seq);
+    }
+  }
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    l[rr] += __shfl_xor_sync(0xffffffffu, l[rr], 1);
+    l[rr] += __shfl_xor_sync(0xffffffffu, l[rr], 2);
+  }
+  const float inv[2] = {1.f / l[0], 1.f / l[1]};
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] *= inv[(i >> 1) & 1];
+  const long long row0 = (long long)seq * p.S + q0;
+  store_frag(o, 1.f, p.out + h * kD, row0, p.S, q0, p.C);
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const int r = warp * 16 + (lane >> 2) + rr * 8;
+    if (q0 + r >= p.S) continue;
+    if (p.res) {  // second output: attention + residual, added in fp32 before the rounding
+      const long long off = (row0 + r) * p.C + h * kD + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.res + off + 8 * j));
+        *reinterpret_cast<uint32_t*>(p.out_res + off + 8 * j) =
+            pack_bf16x2(o[4 * j + 2 * rr] + t.x, o[4 * j + 2 * rr + 1] + t.y);
+      }
+    }
+    if (p.lse && (lane & 3) == 0)
+      p.lse[((long long)seq * p.nh + h) * p.S + q0 + r] = (m[rr] + __log2f(l[rr])) * 0.6931471805599453f;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// backward (see the file header). The softmax scale is applied once per output element of dK / dQ, not per score.
+// ------------------------------------------------------------------------------------------------
 template <int MODE>
-__global__ void __launch_bounds__(kFaBwdThreads, 1)
+__global__ void __launch_bounds__(kFaThreads)
     og_flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                              const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
                              const FaBwdParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sFix = smem;                    // stationary pair: MODE 0: K_j, V_j ; MODE 1: Q_i, dO_i   (2 x 16 KiB)
-  uint8_t* sStr = smem + 2 * kTileBytes;   // streamed pair, 2 stages x (2 x 16 KiB)
-  // P and dS are DOUBLE-buffered: the softmax warps write the tiles of step `it` while the gradient MMAs of step
-  // it-1 (issued after S_it / dP_it, i.e. not covered by sd_ready) are still reading theirs.
-  uint8_t* sP = sStr + 4 * kTileBytes;     // P  bf16 [2 buffers][2 k-blocks][128][128 B]
-  uint8_t* sDS = sP + 4 * kTileBytes;      // dS bf16, same shape
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sDS + 4 * kTileBytes);
+  uint8_t* sFix = smem;                    // stationary pair: MODE 0: K_j, V_j ; MODE 1: Q_i, dO_i   (2 x 8 KiB)
+  uint8_t* sStr = smem + 2 * kTileBytes;   // streamed pair, 2 stages x (2 x 8 KiB)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sStr + 4 * kTileBytes);
   uint64_t* fix_full = bars;
   uint64_t* str_full = bars + 1;   // [2]
-  uint64_t* str_empty = bars + 3;  // [2]
-  uint64_t* sd_ready = bars + 5;
-  uint64_t* p_ready = bars + 6;
-  uint64_t* acc_ready = bars + 7;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+  const CUtensorMap* mapF0 = MODE == 0 ? &mapK : &mapQ;
+  const CUtensorMap* mapF1 = MODE == 0 ? &mapV : &mapDO;
+  const CUtensorMap* mapS0 = MODE == 0 ? &mapQ : &mapK;
+  const CUtensorMap* mapS1 = MODE == 0 ? &mapDO : &mapV;
 
-  const int warp = warp_idx_uniform(), lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int id = blockIdx.x;
   const int own = id % p.tiles;  // MODE 0: kv tile ; MODE 1: q tile
   id /= p.tiles;
   const int h = id % p.nh;
   const int seq = id / p.nh;
+  const long long stat0 = ((long long)seq * p.nh + h) * p.S;   // lse / delta row of this (sequence, head)
 
-  if (warp == 0 && lane == 0) {
+  if (tid == 0) {
     tma_prefetch_desc(&mapQ);
     tma_prefetch_desc(&mapK);
     tma_prefetch_desc(&mapV);
     tma_prefetch_desc(&mapDO);
     mbar_init(fix_full, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&str_full[s], 1);
-      mbar_init(&str_empty[s], 1);
-    }
-    mbar_init(sd_ready, 1);
-    mbar_init(p_ready, 8);
-    mbar_init(acc_ready, 1);
+    mbar_init(&str_full[0], 1);
+    mbar_init(&str_full[1], 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base, tDP = tmem_base + 128, tAcc0 = tmem_base + 256, tAcc1 = tmem_base + 320;
-
-  if (warp == 0) {
-    {
-      if (elect_one()) {
-        mbar_expect_tx(fix_full, 2 * kTileBytes);
-        if (MODE == 0) {
-          tma_load_3d(sFix, &mapK, fix_full, h * kD, own * kTile, seq);
-          tma_load_3d(sFix + kTileBytes, &mapV, fix_full, h * kD, own * kTile, seq);
-        } else {
-          tma_load_3d(sFix, &mapQ, fix_full, h * kD, own * kTile, seq);
-          tma_load_3d(sFix + kTileBytes, &mapDO, fix_full, h * kD, own * kTile, seq);
-        }
-      }
-      __syncwarp();
-      for (int it = 0; it < p.tiles; ++it) {
-        const int st = it & 1;
-        mbar_wait(&str_empty[st], ((it >> 1) & 1) ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(&str_full[st], 2 * kTileBytes);
-          uint8_t* d = sStr + st * 2 * kTileBytes;
-          if (MODE == 0) {
-            tma_load_3d(d, &mapQ, &str_full[st], h * kD, it * kTile, seq);
-            tma_load_3d(d + kTileBytes, &mapDO, &str_full[st], h * kD, it * kTile, seq);
-          } else {
-            tma_load_3d(d, &mapK, &str_full[st], h * kD, it * kTile, seq);
-            tma_load_3d(d + kTileBytes, &mapV, &str_full[st], h * kD, it * kTile, seq);
-          }
-        }
-        __syncwarp();
-      }
+  if (tid == 0) {
+    mbar_expect_tx(fix_full, 2 * kTileBytes);
+    tma_load_3d(sFix, mapF0, fix_full, h * kD, own * kTile, seq);
+    tma_load_3d(sFix + kTileBytes, mapF1, fix_full, h * kD, own * kTile, seq);
+    for (int it = 0; it < 2 && it < p.tiles; ++it) {
+      mbar_expect_tx(&str_full[it], 2 * kTileBytes);
+      tma_load_3d(sStr + it * 2 * kTileBytes, mapS0, &str_full[it], h * kD, it * kTile, seq);
+      tma_load_3d(sStr + it * 2 * kTileBytes + kTileBytes, mapS1, &str_full[it], h * kD, it * kTile, seq);
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    {
-      const uint32_t idesc_kk = umma_idesc_bf16(128, 128, 0u, 0u);  // S, dP: both operands K-major
-      const uint32_t idesc_mm = umma_idesc_bf16(128, 64, 1u, 1u);   // dV, dK: A (P / dS transposed) and B MN-major
-      const uint32_t idesc_km = umma_idesc_bf16(128, 64, 0u, 1u);   // dQ: A = dS K-major, B = K MN-major
-      const uint32_t p_base = smem_u32(sP), ds_base = smem_u32(sDS);
-      mbar_wait(fix_full, 0);
-      for (int it = 0; it <= p.tiles; ++it) {
-        if (it < p.tiles) {
-          const int st = it & 1;
-          mbar_wait(&str_full[st], (it >> 1) & 1);
-          tc_fence_after();
-          if (it > 0) {
-            mbar_wait(p_ready, (it - 1) & 1);
-            tc_fence_after();
-          }
-          const uint32_t fixa = smem_u32(sFix), stra = smem_u32(sStr + st * 2 * kTileBytes);
-          const uint32_t q_addr = MODE == 0 ? stra : fixa, do_addr = q_addr + kTileBytes;
-          const uint32_t k_addr = MODE == 0 ? fixa : stra, v_addr = k_addr + kTileBytes;
-          if (elect_one()) {
+  }
+  const float cl2 = p.scale * 1.4426950408889634f;
+  const int r_base = warp * 16 + (lane >> 2);   // fragment rows r_base, r_base + 8
+  const int c_base = 2 * (lane & 3);            // fragment columns 8j + c_base + {0, 1}
+  // MODE 1: rows are queries of the own tile -> per-row lse / delta, loaded once
+  float lse_r[2] = {0.f, 0.f}, delta_r[2] = {0.f, 0.f};
+  if (MODE == 1) {
 #pragma unroll
-            for (int k = 0; k < kD / 16; ++k)
-              umma_bf16_ss(tS, umma_smem_desc_sw128(q_addr + k * 32, 16, 1024),
-                           umma_smem_desc_sw128(k_addr + k * 32, 16, 1024), idesc_kk, k > 0 ? 1u : 0u);
-#pragma unroll
-            for (int k = 0; k < kD / 16; ++k)
-              umma_bf16_ss(tDP, umma_smem_desc_sw128(do_addr + k * 32, 16, 1024),
-                           umma_smem_desc_sw128(v_addr + k * 32, 16, 1024), idesc_kk, k > 0 ? 1u : 0u);
-            umma_commit(sd_ready);
-          }
-          __syncwarp();
-        }
-        if (it > 0) {
-          const int jj = it - 1, st = jj & 1;
-          if (it == p.tiles) {
-            mbar_wait(p_ready, jj & 1);
-            tc_fence_after();
-          }
-          const uint32_t fixa = smem_u32(sFix), stra = smem_u32(sStr + st * 2 * kTileBytes);
-          const uint32_t p_addr = p_base + (jj & 1) * 2 * kTileBytes, ds_addr = ds_base + (jj & 1) * 2 * kTileBytes;
-          if (!elect_one()) {
-          } else if (MODE == 0) {
-            const uint32_t q_addr = stra, do_addr = stra + kTileBytes;
-#pragma unroll
-            for (int k = 0; k < kTile / 16; ++k) {  // K dim = 128 query rows, 16 per MMA
-              umma_bf16_ss(tAcc0, umma_smem_desc_sw128(p_addr + k * 2048, kTileBytes, 1024),
-                           umma_smem_desc_sw128(do_addr + k * 2048, 8192, 1024), idesc_mm, (jj > 0 || k > 0) ? 1u : 0u);
-              umma_bf16_ss(tAcc1, umma_smem_desc_sw128(ds_addr + k * 2048, kTileBytes, 1024),
-                           umma_smem_desc_sw128(q_addr + k * 2048, 8192, 1024), idesc_mm, (jj > 0 || k > 0) ? 1u : 0u);
-            }
-          } else {
-            const uint32_t k_addr = stra;
-#pragma unroll
-            for (int k = 0; k < kTile / 16; ++k)  // K dim = 128 keys
-              umma_bf16_ss(tAcc0, umma_smem_desc_sw128(ds_addr + (k >> 2) * kTileBytes + (k & 3) * 32, 16, 1024),
-                           umma_smem_desc_sw128(k_addr + k * 2048, 8192, 1024), idesc_km, (jj > 0 || k > 0) ? 1u : 0u);
-          }
-          __syncwarp();
-          if (elect_one()) umma_commit(&str_empty[st]);
-          __syncwarp();
-          (void)fixa;
-        }
-      }
-      if (elect_one()) umma_commit(acc_ready);
-    }
-    __syncwarp();
-  } else {
-    // 8 warps: warps w and w+4 share TMEM lane quarter (w & 3) and split the 128 columns of S / dP in halves.
-    // The backward softmax has no cross-column reduction (lse and delta are per-row inputs), so the split is free
-    // and doubles the warps per scheduler. p = 2^(s*c - lse*log2e); dS is written WITHOUT the softmax scale,
-    // which is applied once per output element to the dK / dQ accumulators instead of once per score.
-    const int qd = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int row = qd * 32 + lane;  // TMEM lane: query row of the current pair
-    const uint32_t lane_addr = (uint32_t)(qd * 32) << 16;
-    const float cl2 = p.scale * 1.4426950408889634f;
-    float lse_fix = 0.f, delta_fix = 0.f;
-    if (MODE == 1) {
-      const int qrow = own * kTile + row;
+    for (int rr = 0; rr < 2; ++rr) {
+      const int qrow = own * kTile + r_base + rr * 8;
       if (qrow < p.S) {
-        lse_fix = p.lse[((long long)seq * p.nh + h) * p.S + qrow] * 1.4426950408889634f;
-        delta_fix = p.delta[((long long)seq * p.nh + h) * p.S + qrow];
+        lse_r[rr] = p.lse[stat0 + qrow] * 1.4426950408889634f;
+        delta_r[rr] = p.delta[stat0 + qrow];
       }
     }
-    for (int it = 0; it < p.tiles; ++it) {
-      const int q_tile = MODE == 0 ? it : own, kv_tile = MODE == 0 ? own : it;
-      const int qrow = q_tile * kTile + row;
-      float lse2 = lse_fix, delta = delta_fix;
-      if (MODE == 0 && qrow < p.S) {
-        lse2 = p.lse[((long long)seq * p.nh + h) * p.S + qrow] * 1.4426950408889634f;
-        delta = p.delta[((long long)seq * p.nh + h) * p.S + qrow];
-      }
-      const bool q_ok = qrow < p.S;
-      const int kv_valid = p.S - kv_tile * kTile;
-      const bool full = (q_tile + 1) * kTile <= p.S && kv_valid >= kTile;  // warp-uniform fast path
-      mbar_wait(sd_ready, it & 1);
-      tc_fence_after();
+  }
+  float acc0[32], acc1[32];   // MODE 0: dV, dK ; MODE 1: dQ (acc1 unused)
 #pragma unroll
-      for (int cc = 0; cc < 64; cc += 32) {
-        const int c = half * 64 + cc;
-        uint32_t vs[32], vd[32];
-        tmem_ld_32x32(tS + lane_addr + c, vs);
-        tmem_ld_32x32(tDP + lane_addr + c, vd);
-        tmem_ld_wait();
-        float pf[32], df[32];
+  for (int i = 0; i < 32; ++i) acc0[i] = acc1[i] = 0.f;
+  const uint32_t f0 = smem_u32(sFix), f1 = f0 + kTileBytes;
+  mbar_wait(fix_full, 0);
+  for (int it = 0; it < p.tiles; ++it) {
+    const int st = it & 1;
+    mbar_wait(&str_full[st], (it >> 1) & 1);
+    const uint32_t s0 = smem_u32(sStr + st * 2 * kTileBytes), s1 = s0 + kTileBytes;
+    // MODE 0: s = S^T = K Q^T, dp = dP^T = V dO^T (rows = keys, columns = queries)
+    // MODE 1: s = S   = Q K^T, dp = dP   = dO V^T (rows = queries, columns = keys)
+    float s[32], dp[32];
+    wgmma_fence();
+    gemm_rows(s, f0, s0);
+    gemm_rows(dp, f1, s1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    reg_fence(dp);
+    const int row_tile = own, col_tile = it;
+    const bool rows_full = (row_tile + 1) * kTile <= p.S, cols_full = (col_tile + 1) * kTile <= p.S;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          float pv = ex2_approx(fmaf(__uint_as_float(vs[i]), cl2, -lse2));
-          if (!full) pv = (q_ok && (c + i < kv_valid)) ? pv : 0.f;
-          pf[i] = pv;
-          df[i] = pv * (__uint_as_float(vd[i]) - delta);
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = col_tile * kTile + 8 * j + c_base + e;
+        float lse2c = 0.f, deltac = 0.f;
+        if (MODE == 0 && col < p.S) {   // columns are queries
+          lse2c = p.lse[stat0 + col] * 1.4426950408889634f;
+          deltac = p.delta[stat0 + col];
         }
 #pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          const int col = c + i;
-          uint4 u;
-          if (MODE == 0) {
-            u.x = pack_bf16x2(pf[i], pf[i + 1]);
-            u.y = pack_bf16x2(pf[i + 2], pf[i + 3]);
-            u.z = pack_bf16x2(pf[i + 4], pf[i + 5]);
-            u.w = pack_bf16x2(pf[i + 6], pf[i + 7]);
-            st_swizzled_chunk(sP + ((it & 1) * 2 + (col >> 6)) * kTileBytes, row, (col & 63) >> 3, u);
+        for (int rr = 0; rr < 2; ++rr) {
+          const int i = 4 * j + 2 * rr + e;
+          const float lse2 = MODE == 0 ? lse2c : lse_r[rr], dl = MODE == 0 ? deltac : delta_r[rr];
+          float pv = ex2_approx(fmaf(s[i], cl2, -lse2));
+          if (!(rows_full && cols_full)) {
+            const int row = row_tile * kTile + r_base + rr * 8;
+            if (row >= p.S || col >= p.S) pv = 0.f;
           }
-          u.x = pack_bf16x2(df[i], df[i + 1]);
-          u.y = pack_bf16x2(df[i + 2], df[i + 3]);
-          u.z = pack_bf16x2(df[i + 4], df[i + 5]);
-          u.w = pack_bf16x2(df[i + 6], df[i + 7]);
-          st_swizzled_chunk(sDS + ((it & 1) * 2 + (col >> 6)) * kTileBytes, row, (col & 63) >> 3, u);
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_ready);
-    }
-    // accumulators complete: TMEM lane = output row (kv row in MODE 0, query row in MODE 1); the two warps of a
-    // lane quarter take 32 of the 64 columns each. dK / dQ carry the softmax scale here.
-    mbar_wait_relaxed(acc_ready, 0);
-    tc_fence_after();
-    const int orow = own * kTile + row;
-    for (int a = 0; a < (MODE == 0 ? 2 : 1); ++a) {
-      __nv_bfloat16* base = MODE == 1 ? p.dq : (a == 0 ? p.dv : p.dk);
-      const uint32_t tacc = a == 0 ? tAcc0 : tAcc1;
-      const float osc = (MODE == 0 && a == 0) ? 1.f : p.scale;
-      const int c = half * 32;
-      uint32_t v[32];
-      tmem_ld_32x32(tacc + lane_addr + c, v);
-      tmem_ld_wait();
-      if (orow < p.S) {
-        __nv_bfloat16* dst = base + ((long long)seq * p.S + orow) * p.C + h * kD + c;
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          uint4 u;
-          u.x = pack_bf16x2(__uint_as_float(v[i]) * osc, __uint_as_float(v[i + 1]) * osc);
-          u.y = pack_bf16x2(__uint_as_float(v[i + 2]) * osc, __uint_as_float(v[i + 3]) * osc);
-          u.z = pack_bf16x2(__uint_as_float(v[i + 4]) * osc, __uint_as_float(v[i + 5]) * osc);
-          u.w = pack_bf16x2(__uint_as_float(v[i + 6]) * osc, __uint_as_float(v[i + 7]) * osc);
-          *reinterpret_cast<uint4*>(dst + i) = u;
+          s[i] = pv;
+          dp[i] = pv * (dp[i] - dl);
         }
       }
     }
-    tc_fence_before();
+    uint32_t a_p[4][4], a_ds[4][4];
+    frag_to_a(dp, a_ds);
+    wgmma_fence();
+    if (MODE == 0) {
+      frag_to_a(s, a_p);
+      gemm_acc(acc0, a_p, s1);    // dV_j += P^T dO_i
+      gemm_acc(acc1, a_ds, s0);   // dK_j += dS^T Q_i
+    } else {
+      gemm_acc(acc0, a_ds, s0);   // dQ_i += dS K_j
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(acc0);
+    reg_fence(acc1);
+    __syncthreads();  // every warp is done with stage st
+    if (tid == 0 && it + 2 < p.tiles) {
+      mbar_expect_tx(&str_full[st], 2 * kTileBytes);
+      tma_load_3d(sStr + st * 2 * kTileBytes, mapS0, &str_full[st], h * kD, (it + 2) * kTile, seq);
+      tma_load_3d(sStr + st * 2 * kTileBytes + kTileBytes, mapS1, &str_full[st], h * kD, (it + 2) * kTile, seq);
+    }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// backward, software-pipelined (round 2). Same two passes and the same math as og_flash_attn_bwd_kernel above, but the
-// S accumulator is DOUBLE-buffered in TMEM (S0 | S1 | dP | acc = 128+128+128+128 columns) and the softmax is split in
-// two phases so that the tensor pipe never waits for a whole softmax and the softmax warps never wait for a whole
-// S/dP pair:
-//   phase A(it): P = 2^(S*c - lse) from S(it)              needs S(it)  — issued one iteration EARLY
-//   phase B(it): dS = P * (dP - delta) from dP(it)          needs dP(it) — issued when phase B(it-1) has read dP(it-1)
-// MMA issue order per iteration:  dP(it) | dV,dK / dQ of it-1 | S(it+1).
-// In the first version the order was S,dP(it) -> softmax(it) -> S,dP(it+1): the softmax warps idled while S/dP ran
-// (~700 clk of a ~3400 clk iteration) and the MMAs idled during the softmax.
-// MODE 1 has no P tile in shared memory and uses the room for four K/V stages instead of two.
-// ------------------------------------------------------------------------------------------------
-template <int MODE, int NW>   // NW softmax warps (8 or 16): 4 TMEM lane quarters x NW/4 column groups of 512/NW columns
-__global__ void __launch_bounds__(64 + 32 * NW, 1)
-    og_flash_attn_bwd2_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                              const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
-                              const FaBwdParams p) {
-  constexpr int kStages = MODE == 0 ? 2 : 4;
-  constexpr int CW = 512 / NW;  // columns of S / dP per softmax warp
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sFix = smem;                    // stationary pair: MODE 0: K_j, V_j ; MODE 1: Q_i, dO_i   (2 x 16 KiB)
-  uint8_t* sStr = smem + 2 * kTileBytes;   // streamed pair, kStages x (2 x 16 KiB)   (MODE 1: covers the unused P region)
-  uint8_t* sP = smem + 6 * kTileBytes;     // P  bf16 [2 buffers][2 k-blocks][128][128 B]   (MODE 0 only)
-  uint8_t* sDS = smem + 10 * kTileBytes;   // dS bf16, same shape
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 14 * kTileBytes);
-  uint64_t* fix_full = bars;
-  uint64_t* str_full = bars + 1;   // [4]
-  uint64_t* str_empty = bars + 5;  // [4]
-  uint64_t* s_full = bars + 9;     // [2]
-  uint64_t* dp_full = bars + 11;
-  uint64_t* dp_free = bars + 12;
-  uint64_t* p_ready = bars + 13;
-  uint64_t* acc_ready = bars + 14;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 15);
-
-  const int warp = warp_idx_uniform(), lane = threadIdx.x & 31;
-  int id = blockIdx.x;
-  const int own = id % p.tiles;  // MODE 0: kv tile ; MODE 1: q tile
-  id /= p.tiles;
-  const int h = id % p.nh;
-  const int seq = id / p.nh;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&mapQ);
-    tma_prefetch_desc(&mapK);
-    tma_prefetch_desc(&mapV);
-    tma_prefetch_desc(&mapDO);
-    mbar_init(fix_full, 1);
-    for (int s = 0; s < 4; ++s) {
-      mbar_init(&str_full[s], 1);
-      mbar_init(&str_empty[s], 1);
-    }
-    mbar_init(&s_full[0], 1);
-    mbar_init(&s_full[1], 1);
-    mbar_init(dp_full, 1);
-    mbar_init(dp_free, NW);
-    mbar_init(p_ready, NW);
-    mbar_init(acc_ready, 1);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS0 = tmem_base, tDP = tmem_base + 256, tAcc0 = tmem_base + 384, tAcc1 = tmem_base + 448;
-
-  if (warp == 0) {
-    if (elect_one()) {
-      mbar_expect_tx(fix_full, 2 * kTileBytes);
-      if (MODE == 0) {
-        tma_load_3d(sFix, &mapK, fix_full, h * kD, own * kTile, seq);
-        tma_load_3d(sFix + kTileBytes, &mapV, fix_full, h * kD, own * kTile, seq);
-      } else {
-        tma_load_3d(sFix, &mapQ, fix_full, h * kD, own * kTile, seq);
-        tma_load_3d(sFix + kTileBytes, &mapDO, fix_full, h * kD, own * kTile, seq);
-      }
-    }
-    __syncwarp();
-    int st = 0;
-    uint32_t ph = 1;   // the first pass over the ring finds every slot free
-    for (int it = 0; it < p.tiles; ++it) {
-      mbar_wait(&str_empty[st], ph);
-      if (p.dbg & 64) {
-        if (elect_one()) mbar_arrive(&str_full[st]);
-      } else if (elect_one()) {
-        mbar_expect_tx(&str_full[st], 2 * kTileBytes);
-        uint8_t* d = sStr + st * 2 * kTileBytes;
-        if (MODE == 0) {
-          tma_load_3d(d, &mapQ, &str_full[st], h * kD, it * kTile, seq);
-          tma_load_3d(d + kTileBytes, &mapDO, &str_full[st], h * kD, it * kTile, seq);
-        } else {
-          tma_load_3d(d, &mapK, &str_full[st], h * kD, it * kTile, seq);
-          tma_load_3d(d + kTileBytes, &mapV, &str_full[st], h * kD, it * kTile, seq);
-        }
-      }
-      __syncwarp();
-      if (++st == kStages) {
-        st = 0;
-        ph ^= 1;
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    const uint32_t idesc_kk = umma_idesc_bf16(128, 128, 0u, 0u);  // S, dP: both operands K-major
-    const uint32_t idesc_mm = umma_idesc_bf16(128, 64, 1u, 1u);   // dV, dK: A (P / dS transposed) and B MN-major
-    const uint32_t idesc_km = umma_idesc_bf16(128, 64, 0u, 1u);   // dQ: A = dS K-major, B = K MN-major
-    const uint32_t p_base = smem_u32(sP), ds_base = smem_u32(sDS);
-    const uint32_t fixa = smem_u32(sFix), str0 = smem_u32(sStr);
-    mbar_wait(fix_full, 0);
-    // ring position of tile `it` (st_cur) and of tile it+1 (st_nxt); parities of their `full` barriers
-    int st_prev = 0, st_cur = 0, st_nxt = kStages > 1 ? 1 : 0;
-    uint32_t ph_nxt = 0;
-    {  // S(0)
-      mbar_wait(&str_full[0], 0);
-      tc_fence_after();
-      const uint32_t q_addr = MODE == 0 ? str0 : fixa, k_addr = MODE == 0 ? fixa : str0;
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < kD / 16; ++k)
-          umma_bf16_ss(tS0, umma_smem_desc_sw128(q_addr + k * 32, 16, 1024),
-                       umma_smem_desc_sw128(k_addr + k * 32, 16, 1024), idesc_kk, k > 0 ? 1u : 0u);
-        umma_commit(&s_full[0]);
-      }
-      __syncwarp();
-    }
-    for (int it = 0; it <= p.tiles; ++it) {
-      if (it < p.tiles) {  // dP(it): the slot of tile `it` is loaded (S(it) waited for it)
-        if (it > 0) {
-          mbar_wait(dp_free, (it - 1) & 1);
-          tc_fence_after();
-        }
-        const uint32_t stra = str0 + st_cur * 2 * kTileBytes;
-        const uint32_t do_addr = (MODE == 0 ? stra : fixa) + kTileBytes, v_addr = (MODE == 0 ? fixa : stra) + kTileBytes;
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < ((p.dbg & 8) ? 0 : kD / 16); ++k)
-            umma_bf16_ss(tDP, umma_smem_desc_sw128(do_addr + k * 32, 16, 1024),
-                         umma_smem_desc_sw128(v_addr + k * 32, 16, 1024), idesc_kk, k > 0 ? 1u : 0u);
-          umma_commit(dp_full);
-        }
-        __syncwarp();
-      }
-      if (it > 0) {  // gradient MMAs of tile it-1 (P / dS buffer (it-1) & 1, stream slot st_prev)
-        const int jj = it - 1;
-        mbar_wait(p_ready, jj & 1);
-        tc_fence_after();
-        const uint32_t stra = str0 + st_prev * 2 * kTileBytes;
-        const uint32_t p_addr = p_base + (jj & 1) * 2 * kTileBytes, ds_addr = ds_base + (jj & 1) * 2 * kTileBytes;
-        if (!elect_one() || (p.dbg & 4)) {
-        } else if (MODE == 0) {
-          const uint32_t q_addr = stra, do_addr = stra + kTileBytes;
-#pragma unroll
-          for (int k = 0; k < kTile / 16; ++k) {  // K dim = 128 query rows, 16 per MMA
-            umma_bf16_ss(tAcc0, umma_smem_desc_sw128(p_addr + k * 2048, kTileBytes, 1024),
-                         umma_smem_desc_sw128(do_addr + k * 2048, 8192, 1024), idesc_mm, (jj > 0 || k > 0) ? 1u : 0u);
-            umma_bf16_ss(tAcc1, umma_smem_desc_sw128(ds_addr + k * 2048, kTileBytes, 1024),
-                         umma_smem_desc_sw128(q_addr + k * 2048, 8192, 1024), idesc_mm, (jj > 0 || k > 0) ? 1u : 0u);
-          }
-        } else {
-          const uint32_t k_addr = stra;
-#pragma unroll
-          for (int k = 0; k < kTile / 16; ++k)  // K dim = 128 keys
-            umma_bf16_ss(tAcc0, umma_smem_desc_sw128(ds_addr + (k >> 2) * kTileBytes + (k & 3) * 32, 16, 1024),
-                         umma_smem_desc_sw128(k_addr + k * 2048, 8192, 1024), idesc_km, (jj > 0 || k > 0) ? 1u : 0u);
-        }
-        __syncwarp();
-        if (elect_one()) umma_commit(&str_empty[st_prev]);
-        __syncwarp();
-      }
-      if (it + 1 < p.tiles) {  // S(it+1) into the S buffer phase A(it-1) has finished with (implied by p_ready(it-1))
-        mbar_wait(&str_full[st_nxt], ph_nxt);
-        tc_fence_after();
-        const uint32_t stra = str0 + st_nxt * 2 * kTileBytes;
-        const uint32_t q_addr = MODE == 0 ? stra : fixa, k_addr = MODE == 0 ? fixa : stra;
-        const uint32_t tS = tS0 + (((it + 1) & 1) ? 128u : 0u);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < ((p.dbg & 8) ? 0 : kD / 16); ++k)
-            umma_bf16_ss(tS, umma_smem_desc_sw128(q_addr + k * 32, 16, 1024),
-                         umma_smem_desc_sw128(k_addr + k * 32, 16, 1024), idesc_kk, k > 0 ? 1u : 0u);
-          umma_commit(&s_full[(it + 1) & 1]);
-        }
-        __syncwarp();
-      }
-      st_prev = st_cur;
-      st_cur = st_nxt;
-      if (++st_nxt == kStages) {
-        st_nxt = 0;
-        ph_nxt ^= 1;
-      }
-    }
-    if (elect_one()) umma_commit(acc_ready);
-    __syncwarp();
+  const long long row0 = (long long)seq * p.S + own * kTile;
+  if (MODE == 0) {
+    store_frag(acc0, 1.f, p.dv + h * kD, row0, p.S, own * kTile, p.C);
+    store_frag(acc1, p.scale, p.dk + h * kD, row0, p.S, own * kTile, p.C);
   } else {
-    // NW warps: warp w works on TMEM lane quarter (w & 3) (a hardware rule) and on column group (w - 2) / 4 of S / dP.
-    // The backward softmax has no cross-column reduction (lse and delta are per-row inputs), so the split is free.
-    // With 8 warps (2 per scheduler) the issue slots were 35-40 % busy: each warp stalls on MUFU / TMEM-load / fixed
-    // latencies with nothing else to issue; 16 warps hide them.
-    const int qd = warp & 3;
-    const int cg = (warp - 2) >> 2;
-    const int c0 = cg * CW;
-    const int row = qd * 32 + lane;  // TMEM lane: query row of the current pair
-    const uint32_t lane_addr = (uint32_t)(qd * 32) << 16;
-    const float cl2 = p.scale * 1.4426950408889634f;
-    float lse_fix = 0.f, delta_fix = 0.f;
-    if (MODE == 1) {
-      const int qrow = own * kTile + row;
-      if (qrow < p.S) {
-        lse_fix = p.lse[((long long)seq * p.nh + h) * p.S + qrow] * 1.4426950408889634f;
-        delta_fix = p.delta[((long long)seq * p.nh + h) * p.S + qrow];
-      }
-    }
-    // MODE 0 streams the query tiles: the per-row lse / delta of tile it+1 are fetched while tile it is processed
-    // (as dependent loads at the top of the iteration they were 12 % of the softmax warps' time)
-    const float* lse_row = p.lse + ((long long)seq * p.nh + h) * p.S;
-    const float* delta_row = p.delta + ((long long)seq * p.nh + h) * p.S;
-    float lse_nxt = 0.f, delta_nxt = 0.f;
-    if (MODE == 0 && row < p.S) {
-      lse_nxt = __ldg(lse_row + row);
-      delta_nxt = __ldg(delta_row + row);
-    }
-    for (int it = 0; it < p.tiles; ++it) {
-      const int q_tile = MODE == 0 ? it : own, kv_tile = MODE == 0 ? own : it;
-      const int qrow = q_tile * kTile + row;
-      float lse2 = lse_fix, delta = delta_fix;
-      if (MODE == 0) {
-        lse2 = lse_nxt * 1.4426950408889634f;
-        delta = delta_nxt;
-        if (qrow + kTile < p.S) {
-          lse_nxt = __ldg(lse_row + qrow + kTile);
-          delta_nxt = __ldg(delta_row + qrow + kTile);
-        }
-      }
-      const bool q_ok = qrow < p.S;
-      const int kv_valid = p.S - kv_tile * kTile;
-      const bool full = (q_tile + 1) * kTile <= p.S && kv_valid >= kTile;  // warp-uniform fast path
-      const uint32_t tS = tS0 + ((it & 1) ? 128u : 0u);
-      float pf[CW];
-      // ---- phase A: probabilities from S(it)
-      mbar_wait(&s_full[it & 1], (it >> 1) & 1);
-      tc_fence_after();
-      if (p.dbg & 32) {  // barrier protocol only
-        mbar_wait(dp_full, it & 1);
-        tc_fence_after();
-        if (!(p.dbg & 16)) {
-          uint32_t vs[32];
-          tmem_ld_32x32(tS + lane_addr + c0, vs);
-          tmem_ld_32x32(tDP + lane_addr + c0, vs);
-          tmem_ld_32x32(tS + lane_addr + c0 + 32, vs);
-          tmem_ld_32x32(tDP + lane_addr + c0 + 32, vs);
-          tmem_ld_wait();
-          if (vs[0] == 0x12345678u) pf[0] = 1.f;
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(dp_free);
-        fence_proxy_async_smem();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(p_ready);
-        continue;
-      }
-      if (NW == 8 && full && p.interleave) {
-        // two 32-column chunks per warp: exps(chunk 0) | exps(chunk 1) interleaved with the dS (and P) work of chunk 0 |
-        // dS (and P) of chunk 1. Every 8 MUFU.EX2 are followed by the ~30 FMA / ALU / store instructions of 8 finished
-        // elements, which issue while the XU pipe works its queue off.
-        uint32_t vs[32], vd[32];
-        tmem_ld_32x32(tS + lane_addr + c0, vs);
-        tmem_ld_wait();
-        if (p.dbg & 1) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) pf[i] = fmaf(__uint_as_float(vs[i]), cl2, -lse2);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) pf[i] = ex2_approx(fmaf(__uint_as_float(vs[i]), cl2, -lse2));
-        }
-        mbar_wait(dp_full, it & 1);
-        tc_fence_after();
-        tmem_ld_32x32(tDP + lane_addr + c0, vd);
-        tmem_ld_32x32(tS + lane_addr + c0 + 32, vs);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const float x = fmaf(__uint_as_float(vs[i + e]), cl2, -lse2);
-            pf[32 + i + e] = (p.dbg & 1) ? x : ex2_ordered(x);
-          }
-          const int col = c0 + i;
-          uint4 u;
-          if (MODE == 0) {
-            u.x = pack_bf16x2(pf[i], pf[i + 1]);
-            u.y = pack_bf16x2(pf[i + 2], pf[i + 3]);
-            u.z = pack_bf16x2(pf[i + 4], pf[i + 5]);
-            u.w = pack_bf16x2(pf[i + 6], pf[i + 7]);
-            if (!(p.dbg & 2)) st_swizzled_chunk_ordered(sP + ((it & 1) * 2 + (col >> 6)) * kTileBytes, row, (col & 63) >> 3, u);
-          }
-          float df[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) df[e] = pf[i + e] * (__uint_as_float(vd[i + e]) - delta);
-          u.x = pack_bf16x2(df[0], df[1]);
-          u.y = pack_bf16x2(df[2], df[3]);
-          u.z = pack_bf16x2(df[4], df[5]);
-          u.w = pack_bf16x2(df[6], df[7]);
-          if (!(p.dbg & 2)) st_swizzled_chunk_ordered(sDS + ((it & 1) * 2 + (col >> 6)) * kTileBytes, row, (col & 63) >> 3, u);
-        }
-        tmem_ld_32x32(tDP + lane_addr + c0 + 32, vd);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(dp_free);
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          const int col = c0 + 32 + i;
-          uint4 u;
-          if (MODE == 0) {
-            u.x = pack_bf16x2(pf[32 + i], pf[32 + i + 1]);
-            u.y = pack_bf16x2(pf[32 + i + 2], pf[32 + i + 3]);
-            u.z = pack_bf16x2(pf[32 + i + 4], pf[32 + i + 5]);
-            u.w = pack_bf16x2(pf[32 + i + 6], pf[32 + i + 7]);
-            st_swizzled_chunk(sP + ((it & 1) * 2 + (col >> 6)) * kTileBytes, row, (col & 63) >> 3, u);
-          }
-          float df[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) df[e] = pf[32 + i + e] * (__uint_as_float(vd[i + e]) - delta);
-          u.x = pack_bf16x2(df[0], df[1]);
-          u.y = pack_bf16x2(df[2], df[3]);
-          u.z = pack_bf16x2(df[4], df[5]);
-          u.w = pack_bf16x2(df[6], df[7]);
-          st_swizzled_chunk(sDS + ((it & 1) * 2 + (col >> 6)) * kTileBytes, row, (col & 63) >> 3, u);
-        }
-        fence_proxy_async_smem();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(p_ready);
-        continue;
-      }
-#pragma unroll
-      for (int cc = 0; cc < CW; cc += 32) {
-        const int c = c0 + cc;
-        uint32_t vs[32];
-        tmem_ld_32x32(tS + lane_addr + c, vs);
-        tmem_ld_wait();
-        if (full) {  // whole tiles: no per-element select / compare (they were a quarter of the issued instructions)
-#pragma unroll
-          for (int i = 0; i < 32; ++i) pf[cc + i] = ex2_approx(fmaf(__uint_as_float(vs[i]), cl2, -lse2));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float pv = ex2_approx(fmaf(__uint_as_float(vs[i]), cl2, -lse2));
-            pf[cc + i] = (q_ok && (c + i < kv_valid)) ? pv : 0.f;
-          }
-        }
-        if (MODE == 0) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 8) {
-            const int col = c + i;
-            uint4 u;
-            u.x = pack_bf16x2(pf[cc + i], pf[cc + i + 1]);
-            u.y = pack_bf16x2(pf[cc + i + 2], pf[cc + i + 3]);
-            u.z = pack_bf16x2(pf[cc + i + 4], pf[cc + i + 5]);
-            u.w = pack_bf16x2(pf[cc + i + 6], pf[cc + i + 7]);
-            st_swizzled_chunk(sP + ((it & 1) * 2 + (col >> 6)) * kTileBytes, row, (col & 63) >> 3, u);
-          }
-        }
-      }
-      // ---- phase B: dS from dP(it); the dP accumulator is handed back as soon as it sits in registers
-      mbar_wait(dp_full, it & 1);
-      tc_fence_after();
-      uint32_t vd[CW / 32][32];
-#pragma unroll
-      for (int g = 0; g < CW / 32; ++g) tmem_ld_32x32(tDP + lane_addr + c0 + g * 32, vd[g]);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(dp_free);
-#pragma unroll
-      for (int cc = 0; cc < CW; cc += 32) {
-        const int c = c0 + cc;
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          const int col = c + i;
-          float df[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) df[e] = pf[cc + i + e] * (__uint_as_float(vd[cc / 32][i + e]) - delta);
-          uint4 u;
-          u.x = pack_bf16x2(df[0], df[1]);
-          u.y = pack_bf16x2(df[2], df[3]);
-          u.z = pack_bf16x2(df[4], df[5]);
-          u.w = pack_bf16x2(df[6], df[7]);
-          st_swizzled_chunk(sDS + ((it & 1) * 2 + (col >> 6)) * kTileBytes, row, (col & 63) >> 3, u);
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_ready);
-    }
-    // accumulators complete: TMEM lane = output row (kv row in MODE 0, query row in MODE 1); two warps of a lane
-    // quarter take 32 of the 64 columns each. dK / dQ carry the softmax scale here.
-    mbar_wait_relaxed(acc_ready, 0);
-    tc_fence_after();
-    const int orow = own * kTile + row;
-    const int half = cg;
-    for (int a = 0; a < (cg >= 2 ? 0 : (MODE == 0 ? 2 : 1)); ++a) {
-      __nv_bfloat16* base = MODE == 1 ? p.dq : (a == 0 ? p.dv : p.dk);
-      const uint32_t tacc = a == 0 ? tAcc0 : tAcc1;
-      const float osc = (MODE == 0 && a == 0) ? 1.f : p.scale;
-      const int c = half * 32;
-      uint32_t v[32];
-      tmem_ld_32x32(tacc + lane_addr + c, v);
-      tmem_ld_wait();
-      if (orow < p.S) {
-        __nv_bfloat16* dst = base + ((long long)seq * p.S + orow) * p.C + h * kD + c;
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          uint4 u;
-          u.x = pack_bf16x2(__uint_as_float(v[i]) * osc, __uint_as_float(v[i + 1]) * osc);
-          u.y = pack_bf16x2(__uint_as_float(v[i + 2]) * osc, __uint_as_float(v[i + 3]) * osc);
-          u.z = pack_bf16x2(__uint_as_float(v[i + 4]) * osc, __uint_as_float(v[i + 5]) * osc);
-          u.w = pack_bf16x2(__uint_as_float(v[i + 6]) * osc, __uint_as_float(v[i + 7]) * osc);
-          *reinterpret_cast<uint4*>(dst + i) = u;
-        }
-      }
-    }
-    tc_fence_before();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// backward, persistent form of og_flash_attn_bwd2_kernel (8 softmax warps): one CTA per SM walks the work items
-// (frame, head, own tile) w = blockIdx.x, blockIdx.x + gridDim.x, ... with the same pipeline, but TMEM, the barriers and
-// the tensor maps are set up ONCE, and the next item's stationary / first streamed tiles are loaded (and its S(0), dP(0)
-// issued) while the softmax warps still store the current item's accumulators. All barrier parities derive from running
-// counters: T = global index of the streamed tile (slot T % kStages, S buffer T & 1), wi = index of the work item.
-// Measured motivation (profiles/r02u_ncu_flash_attention_bwd.md): ~6 us of fixed cost per CTA, 12 % of the backward at
-// S = 4096 and 75 % at S = 256.
-// ------------------------------------------------------------------------------------------------
-template <int MODE>
-__global__ void __launch_bounds__(kFaBwdThreads, 1)
-    og_flash_attn_bwd3_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                              const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
-                              const FaBwdParams p, const int total_items) {
-  constexpr int kStages = MODE == 0 ? 2 : 4;   // power of two
-  constexpr int NW = 8;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sFix = smem;                    // stationary pair: MODE 0: K_j, V_j ; MODE 1: Q_i, dO_i   (2 x 16 KiB)
-  uint8_t* sStr = smem + 2 * kTileBytes;   // streamed pair, kStages x (2 x 16 KiB)   (MODE 1: covers the unused P region)
-  uint8_t* sP = smem + 6 * kTileBytes;     // P  bf16 [2 buffers][2 k-blocks][128][128 B]   (MODE 0 only)
-  uint8_t* sDS = smem + 10 * kTileBytes;   // dS bf16, same shape
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 14 * kTileBytes);
-  uint64_t* fix_full = bars;
-  uint64_t* fix_empty = bars + 1;
-  uint64_t* str_full = bars + 2;   // [4]
-  uint64_t* str_empty = bars + 6;  // [4]
-  uint64_t* s_full = bars + 10;    // [2]
-  uint64_t* dp_full = bars + 12;
-  uint64_t* dp_free = bars + 13;
-  uint64_t* p_ready = bars + 14;
-  uint64_t* acc_ready = bars + 15;
-  uint64_t* acc_free = bars + 16;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 17);
-
-  const int warp = warp_idx_uniform(), lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&mapQ);
-    tma_prefetch_desc(&mapK);
-    tma_prefetch_desc(&mapV);
-    tma_prefetch_desc(&mapDO);
-    mbar_init(fix_full, 1);
-    mbar_init(fix_empty, 1);
-    for (int s = 0; s < 4; ++s) {
-      mbar_init(&str_full[s], 1);
-      mbar_init(&str_empty[s], 1);
-    }
-    mbar_init(&s_full[0], 1);
-    mbar_init(&s_full[1], 1);
-    mbar_init(dp_full, 1);
-    mbar_init(dp_free, NW);
-    mbar_init(p_ready, NW);
-    mbar_init(acc_ready, 1);
-    mbar_init(acc_free, NW);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS0 = tmem_base, tDP = tmem_base + 256, tAcc0 = tmem_base + 384, tAcc1 = tmem_base + 448;
-  const int tiles = p.tiles;
-
-  if (warp == 0) {
-    // ------------------------------------------------ TMA producer
-    int T = 0, wi = 0;
-    for (int w = blockIdx.x; w < total_items; w += gridDim.x, ++wi) {
-      int id = w;
-      const int own = id % tiles;
-      id /= tiles;
-      const int h = id % p.nh, seq = id / p.nh;
-      mbar_wait(fix_empty, (wi & 1) ^ 1);   // the previous item's last S / dP MMAs have read the stationary tiles
-      if (elect_one()) {
-        mbar_expect_tx(fix_full, 2 * kTileBytes);
-        if (MODE == 0) {
-          tma_load_3d(sFix, &mapK, fix_full, h * kD, own * kTile, seq);
-          tma_load_3d(sFix + kTileBytes, &mapV, fix_full, h * kD, own * kTile, seq);
-        } else {
-          tma_load_3d(sFix, &mapQ, fix_full, h * kD, own * kTile, seq);
-          tma_load_3d(sFix + kTileBytes, &mapDO, fix_full, h * kD, own * kTile, seq);
-        }
-      }
-      __syncwarp();
-      for (int it = 0; it < tiles; ++it, ++T) {
-        const int st = T & (kStages - 1);
-        mbar_wait(&str_empty[st], ((T / kStages) & 1) ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(&str_full[st], 2 * kTileBytes);
-          uint8_t* d = sStr + st * 2 * kTileBytes;
-          if (MODE == 0) {
-            tma_load_3d(d, &mapQ, &str_full[st], h * kD, it * kTile, seq);
-            tma_load_3d(d + kTileBytes, &mapDO, &str_full[st], h * kD, it * kTile, seq);
-          } else {
-            tma_load_3d(d, &mapK, &str_full[st], h * kD, it * kTile, seq);
-            tma_load_3d(d + kTileBytes, &mapV, &str_full[st], h * kD, it * kTile, seq);
-          }
-        }
-        __syncwarp();
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ------------------------------------------------ MMA issuer
-    const uint32_t idesc_kk = umma_idesc_bf16(128, 128, 0u, 0u);  // S, dP: both operands K-major
-    const uint32_t idesc_mm = umma_idesc_bf16(128, 64, 1u, 1u);   // dV, dK: A (P / dS transposed) and B MN-major
-    const uint32_t idesc_km = umma_idesc_bf16(128, 64, 0u, 1u);   // dQ: A = dS K-major, B = K MN-major
-    const uint32_t p_base = smem_u32(sP), ds_base = smem_u32(sDS);
-    const uint32_t fixa = smem_u32(sFix), str0 = smem_u32(sStr);
-    int T0 = 0, wi = 0;
-    for (int w = blockIdx.x; w < total_items; w += gridDim.x, ++wi, T0 += tiles) {
-      mbar_wait(fix_full, wi & 1);
-      tc_fence_after();
-      {  // S(0) of this item
-        const int st = T0 & (kStages - 1);
-        mbar_wait(&str_full[st], (T0 / kStages) & 1);
-        tc_fence_after();
-        const uint32_t stra = str0 + st * 2 * kTileBytes;
-        const uint32_t q_addr = MODE == 0 ? stra : fixa, k_addr = MODE == 0 ? fixa : stra;
-        const uint32_t tS = tS0 + ((T0 & 1) ? 128u : 0u);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < kD / 16; ++k)
-            umma_bf16_ss(tS, umma_smem_desc_sw128(q_addr + k * 32, 16, 1024),
-                         umma_smem_desc_sw128(k_addr + k * 32, 16, 1024), idesc_kk, k > 0 ? 1u : 0u);
-          umma_commit(&s_full[T0 & 1]);
-        }
-        __syncwarp();
-      }
-      for (int it = 0; it <= tiles; ++it) {
-        const int T = T0 + it;
-        if (it < tiles) {  // dP(it)
-          if (T > 0) {
-            mbar_wait(dp_free, (T - 1) & 1);
-            tc_fence_after();
-          }
-          const uint32_t stra = str0 + (T & (kStages - 1)) * 2 * kTileBytes;
-          const uint32_t do_addr = (MODE == 0 ? stra : fixa) + kTileBytes, v_addr = (MODE == 0 ? fixa : stra) + kTileBytes;
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < kD / 16; ++k)
-              umma_bf16_ss(tDP, umma_smem_desc_sw128(do_addr + k * 32, 16, 1024),
-                           umma_smem_desc_sw128(v_addr + k * 32, 16, 1024), idesc_kk, k > 0 ? 1u : 0u);
-            umma_commit(dp_full);
-            if (it == tiles - 1) umma_commit(fix_empty);   // every S / dP of this item has been issued
-          }
-          __syncwarp();
-        }
-        if (it > 0) {  // gradient MMAs of tile it-1
-          const int jj = it - 1, Tj = T - 1;
-          mbar_wait(p_ready, Tj & 1);
-          tc_fence_after();
-          if (jj == 0 && wi > 0) {   // they overwrite the accumulators: the previous item's must be in registers
-            mbar_wait(acc_free, (wi - 1) & 1);
-            tc_fence_after();
-          }
-          const int st = Tj & (kStages - 1);
-          const uint32_t stra = str0 + st * 2 * kTileBytes;
-          const uint32_t p_addr = p_base + (Tj & 1) * 2 * kTileBytes, ds_addr = ds_base + (Tj & 1) * 2 * kTileBytes;
-          if (!elect_one()) {
-          } else if (MODE == 0) {
-            const uint32_t q_addr = stra, do_addr = stra + kTileBytes;
-#pragma unroll
-            for (int k = 0; k < kTile / 16; ++k) {  // K dim = 128 query rows, 16 per MMA
-              umma_bf16_ss(tAcc0, umma_smem_desc_sw128(p_addr + k * 2048, kTileBytes, 1024),
-                           umma_smem_desc_sw128(do_addr + k * 2048, 8192, 1024), idesc_mm, (jj > 0 || k > 0) ? 1u : 0u);
-              umma_bf16_ss(tAcc1, umma_smem_desc_sw128(ds_addr + k * 2048, kTileBytes, 1024),
-                           umma_smem_desc_sw128(q_addr + k * 2048, 8192, 1024), idesc_mm, (jj > 0 || k > 0) ? 1u : 0u);
-            }
-          } else {
-            const uint32_t k_addr = stra;
-#pragma unroll
-            for (int k = 0; k < kTile / 16; ++k)  // K dim = 128 keys
-              umma_bf16_ss(tAcc0, umma_smem_desc_sw128(ds_addr + (k >> 2) * kTileBytes + (k & 3) * 32, 16, 1024),
-                           umma_smem_desc_sw128(k_addr + k * 2048, 8192, 1024), idesc_km, (jj > 0 || k > 0) ? 1u : 0u);
-          }
-          __syncwarp();
-          if (elect_one()) umma_commit(&str_empty[st]);
-          __syncwarp();
-        }
-        if (it + 1 < tiles) {  // S(it+1)
-          const int Tn = T + 1, st = Tn & (kStages - 1);
-          mbar_wait(&str_full[st], (Tn / kStages) & 1);
-          tc_fence_after();
-          const uint32_t stra = str0 + st * 2 * kTileBytes;
-          const uint32_t q_addr = MODE == 0 ? stra : fixa, k_addr = MODE == 0 ? fixa : stra;
-          const uint32_t tS = tS0 + ((Tn & 1) ? 128u : 0u);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < kD / 16; ++k)
-              umma_bf16_ss(tS, umma_smem_desc_sw128(q_addr + k * 32, 16, 1024),
-                           umma_smem_desc_sw128(k_addr + k * 32, 16, 1024), idesc_kk, k > 0 ? 1u : 0u);
-            umma_commit(&s_full[Tn & 1]);
-          }
-          __syncwarp();
-        }
-      }
-      if (elect_one()) umma_commit(acc_ready);
-      __syncwarp();
-    }
-  } else {
-    // ------------------------------------------------ softmax / epilogue warps
-    const int qd = warp & 3;
-    const int cg = (warp - 2) >> 2;      // column group: 64 of the 128 columns of S / dP
-    const int c0 = cg * 64;
-    const int row = qd * 32 + lane;      // TMEM lane: query row of the current pair
-    const uint32_t lane_addr = (uint32_t)(qd * 32) << 16;
-    const float cl2 = p.scale * 1.4426950408889634f;
-    int T0 = 0, wi = 0;
-    for (int w = blockIdx.x; w < total_items; w += gridDim.x, ++wi, T0 += tiles) {
-      int id = w;
-      const int own = id % tiles;
-      id /= tiles;
-      const int h = id % p.nh, seq = id / p.nh;
-      const float* lse_row = p.lse + ((long long)seq * p.nh + h) * p.S;
-      const float* delta_row = p.delta + ((long long)seq * p.nh + h) * p.S;
-      float lse_fix = 0.f, delta_fix = 0.f, lse_nxt = 0.f, delta_nxt = 0.f;
-      if (MODE == 1) {
-        const int qrow = own * kTile + row;
-        if (qrow < p.S) {
-          lse_fix = __ldg(lse_row + qrow) * 1.4426950408889634f;
-          delta_fix = __ldg(delta_row + qrow);
-        }
-      } else if (row < p.S) {
-        lse_nxt = __ldg(lse_row + row);
-        delta_nxt = __ldg(delta_row + row);
-      }
-      for (int it = 0; it < tiles; ++it) {
-        const int T = T0 + it;
-        const int q_tile = MODE == 0 ? it : own, kv_tile = MODE == 0 ? own : it;
-        const int qrow = q_tile * kTile + row;
-        float lse2 = lse_fix, delta = delta_fix;
-        if (MODE == 0) {
-          lse2 = lse_nxt * 1.4426950408889634f;
-          delta = delta_nxt;
-          if (qrow + kTile < p.S) {
-            lse_nxt = __ldg(lse_row + qrow + kTile);
-            delta_nxt = __ldg(delta_row + qrow + kTile);
-          }
-        }
-        const bool q_ok = qrow < p.S;
-        const int kv_valid = p.S - kv_tile * kTile;
-        const bool full = (q_tile + 1) * kTile <= p.S && kv_valid >= kTile;  // warp-uniform fast path
-        const uint32_t tS = tS0 + ((T & 1) ? 128u : 0u);
-        uint8_t* sPb = sP + (T & 1) * 2 * kTileBytes;
-        uint8_t* sDSb = sDS + (T & 1) * 2 * kTileBytes;
-        float pf[64];
-        uint32_t vs[32], vd[32];
-        mbar_wait(&s_full[T & 1], (T >> 1) & 1);
-        tc_fence_after();
-        // chunk 0 exponentials
-        tmem_ld_32x32(tS + lane_addr + c0, vs);
-        tmem_ld_wait();
-        if (full) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) pf[i] = ex2_approx(fmaf(__uint_as_float(vs[i]), cl2, -lse2));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float pv = ex2_approx(fmaf(__uint_as_float(vs[i]), cl2, -lse2));
-            pf[i] = (q_ok && (c0 + i < kv_valid)) ? pv : 0.f;
-          }
-        }
-        mbar_wait(dp_full, T & 1);
-        tc_fence_after();
-        tmem_ld_32x32(tDP + lane_addr + c0, vd);
-        tmem_ld_32x32(tS + lane_addr + c0 + 32, vs);
-        tmem_ld_wait();
-        // chunk 1 exponentials interleaved with chunk 0's P / dS work (two copies: the whole-tile one carries no
-        // per-element compare / select)
-        auto chunk1 = [&](auto whole) {
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const float pv = ex2_ordered(fmaf(__uint_as_float(vs[i + e]), cl2, -lse2));
-            if constexpr (decltype(whole)::value)
-              pf[32 + i + e] = pv;
-            else
-              pf[32 + i + e] = (q_ok && (c0 + 32 + i + e < kv_valid)) ? pv : 0.f;
-          }
-          const int col = c0 + i;
-          uint4 u;
-          if (MODE == 0) {
-            u.x = pack_bf16x2(pf[i], pf[i + 1]);
-            u.y = pack_bf16x2(pf[i + 2], pf[i + 3]);
-            u.z = pack_bf16x2(pf[i + 4], pf[i + 5]);
-            u.w = pack_bf16x2(pf[i + 6], pf[i + 7]);
-            st_swizzled_chunk_ordered(sPb + (col >> 6) * kTileBytes, row, (col & 63) >> 3, u);
-          }
-          float df[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) df[e] = pf[i + e] * (__uint_as_float(vd[i + e]) - delta);
-          u.x = pack_bf16x2(df[0], df[1]);
-          u.y = pack_bf16x2(df[2], df[3]);
-          u.z = pack_bf16x2(df[4], df[5]);
-          u.w = pack_bf16x2(df[6], df[7]);
-          st_swizzled_chunk_ordered(sDSb + (col >> 6) * kTileBytes, row, (col & 63) >> 3, u);
-        }
-        };
-        if (full)
-          chunk1(std::true_type{});
-        else
-          chunk1(std::false_type{});
-        tmem_ld_32x32(tDP + lane_addr + c0 + 32, vd);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(dp_free);
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          const int col = c0 + 32 + i;
-          uint4 u;
-          if (MODE == 0) {
-            u.x = pack_bf16x2(pf[32 + i], pf[32 + i + 1]);
-            u.y = pack_bf16x2(pf[32 + i + 2], pf[32 + i + 3]);
-            u.z = pack_bf16x2(pf[32 + i + 4], pf[32 + i + 5]);
-            u.w = pack_bf16x2(pf[32 + i + 6], pf[32 + i + 7]);
-            st_swizzled_chunk(sPb + (col >> 6) * kTileBytes, row, (col & 63) >> 3, u);
-          }
-          float df[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) df[e] = pf[32 + i + e] * (__uint_as_float(vd[i + e]) - delta);
-          u.x = pack_bf16x2(df[0], df[1]);
-          u.y = pack_bf16x2(df[2], df[3]);
-          u.z = pack_bf16x2(df[4], df[5]);
-          u.w = pack_bf16x2(df[6], df[7]);
-          st_swizzled_chunk(sDSb + (col >> 6) * kTileBytes, row, (col & 63) >> 3, u);
-        }
-        fence_proxy_async_smem();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(p_ready);
-      }
-      // accumulators of this item: TMEM -> registers, hand TMEM back, then scale / round / store
-      mbar_wait_relaxed(acc_ready, wi & 1);
-      tc_fence_after();
-      uint32_t va[2][32];
-      tmem_ld_32x32(tAcc0 + lane_addr + cg * 32, va[0]);
-      if (MODE == 0) tmem_ld_32x32(tAcc1 + lane_addr + cg * 32, va[1]);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_free);
-      const int orow = own * kTile + row;
-      if (orow < p.S) {
-#pragma unroll
-        for (int a = 0; a < (MODE == 0 ? 2 : 1); ++a) {
-          __nv_bfloat16* base = MODE == 1 ? p.dq : (a == 0 ? p.dv : p.dk);
-          const float osc = (MODE == 0 && a == 0) ? 1.f : p.scale;
-          __nv_bfloat16* dst = base + ((long long)seq * p.S + orow) * p.C + h * kD + cg * 32;
-#pragma unroll
-          for (int i = 0; i < 32; i += 8) {
-            uint4 u;
-            u.x = pack_bf16x2(__uint_as_float(va[a][i]) * osc, __uint_as_float(va[a][i + 1]) * osc);
-            u.y = pack_bf16x2(__uint_as_float(va[a][i + 2]) * osc, __uint_as_float(va[a][i + 3]) * osc);
-            u.z = pack_bf16x2(__uint_as_float(va[a][i + 4]) * osc, __uint_as_float(va[a][i + 5]) * osc);
-            u.w = pack_bf16x2(__uint_as_float(va[a][i + 6]) * osc, __uint_as_float(va[a][i + 7]) * osc);
-            *reinterpret_cast<uint4*>(dst + i) = u;
-          }
-        }
-      }
-    }
-    tc_fence_before();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    store_frag(acc0, p.scale, p.dq + h * kD, row0, p.S, own * kTile, p.C);
   }
 }
 
@@ -1754,6 +376,7 @@ __global__ void og_attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const 
     if (lane == 0) delta[((row / S) * nh + h) * (long long)S + row % S] = v;
   }
 }
+
 
 static int make_seq_map(CUtensorMap* m, const void* base, int nseq, int S, int C) {
   uint64_t dims[3] = {(uint64_t)C, (uint64_t)S, (uint64_t)nseq};
@@ -1788,35 +411,16 @@ extern "C" int og_flash_attn_fwd(const void* q, const void* k, const void* v, vo
   if ((r = make_seq_map(&mq, q, nseq, S, C)) != OG_OK) return r;
   if ((r = make_seq_map(&mk, k, nseq, S, C)) != OG_OK) return r;
   if ((r = make_seq_map(&mv, v, nseq, S, C)) != OG_OK) return r;
-  const size_t smem_bytes = 7 * kTileBytes + 128;
+  const size_t smem_bytes = 5 * kTileBytes + 1024 + 64;
   static bool attr = false;
   if (!attr) {
     OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)smem_bytes));
-    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_fwd_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                       (int)cudaSharedmemCarveoutMaxShared));
-    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_fwd2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)smem_bytes));
-    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_fwd2_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                       (int)cudaSharedmemCarveoutMaxShared));
     attr = true;
   }
   const long long grid = (long long)nseq * n_head * p.q_tiles;
-  // Persistent form for SHORT sequences only. Measured on B200 (32 x 4096 / 128 x 1024 / 512 x 256 tokens, 4 heads):
-  // 0.888 vs 0.857 ms at S = 4096 (static round-robin of 4096 equal items loses to the hardware's dynamic CTA placement with two
-  // CTAs per SM), 0.251 vs 0.254 at S = 1024, 0.196 vs 0.204 at S = 768, 0.141 vs 0.157 at S = 512, 0.086 vs 0.106 at S = 256
-  // (where the per-CTA set-up is half of the kernel). OG_FLASH_FWD_PERSISTENT: 0 = never, 2 = always, otherwise S <= 1024.
-  static const int persistent = [] {
-    const char* e = getenv("OG_FLASH_FWD_PERSISTENT");
-    return e ? atoi(e) : 1;
-  }();
-  if ((persistent == 2 || (persistent == 1 && p.kv_tiles <= 8)) && grid < (1LL << 31)) {
-    const int items = (int)grid;
-    const int ctas = items < 2 * num_sms() ? items : 2 * num_sms();
-    og_flash_attn_fwd2_kernel<<<ctas, kFaThreads, smem_bytes, (cudaStream_t)stream>>>(mq, mk, mv, p, items);
-  } else {
-    og_flash_attn_fwd_kernel<<<(unsigned)grid, kFaThreads, smem_bytes, (cudaStream_t)stream>>>(mq, mk, mv, p);
-  }
+  OG_REQUIRE(grid < (1LL << 31), "flash_attn_fwd: too many tiles");
+  og_flash_attn_fwd_kernel<<<(unsigned)grid, kFaThreads, smem_bytes, (cudaStream_t)stream>>>(mq, mk, mv, p);
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   return OG_OK;
@@ -1850,64 +454,21 @@ extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, co
   if ((r = make_seq_map(&mk, k, nseq, S, C)) != OG_OK) return r;
   if ((r = make_seq_map(&mv, v, nseq, S, C)) != OG_OK) return r;
   if ((r = make_seq_map(&mdo, dout, nseq, S, C)) != OG_OK) return r;
-  const size_t smem_bytes = 14 * kTileBytes + 1024 + 256;
+  const size_t smem_bytes = 6 * kTileBytes + 1024 + 64;
   static bool attr = false;
   if (!attr) {
     OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_bwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)smem_bytes));
     OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)smem_bytes));
-    const void* k2[] = {(const void*)og_flash_attn_bwd2_kernel<0, 8>, (const void*)og_flash_attn_bwd2_kernel<1, 8>,
-                        (const void*)og_flash_attn_bwd2_kernel<0, 16>, (const void*)og_flash_attn_bwd2_kernel<1, 16>,
-                        (const void*)og_flash_attn_bwd3_kernel<0>, (const void*)og_flash_attn_bwd3_kernel<1>};
-    for (const void* f : k2)
-      OG_CHECK_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
     attr = true;
   }
   const long long grid = (long long)nseq * n_head * p.tiles;
-  // OG_FLASH_BWD_V1=1: the un-pipelined first version (kept for A/B timing)
-  static const bool v1 = [] {
-    const char* e = getenv("OG_FLASH_BWD_V1");
-    return e && atoi(e) == 1;
-  }();
-  if (v1) {
-    og_flash_attn_bwd_kernel<0><<<(unsigned)grid, kFaBwdThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
-    OG_CHECK_CUDA(cudaGetLastError());
-    og_flash_attn_bwd_kernel<1><<<(unsigned)grid, kFaBwdThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
-    OG_CHECK_CUDA(cudaGetLastError());
-  } else {
-    static const int il = [] {
-      const char* e = getenv("OG_FLASH_BWD_INTERLEAVE");
-      return (e && atoi(e) == 0) ? 0 : 1;
-    }();
-    p.interleave = il;
-    static const int dbg = [] {
-      const char* e = getenv("OG_FLASH_DBG");
-      return e ? atoi(e) : 0;
-    }();
-    p.dbg = dbg;
-    static const int nw = [] {
-      const char* e = getenv("OG_FLASH_BWD_WARPS");   // 8 or 16 softmax warps
-      return (e && atoi(e) == 16) ? 16 : 8;
-    }();
-    static const int persistent = [] {
-      const char* e = getenv("OG_FLASH_BWD_PERSISTENT");   // 0: one CTA per work item (og_flash_attn_bwd2_kernel)
-      return (e && atoi(e) == 0) ? 0 : 1;
-    }();
-    if (persistent && nw == 8 && p.interleave && !p.dbg && grid < (1LL << 31)) {
-      const int items = (int)grid;
-      const int ctas = items < num_sms() ? items : num_sms();
-      og_flash_attn_bwd3_kernel<0><<<ctas, kFaBwdThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p, items);
-      og_flash_attn_bwd3_kernel<1><<<ctas, kFaBwdThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p, items);
-    } else if (nw == 8) {
-      og_flash_attn_bwd2_kernel<0, 8><<<(unsigned)grid, 64 + 32 * 8, smem_bytes, s>>>(mq, mk, mv, mdo, p);
-      og_flash_attn_bwd2_kernel<1, 8><<<(unsigned)grid, 64 + 32 * 8, smem_bytes, s>>>(mq, mk, mv, mdo, p);
-    } else {
-      og_flash_attn_bwd2_kernel<0, 16><<<(unsigned)grid, 64 + 32 * 16, smem_bytes, s>>>(mq, mk, mv, mdo, p);
-      og_flash_attn_bwd2_kernel<1, 16><<<(unsigned)grid, 64 + 32 * 16, smem_bytes, s>>>(mq, mk, mv, mdo, p);
-    }
-    OG_CHECK_CUDA(cudaGetLastError());
-  }
+  OG_REQUIRE(grid < (1LL << 31), "flash_attn_bwd: too many tiles");
+  og_flash_attn_bwd_kernel<0><<<(unsigned)grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
+  OG_CHECK_CUDA(cudaGetLastError());
+  og_flash_attn_bwd_kernel<1><<<(unsigned)grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
+  OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(2);
   return OG_OK;
 }

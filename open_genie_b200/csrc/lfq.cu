@@ -162,16 +162,16 @@ __global__ void __launch_bounds__(1024)
 __global__ void __launch_bounds__(256)
     og_sgemm_kernel(const float* __restrict__ X, long long sxi, long long sxk, const float* __restrict__ Y,
                     long long syj, long long syk, float* __restrict__ C, long long ldc, int M, int N, int K,
-                    float alpha, int k_per_split) {
+                    float alpha) {
   __shared__ float xs[16][65];
   __shared__ float ys[16][65];
   const int i0 = blockIdx.y * 64, j0 = blockIdx.x * 64;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   float acc[4][4] = {};
-  // split-K over blockIdx.z (the batch-mean code distribution reduces over all tokens into a 512 x 512 result: 64 tiles
-  // cannot fill 148 SMs, so the token range is split and the partial sums are combined with fp32 atomics; C is zeroed)
-  const int k_begin = blockIdx.z * k_per_split;
-  const int k_end = min(K, k_begin + k_per_split);
+  // no split-K: every output is one block's fixed-order sum (reproducible), at the price of only 64 tiles for the
+  // 512 x 512 batch-mean code distribution
+  const int k_begin = 0;
+  const int k_end = K;
   for (int k0 = k_begin; k0 < k_end; k0 += 16) {
     for (int e = threadIdx.x; e < 64 * 16; e += 256) {
       int kk, ii;
@@ -203,12 +203,7 @@ __global__ void __launch_bounds__(256)
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
       const int gi = i0 + ty * 4 + r, gj = j0 + tx * 4 + c;
-      if (gi < M && gj < N) {
-        if (gridDim.z > 1)
-          atomicAdd(&C[gi * ldc + gj], alpha * acc[r][c]);
-        else
-          C[gi * ldc + gj] = alpha * acc[r][c];
-      }
+      if (gi < M && gj < N) C[gi * ldc + gj] = alpha * acc[r][c];
     }
 }
 
@@ -320,19 +315,7 @@ static LfqDims make_dims(int D) {
 static int launch_sgemm(const float* X, long long sxi, long long sxk, const float* Y, long long syj, long long syk,
                         float* C, long long ldc, int M, int N, int K, float alpha, cudaStream_t s) {
   dim3 grid((N + 63) / 64, (M + 63) / 64);
-  // fill ~4 CTAs per SM: split the reduction when the output tiles alone cannot (K multiple of 16 per split)
-  int splits = 1;
-  const int tiles = grid.x * grid.y;
-  if (tiles < 2 * num_sms() && K >= 512) {
-    splits = (4 * num_sms() + tiles - 1) / tiles;
-    if (splits > K / 128) splits = K / 128;
-    if (splits < 1) splits = 1;
-  }
-  int kps = ((K + splits - 1) / splits + 15) / 16 * 16;
-  splits = (K + kps - 1) / kps;
-  grid.z = splits;
-  if (splits > 1) OG_CHECK_CUDA(cudaMemsetAsync(C, 0, sizeof(float) * (size_t)M * ldc, s));
-  og_sgemm_kernel<<<grid, 256, 0, s>>>(X, sxi, sxk, Y, syj, syk, C, ldc, M, N, K, alpha, kps);
+  og_sgemm_kernel<<<grid, 256, 0, s>>>(X, sxi, sxk, Y, syj, syk, C, ldc, M, N, K, alpha);
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   return OG_OK;

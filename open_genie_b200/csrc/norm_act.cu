@@ -88,7 +88,7 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
 // statistics: grid (chunks, N); block 256. Thread -> (channel vector cv, row lane rl).
 // ------------------------------------------------------------------------------------------------
 static constexpr int kStatRows = 16;  // granularity of the row ranges handed to a block. (It was 256: the 512-channel
-// 4x8x8 stage has V = 256 rows per sample, i.e. ONE block per sample = 8 CTAs on 148 SMs, each walking 64 dependent
+// 4x8x8 stage has V = 256 rows per sample, i.e. ONE block per sample = 8 CTAs on 132 SMs, each walking 64 dependent
 // iterations — 62 such launches per pass made the low-resolution stages cost as much as the 16x64x64 ones.)
 
 // grid (blocks_per_sample, N); each block owns a contiguous row range of one sample and keeps fp32 partial
@@ -229,7 +229,8 @@ template <int ACT>
 __global__ void __launch_bounds__(256, 3)
     og_affine_act_bwd_reduce_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x,
                                     const float* __restrict__ A, const float* __restrict__ B, long long V, int C,
-                                    int /*act: template parameter ACT*/, long long rows_per_block, float* __restrict__ S) {
+                                    int /*act: template parameter ACT*/, long long rows_per_block, float* __restrict__ S,
+                                    float* __restrict__ partials) {
   constexpr int act = ACT;  // compile-time: the per-element switch cost 20 % of the backward pass as a runtime value
   const int cvs = C >> 3;  // host guarantees cvs <= 256
   const int n = blockIdx.y;
@@ -287,20 +288,55 @@ __global__ void __launch_bounds__(256, 3)
     for (int k = 0; k < 16; ++k) part[threadIdx.x * 16 + k] = 0.f;
   }
   __syncthreads();
-  // thread index == rl * cvs + cv: sum the row lanes of every channel (no contended shared atomics)
+  // thread index == rl * cvs + cv: sum the row lanes of every channel (no contended shared atomics). With several blocks
+  // per sample each block stores its sums as a partial, added up in block order by sum_partials (reproducible); a single
+  // block per sample adds into S itself.
   for (int i = threadIdx.x; i < 2 * C; i += 256) {
     const int c = i >> 1, which = i & 1;
     float a = 0.f;
     for (int l = 0; l < lanes; ++l) a += part[(l * cvs + (c >> 3)) * 16 + which * 8 + (c & 7)];
-    atomicAdd(&S[(long long)n * C * 2 + i], a);
+    if (partials)
+      partials[((long long)n * gridDim.x + blockIdx.x) * 2 * C + i] = a;
+    else
+      S[(long long)n * C * 2 + i] += a;
   }
+}
+
+// dgamma[c] += sum_n s T2, dbeta[c] += sum_n s T1 (s = cond_scale[n][c] or 1), one thread per channel walking the samples
+// in order: reproducible, no atomics.
+__global__ void __launch_bounds__(256)
+    og_gn_param_grads_kernel(const float* __restrict__ S, const float* __restrict__ mean_rstd,
+                             const float* __restrict__ cond_scale, int N, int C, int G, float* __restrict__ dgamma,
+                             float* __restrict__ dbeta) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const int g = c / (C / G);
+  float dg = 0.f, db = 0.f;
+  for (int n = 0; n < N; ++n) {
+    const float mu = mean_rstd[((long long)n * G + g) * 2], rstd = mean_rstd[((long long)n * G + g) * 2 + 1];
+    const float s1 = S[((long long)n * C + c) * 2], s2 = S[((long long)n * C + c) * 2 + 1];
+    const float sc = cond_scale ? cond_scale[(long long)n * C + c] : 1.f;
+    dg += sc * (rstd * (s2 - mu * s1));
+    db += sc * s1;
+  }
+  if (dgamma) dgamma[c] += dg;
+  if (dbeta) dbeta[c] += db;
+}
+
+static int launch_param_grads(const float* S, const float* mean_rstd, const float* cond_scale, int N, int C, int G,
+                              float* dgamma, float* dbeta, cudaStream_t stream) {
+  if (!dgamma && !dbeta) return OG_OK;
+  og_gn_param_grads_kernel<<<(C + 255) / 256, 256, 0, stream>>>(S, mean_rstd, cond_scale, N, C, G, dgamma, dbeta);
+  OG_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1);
+  return OG_OK;
 }
 
 // backward finalize: one block per sample n, 256 threads.
 //   T1 = S1, T2 = rstd*(S2 - mean*S1);  g' = gamma*s
 //   m1_g = sum_{c in g} g' T1 / M,  m2_g = sum_{c in g} g' T2 / M     (M = V * C/G)
 //   P = A,  Q = -rstd^2 m2,  R = rstd (m2 rstd mean - m1)
-//   dgamma[c] += s T2, dbeta[c] += s T1 (atomic over n), dscale[n][c] = gamma T2 + beta T1, dshift[n][c] = T1
+//   dscale[n][c] = gamma T2 + beta T1, dshift[n][c] = T1 (dgamma / dbeta: og_gn_param_grads_kernel)
 __global__ void __launch_bounds__(256)
     og_gn_bwd_finalize_kernel(const float* __restrict__ S, const float* __restrict__ mean_rstd,
                               const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -309,25 +345,30 @@ __global__ void __launch_bounds__(256)
                               float* __restrict__ dcond_scale, float* __restrict__ dcond_shift) {
   const int n = blockIdx.x;
   __shared__ double m1s[64], m2s[64];
-  for (int i = threadIdx.x; i < G; i += blockDim.x) m1s[i] = m2s[i] = 0.0;
-  __syncthreads();
   const int cpg = C / G;
+  // group sums in a fixed order (reproducible): one thread per group walks its channels
+  for (int g = threadIdx.x; g < G; g += blockDim.x) {
+    const float mu = mean_rstd[((long long)n * G + g) * 2], rstd = mean_rstd[((long long)n * G + g) * 2 + 1];
+    double a1 = 0.0, a2 = 0.0;
+    for (int c = g * cpg; c < (g + 1) * cpg; ++c) {
+      const float s1 = S[((long long)n * C + c) * 2], s2 = S[((long long)n * C + c) * 2 + 1];
+      const float gp = (gamma ? gamma[c] : 1.f) * (cond_scale ? cond_scale[(long long)n * C + c] : 1.f);
+      a1 += (double)(gp * s1);
+      a2 += (double)(gp * (rstd * (s2 - mu * s1)));
+    }
+    m1s[g] = a1;
+    m2s[g] = a2;
+  }
+  __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     const int g = c / cpg;
     const float mu = mean_rstd[((long long)n * G + g) * 2], rstd = mean_rstd[((long long)n * G + g) * 2 + 1];
     const float s1 = S[((long long)n * C + c) * 2], s2 = S[((long long)n * C + c) * 2 + 1];
     const float t1 = s1, t2 = rstd * (s2 - mu * s1);
     const float ga = gamma ? gamma[c] : 1.f, be = beta ? beta[c] : 0.f;
-    const float sc = cond_scale ? cond_scale[(long long)n * C + c] : 1.f;
-    const float gp = ga * sc;
-    atomicAdd(&m1s[g], (double)(gp * t1));
-    atomicAdd(&m2s[g], (double)(gp * t2));
-    if (dgamma) atomicAdd(&dgamma[c], sc * t2);
-    if (dbeta) atomicAdd(&dbeta[c], sc * t1);
     if (dcond_scale) dcond_scale[(long long)n * C + c] = ga * t2 + be * t1;
     if (dcond_shift) dcond_shift[(long long)n * C + c] = t1;
   }
-  __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     const int g = c / cpg;
     const float mu = mean_rstd[((long long)n * G + g) * 2], rstd = mean_rstd[((long long)n * G + g) * 2 + 1];
@@ -478,7 +519,8 @@ __global__ void __launch_bounds__(256, 3)
                          const float* __restrict__ cond_scale, const uint4* __restrict__ add, uint4* __restrict__ dx,
                          float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dcond_scale,
                          float* __restrict__ dcond_shift, float* __restrict__ dx_colsum, long long V, int C, int G,
-                         double inv_M, int /*act: template parameter ACT*/, long long rows_per_block) {
+                         double inv_M, int /*act: template parameter ACT*/, long long rows_per_block,
+                         float* __restrict__ partials) {
   constexpr int act = ACT;  // compile-time: the per-element switch cost 20 % of the backward pass as a runtime value
   const int cvs = C >> 3;
   const int n = blockIdx.y;
@@ -489,38 +531,30 @@ __global__ void __launch_bounds__(256, 3)
   const int cpg = C / G;
   __shared__ double m1s[64], m2s[64];
   extern __shared__ float cs_s[];  // [256][8] per-thread column sums of dx (only when dx_colsum)
-  for (int i = threadIdx.x; i < G; i += 256) m1s[i] = m2s[i] = 0.0;
   if (dx_colsum)
     for (int i = threadIdx.x; i < 256 * 8; i += 256) cs_s[i] = 0.f;
   __syncthreads();
   if (S) {
-    const bool warp_uniform = (cpg % 32) == 0;  // then C % 32 == 0 and a warp's 32 channels share one group
+    // group sums in a fixed order (reproducible): one thread per group walks its channels
+    for (int g = threadIdx.x; g < G; g += 256) {
+      const float mu = mean_rstd[((long long)n * G + g) * 2], rstd = mean_rstd[((long long)n * G + g) * 2 + 1];
+      double a1 = 0.0, a2 = 0.0;
+      for (int c = g * cpg; c < (g + 1) * cpg; ++c) {
+        const float s1 = S[((long long)n * C + c) * 2], s2 = S[((long long)n * C + c) * 2 + 1];
+        const float gp = (gamma ? gamma[c] : 1.f) * (cond_scale ? cond_scale[(long long)n * C + c] : 1.f);
+        a1 += (double)(gp * s1);
+        a2 += (double)(gp * (rstd * (s2 - mu * s1)));
+      }
+      m1s[g] = a1;
+      m2s[g] = a2;
+    }
     for (int c = threadIdx.x; c < C; c += 256) {
       const int g = c / cpg;
       const float mu = mean_rstd[((long long)n * G + g) * 2], rstd = mean_rstd[((long long)n * G + g) * 2 + 1];
       const float s1 = S[((long long)n * C + c) * 2], s2 = S[((long long)n * C + c) * 2 + 1];
       const float t1 = s1, t2 = rstd * (s2 - mu * s1);
       const float ga = gamma ? gamma[c] : 1.f, be = beta ? beta[c] : 0.f;
-      const float sc = cond_scale ? cond_scale[(long long)n * C + c] : 1.f;
-      const float gp = ga * sc;
-      double v1 = (double)(gp * t1), v2 = (double)(gp * t2);
-      if (warp_uniform) {
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) {
-          v1 += __shfl_xor_sync(0xffffffffu, v1, off);
-          v2 += __shfl_xor_sync(0xffffffffu, v2, off);
-        }
-        if ((threadIdx.x & 31) == 0) {
-          atomicAdd(&m1s[g], v1);
-          atomicAdd(&m2s[g], v2);
-        }
-      } else {
-        atomicAdd(&m1s[g], v1);
-        atomicAdd(&m2s[g], v2);
-      }
       if (blockIdx.x == 0) {
-        if (dgamma) atomicAdd(&dgamma[c], sc * t2);
-        if (dbeta) atomicAdd(&dbeta[c], sc * t1);
         if (dcond_scale) dcond_scale[(long long)n * C + c] = ga * t2 + be * t1;
         if (dcond_shift) dcond_shift[(long long)n * C + c] = t1;
       }
@@ -598,11 +632,15 @@ __global__ void __launch_bounds__(256, 3)
     }
   }
   if (dx_colsum) {
+    // one partial per block, added up in block order by sum_partials (reproducible); a single block adds directly
     __syncthreads();
     for (int i = threadIdx.x; i < C; i += 256) {
       float a = 0.f;
       for (int l = 0; l < lanes; ++l) a += cs_s[(l * cvs + (i >> 3)) * 8 + (i & 7)];
-      atomicAdd(&dx_colsum[i], a);
+      if (partials)
+        partials[((long long)blockIdx.y * gridDim.x + blockIdx.x) * C + i] = a;
+      else
+        dx_colsum[i] += a;
     }
   }
 }
@@ -717,6 +755,23 @@ static dim3 reduce_grid(int N, long long V, long long* rows_per_block, int per_s
   return dim3((unsigned)((groups + gpb - 1) / gpb), (unsigned)N);
 }
 
+// reduce_grid, with at most as many blocks as the workspace holds partials of `floats_per_block` floats (at least one
+// block per sample; then the blocks add into the output directly)
+static dim3 partial_grid(int N, long long V, long long floats_per_block, void* workspace, size_t workspace_bytes,
+                         long long* rows_per_block) {
+  dim3 grid = reduce_grid(N, V, rows_per_block, 6);
+  const long long fit = workspace ? (long long)(workspace_bytes / sizeof(float)) / floats_per_block : 0;
+  if ((long long)grid.x * grid.y > fit) {
+    long long want = fit / N;
+    if (want < 1) want = 1;
+    const long long groups = (V + kStatRows - 1) / kStatRows;
+    const long long gpb = (groups + want - 1) / want;
+    *rows_per_block = gpb * kStatRows;
+    grid.x = (unsigned)((groups + gpb - 1) / gpb);
+  }
+  return grid;
+}
+
 static int ew_grid(long long total, int block) {
   long long g = (total + block - 1) / block;
   long long cap = (long long)num_sms() * 16;
@@ -768,19 +823,22 @@ extern "C" int og_affine_act_fwd(const void* x, const float* A, const float* B, 
 }
 
 extern "C" int og_affine_act_bwd_reduce(const void* dy, const void* x, const float* A, const float* B, int act,
-                                        float* S, int N, int64_t V, int C, og_stream_t stream) {
+                                        float* S, int N, int64_t V, int C, void* workspace, size_t workspace_bytes,
+                                        og_stream_t stream) {
   OG_REQUIRE(dy && x && A && B && S, "affine_act_bwd_reduce: null pointer");
   OG_REQUIRE(C % 8 == 0 && C <= 2048, "affine_act_bwd_reduce: C=%d must be a multiple of 8 and <= 2048", C);
   long long rpb;
-  const dim3 grid = reduce_grid(N, V, &rpb, 6);
+  const dim3 grid = partial_grid(N, V, 2LL * C, workspace, workspace_bytes, &rpb);
+  float* partials = grid.x > 1 ? reinterpret_cast<float*>(workspace) : nullptr;
 #define OG_LAUNCH(ACT)                                                                                  \
   og_affine_act_bwd_reduce_kernel<ACT><<<grid, 256, 0, (cudaStream_t)stream>>>(                          \
-      reinterpret_cast<const uint4*>(dy), reinterpret_cast<const uint4*>(x), A, B, V, C, act, rpb, S)
+      reinterpret_cast<const uint4*>(dy), reinterpret_cast<const uint4*>(x), A, B, V, C, act, rpb, S, partials)
   OG_REQUIRE(act >= 0 && act <= 3, "affine_act_bwd_reduce: unknown activation code %d", act);
   if (act == 0) OG_LAUNCH(0); else if (act == 1) OG_LAUNCH(1); else if (act == 2) OG_LAUNCH(2); else OG_LAUNCH(3);
 #undef OG_LAUNCH
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
+  if (partials) return sum_partials(partials, N, (int)grid.x, 2LL * C, 2LL * C, 2LL * C, S, (cudaStream_t)stream);
   return OG_OK;
 }
 
@@ -795,7 +853,7 @@ extern "C" int og_gn_bwd_finalize(const float* S, const float* mean_rstd, const 
                                                                  R, dgamma, dbeta, dcond_scale, dcond_shift);
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
-  return OG_OK;
+  return launch_param_grads(S, mean_rstd, cond_scale, N, C, G, dgamma, dbeta, (cudaStream_t)stream);
 }
 
 extern "C" int og_affine_act_bwd_apply(const void* dy, const void* x, const float* A, const float* B, const float* Q,
@@ -838,24 +896,32 @@ extern "C" int og_gn_act_bwd(const void* dy, const void* x, const float* A, cons
                              const float* mean_rstd, const float* gamma, const float* beta, const float* cond_scale,
                              int G, int act, const void* add, void* dx, float* dgamma, float* dbeta,
                              float* dcond_scale, float* dcond_shift, float* dx_colsum, int N, int64_t V, int C,
-                             og_stream_t stream) {
+                             void* workspace, size_t workspace_bytes, og_stream_t stream) {
   OG_REQUIRE(dy && x && A && B && dx, "gn_act_bwd: null pointer");
   OG_REQUIRE((S == nullptr) == (mean_rstd == nullptr), "gn_act_bwd: S and mean_rstd must both be given or both NULL");
   OG_REQUIRE(C % 8 == 0 && C <= 2048 && G >= 1 && G <= 64 && C % G == 0 && (C / G) % 8 == 0,
              "gn_act_bwd: need C%%8==0, C<=2048, G<=64, (C/G)%%8==0 (C=%d G=%d)", C, G);
   long long rpb;
-  const dim3 grid = reduce_grid(N, V, &rpb, 6);
+  // with dx_colsum: one C-wide partial per block in the workspace (the grid shrinks to what fits; one block adds directly)
+  const dim3 grid = dx_colsum ? partial_grid(N, V, (long long)C, workspace, workspace_bytes, &rpb) : reduce_grid(N, V, &rpb, 6);
+  float* partials = (dx_colsum && (long long)grid.x * grid.y > 1) ? reinterpret_cast<float*>(workspace) : nullptr;
+  OG_REQUIRE(!dx_colsum || N == 1 || (workspace && workspace_bytes >= (size_t)N * C * sizeof(float)),
+             "gn_act_bwd: dx_colsum over N=%d samples needs a workspace of at least N*C floats", N);
   const double inv_M = 1.0 / ((double)V * (C / G));
 #define OG_LAUNCH(ACT)                                                                                                    \
   og_gn_act_bwd_kernel<ACT><<<grid, 256, dx_colsum ? 256 * 8 * sizeof(float) : 0, (cudaStream_t)stream>>>(                \
       reinterpret_cast<const uint4*>(dy), reinterpret_cast<const uint4*>(x), A, B, S, mean_rstd, gamma, beta, cond_scale, \
       reinterpret_cast<const uint4*>(add), reinterpret_cast<uint4*>(dx), dgamma, dbeta, dcond_scale, dcond_shift,         \
-      dx_colsum, V, C, G, inv_M, act, rpb)
+      dx_colsum, V, C, G, inv_M, act, rpb, partials)
   OG_REQUIRE(act >= 0 && act <= 3, "gn_act_bwd: unknown activation code %d", act);
   if (act == 0) OG_LAUNCH(0); else if (act == 1) OG_LAUNCH(1); else if (act == 2) OG_LAUNCH(2); else OG_LAUNCH(3);
 #undef OG_LAUNCH
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
+  int rc = OG_OK;
+  if (partials) rc = sum_partials(partials, 1, (int)(grid.x * grid.y), C, C, C, dx_colsum, (cudaStream_t)stream);
+  if (rc != OG_OK) return rc;
+  if (S) return launch_param_grads(S, mean_rstd, cond_scale, N, C, G, dgamma, dbeta, (cudaStream_t)stream);
   return OG_OK;
 }
 

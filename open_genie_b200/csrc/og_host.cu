@@ -65,10 +65,45 @@ int num_sms() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
+}
+
+// One block per 32 consecutive outputs of one group: warp w adds the partials b = w, w + 8, ... in order, then the eight
+// warp sums are added in warp order — a fixed summation tree, so the result does not depend on scheduling.
+__global__ void __launch_bounds__(256)
+    og_sum_partials_kernel(const float* __restrict__ partials, int nparts, long long width, long long row_len,
+                           long long out_ld, float* __restrict__ out) {
+  __shared__ float red[8][32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const long long i = (long long)blockIdx.x * 32 + lane;
+  const long long g = blockIdx.y;
+  float a = 0.f;
+  if (i < width)
+    for (int b = w; b < nparts; b += 8) a += __ldcg(partials + (g * nparts + b) * width + i);
+  red[w][lane] = a;
+  __syncthreads();
+  if (w == 0 && i < width) {
+    float t = red[0][lane];
+    for (int k = 1; k < 8; ++k) t += red[k][lane];
+    const long long o = g * width + i;
+    out[o / row_len * out_ld + o % row_len] += t;
+  }
+}
+
+int sum_partials(const float* partials, int groups, int nparts, long long width, long long row_len, long long out_ld,
+                 float* out, cudaStream_t stream) {
+  OG_REQUIRE(groups >= 1 && groups <= 65535 && nparts >= 1 && width >= 1 && row_len >= 1 && out_ld >= row_len,
+             "sum_partials: bad shape");
+  const long long bx = (width + 31) / 32;
+  OG_REQUIRE(bx < (1LL << 31), "sum_partials: too wide");
+  og_sum_partials_kernel<<<dim3((unsigned)bx, (unsigned)groups), 256, 0, stream>>>(partials, nparts, width, row_len, out_ld,
+                                                                                   out);
+  OG_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1);
+  return OG_OK;
 }
 
 static int pow2_ceil(int v) {
@@ -99,6 +134,6 @@ void choose_voxel_box(int vox, int N, int T, int H, int W, int* bw, int* bh, int
 extern "C" {
 const char* og_last_error(void) { return og::g_err; }
 int og_abi_version(void) { return 1; }
-int og_compiled_sm(void) { return 100; }
+int og_compiled_sm(void) { return 90; }
 uint64_t og_launch_count(void) { return og::g_launches.load(); }
 }

@@ -48,6 +48,12 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
 
 int num_sms();
 
+// Reproducible sums of per-block partial results: out[(g*width + i) / row_len * out_ld + (g*width + i) % row_len] +=
+// sum over b < nparts of partials[(g * nparts + b) * width + i], added in b order (grid: groups g; see og_host.cu).
+int sum_partials(const float* partials, int groups, int nparts, long long width, long long row_len, long long out_ld,
+                 float* out, cudaStream_t stream);
+
+
 // Decompose a block of `vox` (power of two) voxels into a (bw, bh, bt, bn) box over (W, H, T, N):
 // widest-first powers of two. Dimensions need not divide: partial boxes are zero-filled by TMA on
 // load and masked on store.

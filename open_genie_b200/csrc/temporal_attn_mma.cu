@@ -1,13 +1,12 @@
 // temporal_attn_mma.cu — tensor-core form of the temporal (causal, T <= 16, d_head = 64) attention.
 //
-// STATUS: validated on a B200 in round 2 (tests/test_gpu_attention.py and the full-size LatentAction / Dynamics parity
-// tests) and the default path since then; OG_TEMPORAL_MMA=0 falls back to the per-lane kernels in attention_rows.cu.
+// STATUS: checked by tests/test_gpu_attention.py and the full-size LatentAction / Dynamics parity tests; the default path; OG_TEMPORAL_MMA=0 falls back to the per-lane kernels in attention_rows.cu.
 // SASS: LDSM / HMMA.16816.F32.BF16.
 //
 // Why: one (batch, pixel, head) task is a 16 x 16 x 64 score tile and a 16 x 64 x 16 value product. The per-lane
 // dot-product kernels spend ~2.5 K instructions per task and run ~4x above their HBM roofline time; with
-// mma.sync.m16n8k16 the same task is 16 HMMA instructions forward (40 backward). tcgen05 is the wrong tool here:
-// its M = 128 tiles would need 8 unrelated tasks packed block-diagonally.
+// mma.sync.m16n8k16 the same task is 16 HMMA instructions forward (40 backward). wgmma is the wrong tool here:
+// its M = 64 warpgroup tiles would need 4 unrelated tasks packed block-diagonally.
 //
 // Reference semantics: TemporalAttention.forward -> Attention.forward (genie/module/attention.py:309-371,
 // 199-239): SDPA(q, k, v, is_causal=True, scale = n_head * d_head**-0.5) per pixel over t, optional (B, T, C)

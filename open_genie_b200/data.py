@@ -1,7 +1,7 @@
 """Data path — mirrors genie/module/data.py:24-233 (LightningDataset, Platformer2D) and genie/dataset.py:95-161
 (LightningPlatformer2D): same constructors, same `from_config`, same loaders, same tensors.
 
-B200-first change (opt-in, `raw_uint8=True` + VideoBatchPrefetcher): the reference converts every decoded frame to
+GPU-first change (opt-in, `raw_uint8=True` + VideoBatchPrefetcher): the reference converts every decoded frame to
 fp32, divides by 255 and rearranges on the CPU workers, then ships 4 bytes per element over PCIe. Here the workers hand
 over the frames exactly as OpenCV decodes them (uint8, t h w c, BGR); batches are staged in pinned memory, copied on a
 side stream while the previous step computes, and ONE kernel (og_frames_u8_to_video) does the colour swap, the /255 and

@@ -1,5 +1,5 @@
 """DynamicsModel — mirrors genie/dynamics.py:14-194 (MaskGIT dynamics over space-time transformer blocks) on the
-B200 kernels: fused token+action embedding, SpaceTimeAttention blocks, the vocabulary head on the tcgen05 GEMM
+CUDA kernels: fused token+action embedding, SpaceTimeAttention blocks, the vocabulary head on the wgmma GEMM
 kernel, a fused masked cross entropy. Same constructor, forward / compute_loss / generate / get_schedule
 signatures, return values and state_dict keys (tok_emb.weight, act_emb.0.weight, head.{weight,bias},
 dec_layers.N.*)."""

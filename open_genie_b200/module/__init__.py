@@ -45,7 +45,7 @@ def get_module(name: str):
             return SiLU
         case _ if name in _OUT_OF_SCOPE:
             raise NotImplementedError(f'module {name!r} is registered by the reference but lies outside the '
-                                      f'B200 hot-path scope (no shipped blueprint uses it)')
+                                      f'hot-path scope (no shipped blueprint uses it)')
         case _:
             raise ValueError(f'Unknown module name: {name}')
 

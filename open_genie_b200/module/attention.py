@@ -1,5 +1,5 @@
 """Space-time attention — same class names, constructor kwargs and state_dict keys as the reference's
-genie/module/attention.py, executed by the fused B200 kernels (csrc/attention_rows.cu, flash_attn.cu,
+genie/module/attention.py, executed by the fused CUDA kernels (csrc/attention_rows.cu, flash_attn.cu,
 conv3d_*.cu).
 
 Only the HEAD-valid configuration is implemented (SURVEY.md §7 H6/H8): d_inp == d_out == n_head*d_head, so
@@ -30,7 +30,7 @@ class RotaryEmbedding(nn.Module):
     def __init__(self, dim: int, kind: str = '1d', theta=10000, max_freq=10, learned_freq=False) -> None:
         super().__init__()
         if learned_freq:
-            raise NotImplementedError('learned rotary frequencies are outside the B200 hot-path scope')
+            raise NotImplementedError('learned rotary frequencies are outside the hot-path scope')
         match kind:
             case '1d':
                 freq = 1. / (theta ** (torch.arange(0, dim, 2)[:(dim // 2)].float() / dim))
@@ -79,7 +79,7 @@ class Attention(nn.Module):
         if not embed:
             raise NotImplementedError('embed=False is not used by any shipped blueprint')
         if d_head != 64:
-            raise NotImplementedError('the tcgen05 attention kernels are specialised for d_head = 64 '
+            raise NotImplementedError('the flash attention kernels are specialised for d_head = 64 '
                                       '(every shipped blueprint uses 64)')
         self.norm = nn.LayerNorm(hid)
         self.embed = RotaryEmbedding(self.d_inp, kind=self.rope_kind)

@@ -1,5 +1,5 @@
 """GAN critics of the tokenizer objective — mirrors genie/module/discriminator.py:17-221 (same constructors, same
-state_dict keys: proj_in.*, core.N.0.{main,res}.*, to_logits.{0,3}.*) on the B200 kernels."""
+state_dict keys: proj_in.*, core.N.0.{main,res}.*, to_logits.{0,3}.*) on the CUDA kernels."""
 from __future__ import annotations
 
 from itertools import pairwise
@@ -47,7 +47,7 @@ class FrameDiscriminator(nn.Module):
                  act_fn: str = 'leaky') -> None:
         super().__init__()
         if use_attn:
-            raise NotImplementedError('FrameDiscriminator(use_attn=True) is outside the B200 hot-path scope')
+            raise NotImplementedError('FrameDiscriminator(use_attn=True) is outside the hot-path scope')
         if isinstance(inp_size, int):
             inp_size = (inp_size, inp_size)
         dims = [model_dim * mult for mult in dim_mults]

@@ -1,4 +1,4 @@
-"""nn.Linear-compatible parameter holder whose forward runs on the tcgen05 GEMM kernel."""
+"""nn.Linear-compatible parameter holder whose forward runs on the wgmma GEMM kernel."""
 from __future__ import annotations
 
 import math

@@ -10,7 +10,7 @@ from .. import ops
 
 
 class GroupNorm(nn.GroupNorm):
-    """Blueprint 'group_norm' (genie/tokenizer.py:75-78): nn.GroupNorm's parameters, fused B200 kernels."""
+    """Blueprint 'group_norm' (genie/tokenizer.py:75-78): nn.GroupNorm's parameters, fused CUDA kernels."""
 
     def forward(self, x: Tensor) -> Tensor:
         return ops.group_norm_act(x, self.weight, self.bias, self.num_groups, self.eps, 'none')

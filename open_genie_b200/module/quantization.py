@@ -20,7 +20,7 @@ class LookupFreeQuantization(nn.Module):
         super().__init__()
         if num_codebook != 1:
             raise NotImplementedError('num_codebook > 1 duplicates codes in the reference (quantization.py:52,74) '
-                                      'and is outside the B200 hot-path scope')
+                                      'and is outside the hot-path scope')
         codebook_size = (2 ** codebook_dim) * num_codebook
         input_dim = default(input_dim, codebook_size)
         project = input_dim != codebook_dim * num_codebook

@@ -1,5 +1,5 @@
 """Video building blocks — same class names, constructor kwargs and state_dict keys as the reference's
-genie/module/video.py, but every forward runs hand-written sm_100a kernels through the C ABI.
+genie/module/video.py, but every forward runs hand-written sm_90a kernels through the C ABI.
 
 state_dict compatibility: conv weights are ordinary (Cout, Cin, kt, kh, kw) fp32 parameters (stored in
 channels_last_3d memory so their bytes ARE the kernels' [Cout][tap][Cin] operand order); the bf16 operand
@@ -116,7 +116,7 @@ class CausalConv3d(nn.Module):
                  padding=None, pad_mode: str = 'constant', **kwargs):
         super().__init__()
         if _triple(dilation) != (1, 1, 1):
-            raise NotImplementedError('CausalConv3d: dilation != 1 is outside the B200 hot-path scope')
+            raise NotImplementedError('CausalConv3d: dilation != 1 is outside the hot-path scope')
         if pad_mode != 'constant' or padding not in (None, (None, None)):
             raise NotImplementedError('CausalConv3d: only default constant padding is implemented')
         self.conv3d = Conv3dParams(in_channels, out_channels, kernel_size, stride, causal=True,
@@ -257,7 +257,7 @@ class VideoResidualBlock(nn.Module):
     genie/module/video.py:539-656. state_dict keys: main.{0,4}.{weight,bias}, main.{2,6}.{weight,bias},
     res.1.{weight,bias}.
 
-    B200 execution: each GN+SiLU is one statistics pass + one fused apply pass, and the second conv, the
+    GPU execution: each GN+SiLU is one statistics pass + one fused apply pass, and the second conv, the
     shortcut conv and the residual add are a single implicit GEMM (the shortcut's K columns are appended
     to the main conv's operand matrix)."""
 

@@ -136,10 +136,24 @@ class StepScope:
     def __init__(self, arena: Optional[ZeroArena] = None):
         self.arena = arena
         self.ws = {}          # device -> uint8 workspace
+        self.scratch_bufs = {}   # device -> uint8 scratch for per-block / per-split partial sums (no contents kept)
         self.frozen = False
 
+    SCRATCH_BYTES = 64 << 20
+
+    def scratch(self, dev):
+        """Scratch for the reproducible reductions (weight-gradient split-K slabs, GroupNorm backward partials): every
+        use is stream-ordered and complete inside one C-ABI call; the kernels limit their split to what fits."""
+        t = self.scratch_bufs.get(dev)
+        if t is None:
+            if self.frozen or (dev.type == 'cuda' and torch.cuda.is_current_stream_capturing()):
+                raise RuntimeError('open_genie_b200: reduction scratch of a captured training step would have to grow')
+            t = torch.empty(self.SCRATCH_BYTES, dtype=torch.uint8, device=dev)
+            self.scratch_bufs[dev] = t
+        return t
+
     def workspace(self, dev, nbytes: int):
-        # >= 24 MB: room for one partial-sum slab per split (splits x tiles <= 148 tiles of 128 x 256 fp32 = 19.4 MB)
+        # >= 24 MB: room for one partial-sum slab per split (splits x tiles <= 132 tiles of 128 x 128 fp32 = 8.7 MB)
         nbytes = min(max(nbytes, 24 << 20), 1 << 30)
         t = self.ws.get(dev)
         if t is None or t.numel() < nbytes:
@@ -228,11 +242,17 @@ def _gn_bwd(dy, x, A, Bc, S, mr, gamma, beta, G, act, add, dx, dgamma, dbeta, dx
         oa, oc, oS, om = n0 * V * C * 2, n0 * C * 4, n0 * C * 8, n0 * G * 8
         if reduce:
             _lib.call('og_affine_act_bwd_reduce', dy.data_ptr() + oa, x.data_ptr() + oa, A.data_ptr() + oc, Bc.data_ptr() + oc,
-                      act, S.data_ptr() + oS, nb, V, C, s)
+                      act, S.data_ptr() + oS, nb, V, C, *_scratch(dy), s)
         _lib.call('og_gn_act_bwd', dy.data_ptr() + oa, x.data_ptr() + oa, A.data_ptr() + oc, Bc.data_ptr() + oc,
                   S.data_ptr() + oS, mr.data_ptr() + om, gamma.data_ptr(), beta.data_ptr(), None, G, act,
                   (add.data_ptr() + oa) if add is not None else None, dx.data_ptr() + oa, dgamma.data_ptr(), dbeta.data_ptr(),
-                  None, None, dx_colsum.data_ptr() if dx_colsum is not None else None, nb, V, C, s)
+                  None, None, dx_colsum.data_ptr() if dx_colsum is not None else None, nb, V, C, *_scratch(dy), s)
+
+
+def _scratch(t: Tensor):
+    """(pointer, bytes) of the current step scope's reduction scratch on t's device, for the C-ABI workspace arguments."""
+    buf = _SCOPE.scratch(t.device)
+    return buf.data_ptr(), buf.numel()
 
 
 def _workspace(dev, nbytes: int):
@@ -493,10 +513,11 @@ class _Conv3dFn(torch.autograd.Function):
             if want_db and FUSE_BIAS_GRAD and not fused_db[0]:
                 fused_db[0] = True
                 _conv_call('wgrad', fl, 'og_conv3d_wgrad_bias', dyb.data_ptr(), cpad, xin.data_ptr(), cin, g.data_ptr(),
-                           g.shape[1], kt, kh, kw, pt, ph, pw, dims[0], dims[1], dims[2], dims[3], dbs.data_ptr(), cout, s)
+                           g.shape[1], kt, kh, kw, pt, ph, pw, dims[0], dims[1], dims[2], dims[3], dbs.data_ptr(), cout,
+                           *_scratch(dyb), s)
             else:
                 _conv_call('wgrad', fl, 'og_conv3d_wgrad', dyb.data_ptr(), cpad, xin.data_ptr(), cin, g.data_ptr(), g.shape[1],
-                           kt, kh, kw, pt, ph, pw, dims[0], dims[1], dims[2], dims[3], s)
+                           kt, kh, kw, pt, ph, pw, dims[0], dims[1], dims[2], dims[3], *_scratch(dyb), s)
             return g[:cout]
 
         Cp = geom.cin_pad
@@ -536,7 +557,8 @@ class _Conv3dFn(torch.autograd.Function):
                 g = _zeros((rows, geom.ntaps * Cp), f32, dev)
                 _conv_call('wgrad', 2.0 * B * To * Ho * Wo * cout * geom.k_main,
                            'og_conv3d_strided_wgrad', dyb.data_ptr(), cpad, xs.data_ptr(), Cp, g.data_ptr(), g.shape[1],
-                           geom.kt, geom.kh, geom.kw, geom.st, geom.sh, geom.sw, geom.pt, geom.ph, geom.pw, B, T, H, W, s)
+                           geom.kt, geom.kh, geom.kw, geom.st, geom.sh, geom.sw, geom.pt, geom.ph, geom.pw, B, T, H, W,
+                           *_scratch(dyb), s)
                 dw = g[:cout].view(cout, geom.kt, geom.kh, geom.kw, Cp)[..., :C].permute(0, 4, 1, 2, 3)
         else:
             col = xs
@@ -609,7 +631,7 @@ class _GroupNormActFn(torch.autograd.Function):
         dyb = _as_bf16_rows(dy, C, C)
         S = _zeros((B, C, 2), f32, dev)
         _lib.call('og_affine_act_bwd_reduce', dyb.data_ptr(), xi.data_ptr(), A.data_ptr(), Bc.data_ptr(), act,
-                  S.data_ptr(), B, V, C, s)
+                  S.data_ptr(), B, V, C, *_scratch(dyb), s)
         dgamma = _zeros(C, f32, dev) if gamma is not None else None
         dbeta = _zeros(C, f32, dev) if beta is not None else None
         dcs = torch.empty((B, C), dtype=f32, device=dev) if has_cs else None
@@ -619,7 +641,7 @@ class _GroupNormActFn(torch.autograd.Function):
             dx = empty_internal(B, C, T, H, W, bf16, dev)
             _lib.call('og_gn_act_bwd', dyb.data_ptr(), xi.data_ptr(), A.data_ptr(), Bc.data_ptr(), S.data_ptr(),
                       mr.data_ptr(), _ptr(gamma), _ptr(beta), _ptr(cs), G, act, None, dx.data_ptr(), _ptr(dgamma),
-                      _ptr(dbeta), _ptr(dcs), _ptr(dcsh), None, B, V, C, s)
+                      _ptr(dbeta), _ptr(dcs), _ptr(dcsh), None, B, V, C, *_scratch(dyb), s)
             return dx, dgamma, dbeta, dcs, dcsh, None, None, None
         Q = torch.empty((B, C), dtype=f32, device=dev)
         R = torch.empty((B, C), dtype=f32, device=dev)
@@ -1087,14 +1109,15 @@ class _FfnFn(torch.autograd.Function):
                    W, C, ws.data_ptr(), ws.numel(), x.data_ptr(), A.data_ptr(), Bc.data_ptr(), 0, S.data_ptr(), s)
         g = _zeros((C, geom.ntaps * C), f32, dev)
         _conv_call('wgrad', 2.0 * B * V * C * geom.k_main, 'og_conv3d_wgrad', dy.data_ptr(), C, hn.data_ptr(), C,
-                   g.data_ptr(), g.shape[1], geom.kt, geom.kh, geom.kw, geom.pt, geom.ph, geom.pw, B, T, H, W, s)
+                   g.data_ptr(), g.shape[1], geom.kt, geom.kh, geom.kw, geom.pt, geom.ph, geom.pw, B, T, H, W,
+                   *_scratch(dy), s)
         dw = g.view(C, geom.kt, geom.kh, geom.kw, C).permute(0, 4, 1, 2, 3)
         dgw = _zeros(C, f32, dev)
         dgb = _zeros(C, f32, dev)
         dx = torch.empty_like(x)
         _lib.call('og_gn_act_bwd', dh.data_ptr(), x.data_ptr(), A.data_ptr(), Bc.data_ptr(), S.data_ptr(), mr.data_ptr(),
                   gn_w.data_ptr(), gn_b.data_ptr(), None, G, 0, dy.data_ptr(), dx.data_ptr(), dgw.data_ptr(),
-                  dgb.data_ptr(), None, None, None, B, V, C, s)
+                  dgb.data_ptr(), None, None, None, B, V, C, *_scratch(dy), s)
         return dx, dgw, dgb, dw, None, None, None, None
 
 
@@ -1292,11 +1315,12 @@ class _ResBlockFn(torch.autograd.Function):
             gr = _zeros((cout, g.ntaps * cin), f32, dev)
             if dbias is None:
                 _conv_call('wgrad', 2.0 * B * V * cout * cin * g.ntaps, 'og_conv3d_wgrad', dyt.data_ptr(), cout,
-                           xin.data_ptr(), cin, gr.data_ptr(), gr.shape[1], g.kt, g.kh, g.kw, g.pt, g.ph, g.pw, B, T, H, W, s)
+                           xin.data_ptr(), cin, gr.data_ptr(), gr.shape[1], g.kt, g.kh, g.kw, g.pt, g.ph, g.pw, B, T, H, W,
+                           *_scratch(dyt), s)
             else:       # + the bias gradient (column sums of dy) out of the same tensor-core pass
                 _conv_call('wgrad', 2.0 * B * V * cout * cin * g.ntaps, 'og_conv3d_wgrad_bias', dyt.data_ptr(), cout,
                            xin.data_ptr(), cin, gr.data_ptr(), gr.shape[1], g.kt, g.kh, g.kw, g.pt, g.ph, g.pw, B, T, H, W,
-                           dbias.data_ptr(), cout, s)
+                           dbias.data_ptr(), cout, *_scratch(dyt), s)
             return gr.view(cout, g.kt, g.kh, g.kw, cin).permute(0, 4, 1, 2, 3)
 
         gone = ConvGeom(C0, C1, (1, 1, 1))
@@ -1341,7 +1365,7 @@ class _ResBlockFn(torch.autograd.Function):
         if not grouped:
             if not FUSE_RED:
                 _lib.call('og_affine_act_bwd_reduce', d_a1.data_ptr(), xi.data_ptr(), A1.data_ptr(), B1.data_ptr(), act,
-                          S1.data_ptr(), B, V, C0, s)
+                          S1.data_ptr(), B, V, C0, *_scratch(d_a1), s)
             shortcut_dgrad()
         # (the input gradient is always produced: its pass is also what emits dgamma1 / dbeta1)
         dx = empty_internal(B, C0, T, H, W, bf16, dev)

@@ -1,4 +1,4 @@
-"""VideoTokenizer — the reference's Lightning surface (genie/tokenizer.py:225-442) on the B200 hot path.
+"""VideoTokenizer — the reference's Lightning surface (genie/tokenizer.py:225-442) on the H100 hot path.
 
 Same constructor signature, blueprints, method names, return tuples, logged metric keys and state_dict
 keys, including the GAN (frame critic, hinge losses) and perceptual (VGG16 feature distance) terms of

@@ -1,5 +1,5 @@
 """Minimal stand-in for the `lightning` package (not installed in this image) so the UNMODIFIED
-reference at /root/reference can be imported by oracle/make_golden.py. Test infrastructure only."""
+reference checkout can be imported by oracle/make_golden.py. Test infrastructure only."""
 import torch.nn as nn
 
 

@@ -14,7 +14,7 @@ What this is
 
 Pinning
     The reference's own tests hold no value-level vectors (SURVEY.md §4), so this oracle is pinned
-    against outputs of the reference itself, imported from /root/reference in the build container by
+    against outputs of the reference itself, imported from a checkout of the reference by
     oracle/make_golden.py; the resulting vectors are committed under tests/golden/ and checked by
     tests/test_oracle_golden.py (CPU).  Parity status: PINNED against reference outputs.
 """

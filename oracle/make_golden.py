@@ -1,6 +1,6 @@
 """oracle/make_golden.py — generate tests/golden/*.pt by RUNNING THE REAL REFERENCE.   TEST INFRASTRUCTURE.
 
-Run in the build container only (needs /root/reference, which does not exist on the GPU box):
+Run where a checkout of the reference exists (OPEN_GENIE_REFERENCE, default ../open-genie next to this repository):
 
     python oracle/make_golden.py            # writes tests/golden/*.pt, asserts oracle == reference
 
@@ -21,7 +21,7 @@ import torch.nn as nn
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 sys.path.insert(0, os.path.join(HERE, '_shim'))
-sys.path.insert(0, '/root/reference')
+sys.path.insert(0, os.environ.get('OPEN_GENIE_REFERENCE', os.path.join(os.path.dirname(ROOT), 'open-genie')))
 sys.path.insert(0, ROOT)
 
 from oracle import fixtures as fx          # noqa: E402

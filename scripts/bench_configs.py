@@ -1,4 +1,4 @@
-"""Timing of BASELINE.json's parity-test configurations on one B200 (not bench.py lines): configs[0] tokenize()+decode(),
+"""Timing of BASELINE.json's parity-test configurations on one GPU (not bench.py lines): configs[0] tokenize()+decode(),
 configs[2] LatentAction, configs[3] DynamicsModel, configs[4] Genie training steps — whole-step CUDA-event times plus a
 per-kernel table (CUDA events around every C-ABI call; tensor-core kernels with their algorithmic TFLOP/s).
 

@@ -28,12 +28,13 @@ T = N * V * C * 2
 sums = torch.zeros(N, G, 2, dtype=torch.float64, device=dev)
 S = torch.zeros(N, C, 2, device=dev)
 dg = torch.zeros(C, device=dev); db = torch.zeros(C, device=dev); cs = torch.zeros(C, device=dev)
+ws = torch.empty(64 << 20, dtype=torch.uint8, device=dev)   # partial sums of the reproducible reductions
 timeit('gn_stats', lambda i: _lib.call('og_gn_stats', xs[i].data_ptr(), N, V, C, G, sums.data_ptr(), s), T)
 timeit('gn_act_fwd', lambda i: _lib.call('og_gn_act_fwd', xs[i].data_ptr(), sums.data_ptr(), gamma.data_ptr(), beta.data_ptr(), None, None, 1e-5, G, 1, outs[i].data_ptr(), A.data_ptr(), Bc.data_ptr(), mr.data_ptr(), N, V, C, s), 2 * T)
 A.normal_(); Bc.normal_(); mr.uniform_(0.5, 1.5)
-timeit('bwd_reduce', lambda i: _lib.call('og_affine_act_bwd_reduce', dys[i].data_ptr(), xs[i].data_ptr(), A.data_ptr(), Bc.data_ptr(), 1, S.data_ptr(), N, V, C, s), 2 * T)
-timeit('gn_act_bwd', lambda i: _lib.call('og_gn_act_bwd', dys[i].data_ptr(), xs[i].data_ptr(), A.data_ptr(), Bc.data_ptr(), S.data_ptr(), mr.data_ptr(), gamma.data_ptr(), beta.data_ptr(), None, G, 1, None, outs[i].data_ptr(), dg.data_ptr(), db.data_ptr(), None, None, None, N, V, C, s), 3 * T)
-timeit('gn_act_bwd +add +colsum', lambda i: _lib.call('og_gn_act_bwd', dys[i].data_ptr(), xs[i].data_ptr(), A.data_ptr(), Bc.data_ptr(), S.data_ptr(), mr.data_ptr(), gamma.data_ptr(), beta.data_ptr(), None, G, 1, adds[i].data_ptr(), outs[i].data_ptr(), dg.data_ptr(), db.data_ptr(), None, None, cs.data_ptr(), N, V, C, s), 4 * T)
+timeit('bwd_reduce', lambda i: _lib.call('og_affine_act_bwd_reduce', dys[i].data_ptr(), xs[i].data_ptr(), A.data_ptr(), Bc.data_ptr(), 1, S.data_ptr(), N, V, C, ws.data_ptr(), ws.numel(), s), 2 * T)
+timeit('gn_act_bwd', lambda i: _lib.call('og_gn_act_bwd', dys[i].data_ptr(), xs[i].data_ptr(), A.data_ptr(), Bc.data_ptr(), S.data_ptr(), mr.data_ptr(), gamma.data_ptr(), beta.data_ptr(), None, G, 1, None, outs[i].data_ptr(), dg.data_ptr(), db.data_ptr(), None, None, None, N, V, C, ws.data_ptr(), ws.numel(), s), 3 * T)
+timeit('gn_act_bwd +add +colsum', lambda i: _lib.call('og_gn_act_bwd', dys[i].data_ptr(), xs[i].data_ptr(), A.data_ptr(), Bc.data_ptr(), S.data_ptr(), mr.data_ptr(), gamma.data_ptr(), beta.data_ptr(), None, G, 1, adds[i].data_ptr(), outs[i].data_ptr(), dg.data_ptr(), db.data_ptr(), None, None, cs.data_ptr(), N, V, C, ws.data_ptr(), ws.numel(), s), 4 * T)
 timeit('colsum', lambda i: _lib.call('og_colsum', dys[i].data_ptr(), N * V, C, C, cs.data_ptr(), s), T)
 y = torch.empty(N, V, C, device=dev, dtype=torch.bfloat16)
 timeit('torch copy (ref)', lambda i: outs[i].copy_(xs[i]), 2 * T)

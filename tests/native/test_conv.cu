@@ -1,5 +1,5 @@
-// test_conv.cu — GPU self-test of the tcgen05 conv kernels against naive CUDA-core reference kernels
-// (same bf16 inputs, fp32 accumulation). Run on a B200:  tests/native/bin/test_conv
+// test_conv.cu — GPU self-test of the wgmma conv kernels against naive CUDA-core reference kernels
+// (same bf16 inputs, fp32 accumulation). Run on an H100:  tests/native/bin/test_conv
 // This is test infrastructure; the Python parity tests (tests/test_conv_gpu.py) compare against the oracle.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -23,6 +23,8 @@
 
 static void* g_ws = nullptr;
 static size_t g_ws_bytes = 0;
+static void* g_scratch = nullptr;       // weight-gradient split-K slabs
+static size_t g_scratch_bytes = 0;
 static uint32_t g_seed = 12345;
 static float frand() {
   g_seed = g_seed * 1664525u + 1013904223u;
@@ -292,7 +294,7 @@ static bool run_case(const Case& c, bool do_dgrad, bool do_wgrad) {
       CK(cudaMemset(db, 0, c.cout * 4));
       CK(cudaMemset(dbr, 0, c.cout * 4));
       r = og_conv3d_wgrad_bias(dy, c.cout, x0, c.c0, dw, (int64_t)ntaps * c.c0, c.kt, c.kh, c.kw, c.pt, c.ph, c.pw, c.N, c.T,
-                               c.H, c.W, db, c.cout, 0);
+                               c.H, c.W, db, c.cout, g_scratch, g_scratch_bytes, 0);
       if (r == 0) r = og_colsum(dy, V, c.cout, c.cout, dbr, 0);
       if (r == 0) {
         CK(cudaDeviceSynchronize());
@@ -361,7 +363,7 @@ static void bench_case(const Case& c, int iters) {
                             c.W, c.c0, g_ws, g_ws_bytes, nullptr, nullptr, nullptr, 0, nullptr, 0);
       else
         r = og_conv3d_wgrad(dy, c.cout, x0, c.c0, dw, (int64_t)ntaps * c.c0, c.kt, c.kh, c.kw, c.pt, c.ph, c.pw, c.N,
-                            c.T, c.H, c.W, 0);
+                            c.T, c.H, c.W, g_scratch, g_scratch_bytes, 0);
       if (r) {
         printf("bench launch failed: %s\n", og_last_error());
         return;
@@ -387,6 +389,8 @@ int main(int argc, char** argv) {
   printf("device: %s sm_%d%d SMs=%d\n", prop.name, prop.major, prop.minor, prop.multiProcessorCount);
   g_ws_bytes = (size_t)256 << 20;
   CK(cudaMalloc(&g_ws, g_ws_bytes));
+  g_scratch_bytes = (size_t)64 << 20;
+  CK(cudaMalloc(&g_scratch, g_scratch_bytes));
   bool quick = argc > 1 && !strcmp(argv[1], "quick");
   std::vector<Case> cases = {
       // N  T  H   W   c0   c1  cout kt kh kw pt ph pw bias
@@ -403,8 +407,8 @@ int main(int argc, char** argv) {
       {1, 1, 1, 16384, 128, 0, 64, 1, 1, 1, 0, 0, 0, true},  // flattened im2col GEMM view (1,1,1,M)
       {1, 1, 1, 4100, 128, 0, 64, 1, 1, 1, 0, 0, 0, false},  // M not a multiple of the tile: partial boxes
       {3, 4, 8, 8, 64, 0, 128, 3, 3, 3, 1, 1, 1, true},      // odd batch with 2-row-block tiles
-      {1, 2, 16, 16, 64, 0, 320, 1, 1, 1, 0, 0, 0, true},    // Cout = 320: partial last 256-wide N tile, bf16 fast store
-      {8, 16, 64, 64, 64, 64, 64, 3, 3, 3, 1, 1, 1, true},   // enough tiles for the 256-row (m_sub = 2) path
+      {1, 2, 16, 16, 64, 0, 320, 1, 1, 1, 0, 0, 0, true},    // Cout = 320: partial last 128-wide N tile, bf16 fast store
+      {8, 16, 64, 64, 64, 64, 64, 3, 3, 3, 1, 1, 1, true},   // full tokenizer size: many persistent tiles per CTA
   };
   bool all_ok = true;
   const bool bench_only = argc > 1 && !strcmp(argv[1], "benchonly");

@@ -1,73 +1,63 @@
-"""Data path (SURVEY.md §8 f4): Platformer2D / LightningPlatformer2D against the reference's own classes on mp4 files
-written here with OpenCV (CPU), and the device-side frame decode + prefetcher (GPU)."""
+"""Data path (SURVEY.md §8 f4): Platformer2D / LightningPlatformer2D against what the reference's own classes returned for
+the same mp4 files (stored under tests/golden/platformer/, the reference's outputs as SHA-256 digests in
+tests/golden/data_path.json; both written by oracle/make_golden_data_path.py), and the device-side frame decode +
+prefetcher (GPU)."""
+import hashlib
+import json
 import os
-import sys
 
-import numpy as np
 import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+GOLDEN = os.path.join(ROOT, 'tests', 'golden', 'data_path.json')
+CLIPS = os.path.join(ROOT, 'tests', 'golden', 'platformer')   # Coinrun/{train,val,test}/clip*.mp4, 64 x 64 frames
+
+
+def digest(t):
+    return hashlib.sha256(t.contiguous().numpy().tobytes()).hexdigest()
 
 
 @pytest.fixture(scope='module')
-def clips(tmp_path_factory):
-    cv2 = pytest.importorskip('cv2')
-    root = tmp_path_factory.mktemp('platformer')
-    rng = np.random.default_rng(0)
-    for split, n in (('train', 5), ('val', 2), ('test', 2)):
-        d = root / 'Coinrun' / split
-        d.mkdir(parents=True)
-        for i in range(n):
-            w = cv2.VideoWriter(str(d / f'clip{i}.mp4'), cv2.VideoWriter_fourcc(*'mp4v'), 15, (64, 64))
-            assert w.isOpened()
-            base = rng.integers(0, 255, (8, 8, 3))
-            for t in range(12 if i == 0 else 20):          # clip0 is SHORTER than num_frames = 16
-                frame = np.kron((base + 9 * t) % 256, np.ones((8, 8, 1))).astype(np.uint8)
-                w.write(frame)
-            w.release()
-    return str(root)
-
-
-def _reference_classes():
-    """The reference's own dataset classes, when the reference is reachable (build container / vendored copy)."""
-    for cand in ('/root/reference', os.path.join(ROOT, 'baseline', '_ref')):
-        if os.path.isdir(os.path.join(cand, 'genie')):
-            for p in (os.path.join(ROOT, 'oracle', '_shim'), cand):
-                if p not in sys.path:
-                    sys.path.insert(0, p)
-            from genie.module.data import Platformer2D            # noqa
-            from genie.dataset import LightningPlatformer2D       # noqa
-            return Platformer2D, LightningPlatformer2D
-    return None, None
+def clips():
+    pytest.importorskip('cv2')
+    return CLIPS
 
 
 def test_platformer2d_matches_the_reference_dataset(clips):
     import open_genie_b200 as og
-    RefP, RefL = _reference_classes()
+    with open(GOLDEN) as f:
+        ref = json.load(f)
     for fmt in ('t c h w', 'c t h w'):
         for padding in ('none', 'repeat', 'zero'):
             ds = og.Platformer2D(clips, split='train', padding=padding, num_frames=16, output_format=fmt)
             assert len(ds) == 5
-            v = ds[1]
+            v = ds[[n.endswith('clip1.mp4') for n in ds.file_names].index(True)]   # a full-length clip, by name
             shape = (16, 3, 64, 64) if fmt == 't c h w' else (3, 16, 64, 64)
             assert v.shape == shape and v.dtype == torch.float32 and 0.0 <= float(v.min()) and float(v.max()) <= 1.0
             short = [ds[i] for i in range(5) if ds.file_names[i].endswith('clip0.mp4')][0]
             assert short.shape[0 if fmt == 't c h w' else 1] == 12        # whole (shorter) video: data.py:191-193
-            if RefP is not None:
-                rds = RefP(clips, split='train', padding=padding, num_frames=16, output_format=fmt)
-                assert rds.file_names == ds.file_names
-                for i in range(len(ds)):
-                    assert torch.equal(ds[i], rds[i])                          # bit-identical CPU tensors
-    raw = og.Platformer2D(clips, split='val', num_frames=16, raw_uint8=True)[0]
+            r = ref[f'{fmt}|{padding}']   # keyed by file name: directory listing order differs between file systems
+            want = {n: (shp, h) for n, shp, h in zip(r['file_names'], r['shapes'], r['sha256'])}
+            names = [os.path.basename(n) for n in ds.file_names]
+            assert sorted(names) == sorted(want)
+            for i, n in enumerate(names):
+                assert (list(ds[i].shape), digest(ds[i])) == want[n], n                # bit-identical tensors
+    # directory listing order depends on the file system: pick the full-length clip by name
+    raw_ds = og.Platformer2D(clips, split='val', num_frames=16, raw_uint8=True)
+    i = [n.endswith('clip1.mp4') for n in raw_ds.file_names].index(True)
+    raw = raw_ds[i]
     assert raw.dtype == torch.uint8 and raw.shape == (16, 64, 64, 3)
-    ref = og.Platformer2D(clips, split='val', num_frames=16, output_format='t h w c')[0]
-    assert torch.equal(raw.flip(-1).float() / 255., ref)                       # raw frames are BGR
+    rgb = og.Platformer2D(clips, split='val', num_frames=16, output_format='t h w c')[i]
+    assert torch.equal(raw.flip(-1).float() / 255., rgb)                       # raw frames are BGR
 
 
 def test_lightning_datamodule_surface(clips, tmp_path):
     import open_genie_b200 as og
-    dm = og.LightningPlatformer2D(clips, num_frames=16, output_format='c t h w', batch_size=2, num_workers=0)
+    # the short clip0 cannot be collated with 16-frame clips; which index it has depends on the directory listing order
+    full = [i for i, n in enumerate(og.Platformer2D(clips, split='train').file_names) if not n.endswith('clip0.mp4')]
+    dm = og.LightningPlatformer2D(clips, num_frames=16, output_format='c t h w', batch_size=2, num_workers=0,
+                                  train_sampler=full)
     dm.setup('fit')
     batch = next(iter(dm.train_dataloader()))
     assert batch.shape[0] == 2 and batch.shape[1] == 3 and batch.dtype == torch.float32

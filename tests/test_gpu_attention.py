@@ -1,4 +1,4 @@
-"""GPU parity: RoPE+LayerNorm, tcgen05 flash attention, temporal attention, SpaceTimeAttention block."""
+"""GPU parity: RoPE+LayerNorm, wgmma flash attention, temporal attention, SpaceTimeAttention block."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -67,7 +67,7 @@ def test_rope_layernorm_fwd_bwd(kind, C):
 
 
 # amp = 2 with 8 heads (scale = 1.0) gives scores of +-100: the running row maximum jumps by far more than the
-# lazy-rescale threshold (2^8) between key tiles, so the in-TMEM rescale of O is exercised, not only the first tile
+# lazy-rescale threshold (2^8) between key tiles, so the rescale of the O accumulator is exercised, not only the first tile
 @pytest.mark.parametrize('S,nh,amp', [(64, 2, 0.5), (256, 2, 0.5), (320, 1, 0.5), (1024, 4, 0.5), (640, 8, 2.0)])
 def test_flash_attention_fwd_bwd(S, nh, amp):
     nseq, C = 3, 64 * nh
@@ -98,8 +98,8 @@ def test_flash_attention_fwd_bwd(S, nh, amp):
         assert rel_l2(got.float().cpu(), ref) < 2e-2, (name, rel_l2(got.float().cpu(), ref))
 
 
-# Many more work items than SMs with ODD tile counts per item (1, 3, 5): every persistent CTA walks several items, so the
-# running-counter barrier parities of og_flash_attn_fwd2 / bwd3 cross item boundaries on both phases of every barrier.
+# Many more work items than SMs with ODD 64-row tile counts per item (1, 5, 10): thousands of CTAs, ragged last tiles,
+# and both phases of the two-stage TMA ring's barriers.
 # Reference: torch's SDPA in fp32 on the GPU (the small cases above pin the kernels to the CPU oracle values).
 @pytest.mark.parametrize('S,nseq,nh', [(64, 200, 2), (320, 120, 1), (640, 40, 2)])
 def test_flash_attention_many_items_per_cta(S, nseq, nh):

@@ -339,12 +339,10 @@ def test_mse_loss_and_layout_roundtrip():
     assert torch.equal(ops.to_reference(ops.to_internal(x.to(DEV))).cpu(), x)
 
 
-def test_operand_swapped_gemm_matches_plain_tiles(monkeypatch):
-    """Cout = 128 layers with >= 2 x #SM voxel tiles run the operand-swapped GEMM (D^T = W . X^T, transposing
-    epilogue). At the full tokenizer size (8 x 16 x 64 x 64, C = 128) its output, fused GroupNorm statistics and
-    data gradient must equal those of the plain 128 x 128 tile path (OG_IGEMM_SWAP=0): same k order, same fp32
-    accumulation, so bit-exact bf16 — and a small corner is checked against the fp32 oracle."""
-    import torch.nn.functional as F
+def test_full_size_cout128_conv_is_deterministic_and_matches_oracle():
+    """Cout = 128 at the full tokenizer size (8 x 16 x 64 x 64, C = 128: thousands of persistent tiles per launch, fused
+    GroupNorm statistics, MN-major data gradient). Two runs give bit-identical output and data gradient (fixed k order,
+    no atomics on this path), and a small corner is checked against the fp32 oracle."""
     from open_genie_b200.module.video import CausalConv3d
     from open_genie_b200 import ops
     torch.manual_seed(0)
@@ -360,7 +358,6 @@ def test_operand_swapped_gemm_matches_plain_tiles(monkeypatch):
         return y.detach().float(), xin.grad.detach().float()
 
     y1, dx1 = run()
-    monkeypatch.setenv('OG_IGEMM_SWAP', '0')
     y0, dx0 = run()
     assert torch.equal(y1, y0), (y1 - y0).abs().max().item()
     assert torch.equal(dx1, dx0), (dx1 - dx0).abs().max().item()
@@ -370,7 +367,7 @@ def test_operand_swapped_gemm_matches_plain_tiles(monkeypatch):
     xc = bf16_round(ops.to_reference(xi[:1, :, :4, :10, :10].float()).cpu())
     yo = O.causal_conv3d(xc, w, b)[:, :, :, :8, :8]
     got = ops.to_reference(y1[:1, :, :4, :8, :8]).cpu()
-    assert_close(got, bf16_round(yo), BF16_ULP, BF16_ULP * yo.abs().max().item(), 'swapped GEMM corner vs oracle')
+    assert_close(got, bf16_round(yo), BF16_ULP, BF16_ULP * yo.abs().max().item(), 'full-size conv corner vs oracle')
 
 
 def test_zero_arena_gradients_match_plain_allocation():

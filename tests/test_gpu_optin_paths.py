@@ -1,7 +1,6 @@
 """The opt-in kernel paths read their switches once per process, so they are exercised by re-running the relevant parity
-tests in a child process with the switch set: conv3d split-K variants (in-kernel finish, round-1 atomic form) and the
-dynamic tile scheduler against the convolution / tokenizer tests; the flash-attention backward variants (first
-un-pipelined version, 16 softmax warps, no exp / dS interleave, one CTA per work item) against the attention tests."""
+tests in a child process with the switch set: conv3d split-K variants (in-kernel finish, single atomic slab) and the
+dynamic tile scheduler against the convolution / tokenizer tests."""
 import os
 import subprocess
 import sys
@@ -10,7 +9,6 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CONV_TESTS = ['tests/test_gpu_layers.py', 'tests/test_gpu_tokenizer.py']
-ATTN_TESTS = ['tests/test_gpu_attention.py']
 
 
 def _rerun(tests, switch):
@@ -26,9 +24,3 @@ def _rerun(tests, switch):
 def test_conv_parity_with_optin_switch(switch):
     _rerun(CONV_TESTS, switch)
 
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('switch', ['OG_FLASH_BWD_V1=1', 'OG_FLASH_BWD_WARPS=16', 'OG_FLASH_BWD_INTERLEAVE=0',
-                                    'OG_FLASH_BWD_PERSISTENT=0', 'OG_FLASH_FWD_PERSISTENT=2', 'OG_FLASH_FWD_PERSISTENT=0'])
-def test_attention_parity_with_optin_switch(switch):
-    _rerun(ATTN_TESTS, switch)

@@ -1,5 +1,5 @@
 """CPU: the oracle (oracle/genie_oracle.py) against the golden vectors produced by the REAL reference
-(oracle/make_golden.py, run in the build container where /root/reference exists). This is what pins the
+(oracle/make_golden.py, run where a checkout of the reference exists). This is what pins the
 oracle; the GPU tests then compare the CUDA path with the oracle and with the same vectors."""
 import torch
 
