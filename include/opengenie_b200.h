@@ -102,14 +102,15 @@ int og_conv3d_dgrad(const void* dy, int cout, int w_rows, const void* w, int ldw
  *   dw[co][tap][ci] += sum_{n,t,h,w} dy[n,t,h,w,co] * x[n, t+it-pt, h+ih-ph, w+iw-pw, ci]
  * dy: bf16 [N,T,H,W,cout]; x: bf16 [N,T,H,W,cin] (cin % 64 == 0); dw: fp32, row stride ld_dw elements,
  * tap-major / channel-minor inside a row (the channels_last_3d order of the torch weight).
- * workspace (may be NULL): fp32 scratch for split-K — one [cout][taps*cin] (+ bias) partial per split, added in split
- * order, so the result is the same every run; the split count shrinks to what fits (none without a workspace). */
+ * workspace (may be NULL): fp32 scratch for the stream-K split over the SMs — up to two 128 x 256 partial tiles
+ * (+ 128 bias partials) per SM, added in k order, so the result is the same every run; with less workspace the split
+ * shrinks to what fits (whole tiles per CTA without a workspace). */
 int og_conv3d_wgrad(const void* dy, int cout, const void* x, int cin, float* dw, int64_t ld_dw, int kt, int kh,
                     int kw, int pt, int ph, int pw, int N, int T, int H, int W, void* workspace,
                     size_t workspace_bytes, og_stream_t stream);
 /* og_conv3d_wgrad + the bias gradient of the same nn.Conv3d in one launch: dbias[c] += sum over voxels of dy[v][c] for
  * c < n_bias (1 <= n_bias <= cout; caller zeroes dbias). The sums come out of the same tensor-core pass (an extra N = 16
- * product against a tile of ones in the last filter-tap group). Replaces the bias half of autograd's conv3d backward
+ * product against a tile of ones in the tiles that hold the first columns). Replaces the bias half of autograd's conv3d backward
  * (genie/module/video.py:178-192, 609-629). */
 int og_conv3d_wgrad_bias(const void* dy, int cout, const void* x, int cin, float* dw, int64_t ld_dw, int kt, int kh,
                          int kw, int pt, int ph, int pw, int N, int T, int H, int W, float* dbias, int n_bias,
@@ -122,7 +123,8 @@ int og_conv3d_wgrad_bias(const void* dy, int cout, const void* x, int cin, float
  *   dgrad: input position i only receives taps == (i+pad) mod s, so the input grid splits into st*sh*sw residue
  *          classes; each is a stride-1 implicit GEMM over dy with its tap subset, stored at stride s into dx
  *          (st*sh*sw launches, no col2im, no atomics).
- *   wgrad: dY boxes on the output grid, x boxes strided on the input grid; ACCUMULATES into dw.
+ *   wgrad: dY boxes on the output grid, x boxes strided on the input grid; ACCUMULATES into dw; workspace as
+ *          og_conv3d_wgrad.
  * x / dx: bf16 [N,T,H,W,cin] (cin % 64 == 0); out: [N,To,Ho,Wo,cout]; dy: bf16 [N,To,Ho,Wo,cout] with cout % 64 == 0
  * (zero padded by the caller; w_rows = real weight rows); w: packed bf16 [cout][ldw] as for og_conv3d_fwd. */
 int og_conv3d_strided_fwd(const void* x, int cin, int kt, int kh, int kw, int st, int sh, int sw, int pt, int ph, int pw,

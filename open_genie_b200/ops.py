@@ -142,7 +142,7 @@ class StepScope:
     SCRATCH_BYTES = 64 << 20
 
     def scratch(self, dev):
-        """Scratch for the reproducible reductions (weight-gradient split-K slabs, GroupNorm backward partials): every
+        """Scratch for the reproducible reductions (weight-gradient partial tiles, GroupNorm backward partials): every
         use is stream-ordered and complete inside one C-ABI call; the kernels limit their split to what fits."""
         t = self.scratch_bufs.get(dev)
         if t is None:
