@@ -62,23 +62,13 @@ uint64_t og_launch_count(void);
  * residual: optional bf16 [N,T,H,W,cout] added in fp32 before the output rounding (the `ffn(x) + x` skip of
  * SpaceTimeAttention, attention.py:472).
  * Reads outside [0,T)x[0,H)x[0,W) are zero (pad_mode='constant').
- * workspace (optional, may be NULL): N*T*H*W*cout fp32 of scratch enables split-K for problems whose tiles
- * cannot fill the 132 SMs (small T*H*W, deep K); without it the same result is computed unsplit. With room for one
- * such slab per split (20 MB always suffices) every split stores its partial tile with plain stores and the finish pass
- * adds the slabs (and emits gn_sums); a smaller workspace is zeroed and reduced into with red.global.add.
+ * workspace (optional, may be NULL): fp32 scratch that enables split-K for problems whose tiles cannot fill the
+ * 132 SMs (small T*H*W, deep K). Every split stores its partial sums into its own slab of N*T*H*W*cout floats, and a
+ * finish pass adds the slabs in split order (and emits gn_sums), so the result is the same every run. The split
+ * shrinks to the slabs that fit (20 MB always suffices); with room for fewer than two it runs unsplit.
  * gn_sums (optional): fp64 [N][2] += (sum, sum of squares) of the bf16 output per sample — the og_gn_stats
  * result for a following GroupNorm(1, C) — produced in the GEMM epilogue when the tiling allows it, otherwise
  * by an internal og_gn_stats pass; either way the caller just zeroes it first. */
-/* workspace protocol (og_conv3d_fwd / og_conv3d_dgrad). A workspace PREPARED with og_workspace_init (call it once after
- * allocating the buffer; it zeroes the buffer and reserves its last 4096 bytes for self-resetting counters) enables
- *   - with OG_SPLITK_FUSED=1, the in-kernel split-K finish: the last of a tile's split items to arrive reads the tile's
- *     partial sums back, adds the bias, rounds, stores, emits the GroupNorm sums and re-zeroes its part of the workspace —
- *     no memset, no finish launch, no statistics pass (an experiment: 98 fewer launches per step but 1-1.7 ms slower);
- *   - with OG_IGEMM_DYNAMIC=1, dynamic tile scheduling for the persistent CTAs (an experiment: no measurable gain).
- * An unprepared workspace gets the classic memset + partial sums + finish launch; NULL disables split-K. Results are
- * identical up to the order of fp32 additions. Do not write to a prepared workspace from outside these calls. */
-int og_workspace_init(void* workspace, size_t workspace_bytes, og_stream_t stream);
-
 int og_conv3d_fwd(const void* x0, int c0, int kt, int kh, int kw, int pt, int ph, int pw, const void* x1, int c1,
                   const void* w, int ldw, const float* bias0, const float* bias1, const void* residual, void* out,
                   int out_f32, int N, int T, int H, int W, int cout, void* workspace, size_t workspace_bytes,
@@ -90,13 +80,10 @@ int og_conv3d_fwd(const void* x0, int c0, int kt, int kh, int kw, int pt, int ph
  * dy: bf16 [N,T,H,W,cout] (cout % 64 == 0; a narrower gradient is zero-padded by the caller and
  * w_rows <= cout gives the number of real weight rows); w as above (k_off selects the segment inside
  * a packed row, k_off % 8 == 0); dx: [N,T,H,W,cin] (cin % 64 == 0), bf16 or fp32.
- * red_* (optional): when dx is the gradient of y = act(x*A + B) (a GroupNorm+SiLU fed by this conv's input),
- * red_S[n][c] += (sum_v dpre, sum_v dpre*x) with dpre = dx * act'(x*A+B) — exactly og_affine_act_bwd_reduce on
- * (dx, red_x) — is accumulated in the GEMM epilogue (or by an internal pass when the tiling does not allow it). */
+ * workspace (optional): split-K scratch as for og_conv3d_fwd, with slabs of N*T*H*W*cin floats. */
 int og_conv3d_dgrad(const void* dy, int cout, int w_rows, const void* w, int ldw, int k_off, int kt, int kh, int kw,
                     int pt, int ph, int pw, void* dx, int dx_f32, int N, int T, int H, int W, int cin,
-                    void* workspace, size_t workspace_bytes, const void* red_x, const float* red_A,
-                    const float* red_B, int red_act, float* red_S, og_stream_t stream);
+                    void* workspace, size_t workspace_bytes, og_stream_t stream);
 
 /* Weight gradient (autograd's conv3d backward-weight). ACCUMULATES into dw (caller zeroes it):
  *   dw[co][tap][ci] += sum_{n,t,h,w} dy[n,t,h,w,co] * x[n, t+it-pt, h+ih-ph, w+iw-pw, ci]
@@ -220,15 +207,6 @@ int og_ndhwc_to_ncdhw_f32(const void* x, int x_f32, float* y, int N, int C, int6
  * y: bf16 [N,T*p,H*q,W*r,c] shuffled. inverse=0 reads x writes y; inverse=1 reads y writes x (backward). */
 int og_pixel_shuffle3d(const void* x, void* y, int inverse, int N, int T, int H, int W, int c, int p, int q, int r,
                        og_stream_t stream);
-
-/* Explicit im2col for the layers the implicit-GEMM kernel does not take directly: strided
- * CausalConv3d (SpaceTimeDownsample, video.py:477-483) and Cin not a multiple of 64.
- * Causal geometry (video.py:154-164): pt is the FRONT time pad only; ph/pw are symmetric.
- * col: bf16 [N*To*Ho*Wo][kpad], k = tap*C + ci, zero beyond kt*kh*kw*C. col2im is its adjoint. */
-int og_im2col3d(const void* x, void* col, int N, int T, int H, int W, int C, int kt, int kh, int kw, int st, int sh,
-                int sw, int pt, int ph, int pw, int kpad, og_stream_t stream);
-int og_col2im3d(const void* dcol, void* dx, int dx_f32, int N, int T, int H, int W, int C, int kt, int kh, int kw,
-                int st, int sh, int sw, int pt, int ph, int pw, int kpad, og_stream_t stream);
 
 /* BlurPooling3d with num_groups == 1 (genie/module/video.py:487-537): every output channel is
  * blur_k(sum_c x[:, c]) with the normalised Pascal kernel, stride (st,sh,sw), padding (k-1)/2.

@@ -10,8 +10,6 @@
 // Spatial sequences run over (h w) of one frame, temporal ones over t of one pixel. In NDHWC memory both
 // are ROW-WISE operations on the same [B*T*H*W][C] matrix — only the position index of a row differs —
 // so no 'b c t h w -> (b h w) t c' transposition copy is ever made (the reference makes two per block).
-#include <stdlib.h>
-
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 
@@ -719,16 +717,15 @@ __global__ void __launch_bounds__(128)
   if (kv_bcast) flush();
 }
 
-// mma.sync m16n8k16 path (temporal_attn_mma.cu) for d_head = 64, T <= 16 — the default; OG_TEMPORAL_MMA=0 selects the
-// per-lane kernels below, which also cover T in (16, 32].
+// mma.sync m16n8k16 path (temporal_attn_mma.cu) for d_head = 64, T <= 16; the per-lane kernels above cover d_head = 32
+// and T in (16, 32].
 int launch_temporal_fwd_mma(const void* q, const void* k, const void* v, const void* residual, void* out, int B, int T,
                             long long P, int C, int n_head, float scale, int kv_bcast, cudaStream_t stream);
 int launch_temporal_bwd_mma(const void* q, const void* k, const void* v, const void* dout, void* dq, void* dk, void* dv,
                             float* dk_b, float* dv_b, int B, int T, long long P, int C, int n_head, float scale,
                             int kv_bcast, cudaStream_t stream);
 static bool temporal_mma_enabled(int D, int T, int C) {
-  const char* e = getenv("OG_TEMPORAL_MMA");
-  return !(e && atoi(e) == 0) && D == 64 && T <= 16 && C % 8 == 0;
+  return D == 64 && T <= 16 && C % 8 == 0;
 }
 
 static int row_grid(long long rows, int warps_per_block) {

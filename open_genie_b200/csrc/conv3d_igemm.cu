@@ -21,11 +21,6 @@
 //   warps 4-7 one warpgroup: wgmma main loop (128 x BN accumulator = two m64 halves in registers, BN <= 128),
 //             then the epilogue: registers -> fp32 tile in shared memory -> one row per thread -> (+bias) -> global.
 //             The producer keeps filling the stage ring with the next tile's operands meanwhile.
-#include <stdlib.h>
-
-#include <utility>
-#include <vector>
-
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 
@@ -69,21 +64,11 @@ struct IgemmParams {
   int num_kb;  // k-blocks per tile
   int fast_store;  // bf16 output, n_out % 64 == 0, block_n % 64 == 0: coalesced staged stores
   const __nv_bfloat16* residual;  // optional bf16 [voxels][n_out] added to the output (out = conv + bias + residual)
-  // fused epilogue reductions (fast_store path, one sample per CTA tile):
+  // fused epilogue reduction (fast_store path, one sample per CTA tile):
   double* gn_sums;             // forward: [N][2] += (sum y, sum y^2) of the bf16-rounded output (GroupNorm(1,C) statistics)
-  const __nv_bfloat16* red_x;  // data gradient: GN input x [voxels][n_out] ...
-  const float* red_A;          // ... per-(sample, channel) scale / shift of y = act(x*A+B) ...
-  const float* red_B;
-  float* red_S;                // ... S[n][c] += (sum dpre, sum dpre*x), dpre = d * act'(x*A+B)   (og_affine_act_bwd_reduce)
-  int red_act;
-  unsigned int* sched;  // dynamic tile scheduler state {magic, next item, CTAs done} in the caller's workspace, or NULL
-  int splits;      // split-K factor (1 = none): each work item covers a k-block range and reduces into `ws`
-  float* ws;       // fp32 [voxels][n_out] partial-sum workspace (zero on entry) when splits > 1
-  long long ws_slab;  // > 0: every split item STORES its partial tile into its own slab ws[split*ws_slab + ...] (no atomics,
-                      // no memset; the finish pass adds the slabs); 0: red.global.add into one zeroed slab
-  int dbg;         // timing experiments only (OG_IGEMM_DBG): 1 = skip the split-K epilogue's global writes
-  unsigned int* tile_ctr;  // per-tile arrival counters (prepared workspace): the LAST split item of a tile finishes it in-kernel
-                           // (bias, cast, store, GroupNorm sums) and re-zeroes its part of `ws` — no memset, no finish launch
+  int splits;      // split-K factor (1 = none): each work item covers a k-block range of one tile
+  float* ws;       // when splits > 1: `splits` fp32 slabs of [voxels][n_out]; every split item STORES its partial tile into
+  long long ws_slab;  // its own slab ws[split*ws_slab + ...] (no atomics, no memset) and the finish pass adds the slabs
 };
 
 
@@ -92,10 +77,8 @@ static constexpr int kBlockK = 64;                       // 64 bf16 = one 128-by
 static constexpr int kABytes = kBlockM * kBlockK * 2;    // 16 KiB
 static constexpr int kMaxStages = 8;
 static constexpr int kThreads = 256;
-static constexpr int kSchedDepth = 4;
-static constexpr unsigned int kSchedMagic = 0x0695CED0u;   // written by og_workspace_init
-// barriers (256) + bias (1024) + 4 warps x 4 KiB store staging + fused reductions (4352); the fp32 accumulator tile follows
-static constexpr int kTailBytes = 256 + 1024 + 4 * 4096 + 4352;
+// barriers (256) + bias (1024) + 4 warps x 4 KiB store staging + GroupNorm sums (256); the fp32 accumulator tile follows
+static constexpr int kTailBytes = 256 + 1024 + 4 * 4096 + 256;
 __host__ __device__ constexpr int acc_ld(int bn) { return bn + 4; }   // fp32 row stride: conflict-free float4 row reads
 
 template <int NV>
@@ -145,21 +128,9 @@ __global__ void __launch_bounds__(kThreads, 1)
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.num_stages * stage_bytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + kMaxStages;
-  // Dynamic tile scheduler. With the static `item = blockIdx.x + i * gridDim.x` assignment a CTA that cannot be
-  // resident (another kernel — the NCCL all-reduce of the data-parallel step — holds its SM; this kernel's 227 KB of
-  // shared memory exclude co-residency) starts only when a sibling CTA finishes and then still owns its full share of
-  // tiles: the launch takes ~2x as long. Here the producer warp draws work items from a global counter and hands them to
-  // the MMA / epilogue warpgroup through a 4-deep shared-memory ring, so late CTAs simply find no work left.
-  uint64_t* sched_full = bars + 2 * kMaxStages + 5;    // [4]
-  uint64_t* sched_empty = bars + 2 * kMaxStages + 9;   // [4]
-  int* sched_item = reinterpret_cast<int*>(bars + 2 * kMaxStages + 13);  // [4]
-  const bool dyn = p.sched != nullptr && p.sched[0] == kSchedMagic;
   float* bias_s = reinterpret_cast<float*>(bars + 32);                    // [256] bias0+bias1 of the current N tile
   uint8_t* stage_s = reinterpret_cast<uint8_t*>(bars + 32) + 1024;        // 4 warps x 32 rows x 128 B store staging
-  float* coef_s = reinterpret_cast<float*>(stage_s + 4 * 4096);          // [2][256] A, B of the current sample / N tile
-  float* red_s = coef_s + 512;                                            // [256][2] column sums of the current tile
-  double* stat_s = reinterpret_cast<double*>(red_s + 512);                // [2]
-  int* flag_s = reinterpret_cast<int*>(stat_s + 2);                       // [1] "this CTA finishes the tile" (fused split-K)
+  double* stat_s = reinterpret_cast<double*>(stage_s + 4 * 4096);         // [2]
   float* acc_s = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + kTailBytes);  // [128][acc_ld(BN)] fp32
 
   const int warp = warp_idx_uniform();
@@ -174,10 +145,6 @@ __global__ void __launch_bounds__(kThreads, 1)
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 4);   // one arrival per consumer warp
     }
-    for (int a = 0; a < kSchedDepth; ++a) {
-      mbar_init(&sched_full[a], 1);
-      mbar_init(&sched_empty[a], 4);   // the 4 consumer warps
-    }
     fence_mbar_init();
   }
   __syncthreads();
@@ -188,28 +155,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     {
       int stage = 0;
       uint32_t phase = 0;
-      int sslot = 0;
-      uint32_t sphase = 0;
-      for (int iter = 0;; ++iter) {
-        int item;
-        if (dyn) {
-          mbar_wait(&sched_empty[sslot], sphase ^ 1);
-          int got = 0;
-          if (elect_one()) got = (int)atomicAdd(p.sched + 1, 1u);
-          item = __reduce_max_sync(0xffffffffu, got);          // broadcast (items are >= 0)
-          if (elect_one()) {
-            sched_item[sslot] = item;
-            mbar_arrive(&sched_full[sslot]);                    // release: the slot is visible to the waiters
-          }
-          __syncwarp();
-          if (++sslot == kSchedDepth) {
-            sslot = 0;
-            sphase ^= 1;
-          }
-        } else {
-          item = blockIdx.x + iter * gridDim.x;
-        }
-        if (item >= total_tiles) break;
+      for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
         const int tile = item / p.splits, split = item - tile * p.splits;
         const int m_super = tile / p.num_n_tiles;
         const int n_tile = tile - m_super * p.num_n_tiles;
@@ -272,17 +218,6 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
       }
     }
-    __syncwarp();
-    if (dyn && elect_one()) {
-      // last CTA to finish resets the counter for the next launch that uses this workspace (stream-ordered)
-      __threadfence();
-      const unsigned int old = atomicInc(p.sched + 2, gridDim.x - 1);
-      if (old == gridDim.x - 1) {
-        __threadfence();
-        p.sched[1] = 0u;
-      }
-    }
-    __syncwarp();
   } else if (warp >= 4) {
     // ============================ wgmma main loop + epilogue (one warpgroup) ============================
     const int q = warp & 3;  // warp of the warpgroup: wgmma rows 16q..16q+15 of each m64 half; epilogue rows 32q..32q+31
@@ -291,26 +226,9 @@ __global__ void __launch_bounds__(kThreads, 1)
     int stage = 0;
     uint32_t phase = 0;
     float fl_s = 0.f, fl_ss = 0.f;
-    for (int j = et; j < 512; j += 128) red_s[j] = 0.f;
     if (et == 0) stat_s[0] = stat_s[1] = 0.0;
     asm volatile("bar.sync 1, 128;" ::: "memory");
-    int sslot = 0;
-    uint32_t sphase = 0;
-    for (int iter = 0;; ++iter) {
-      int item;
-      if (dyn) {
-        mbar_wait(&sched_full[sslot], sphase);
-        item = sched_item[sslot];
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sched_empty[sslot]);
-        if (++sslot == kSchedDepth) {
-          sslot = 0;
-          sphase ^= 1;
-        }
-      } else {
-        item = blockIdx.x + iter * gridDim.x;
-      }
-      if (item >= total_tiles) break;
+    for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
       const int tile = item / p.splits;
       const int split = item - tile * p.splits;
       const int m_super = tile / p.num_n_tiles;
@@ -381,38 +299,23 @@ __global__ void __launch_bounds__(kThreads, 1)
       const int col0 = n_tile * p.block_n;
 
       if (p.splits > 1) {
-        // split-K: add this item's partial sums into the fp32 workspace (bias / cast happen in the finish pass)
+        // split-K: store this item's partial sums into its own slab of the fp32 workspace with plain stores (each thread
+        // fills one 128-byte line of its row per chunk); bias / cast happen in the finish pass
         for (int c = 0; c < p.block_n; c += 32) {
           if (col0 + c >= p.n_out) break;
           uint32_t v[32];
           ld_acc_row<32>(acc_row + c, v);
-          if (row_ok && p.dbg != 1) {
-            if (p.ws_slab) {
-              // own slab: plain stores (each thread fills one 128-byte line of its row per chunk)
-              float* dst = p.ws + (long long)(item - tile * p.splits) * p.ws_slab + vox * p.ldo + col0 + c;
-              if (p.vec_ok && col0 + c + 32 <= p.n_out) {
+          if (row_ok) {
+            float* dst = p.ws + (long long)split * p.ws_slab + vox * p.ldo + col0 + c;
+            if (p.vec_ok && col0 + c + 32 <= p.n_out) {
 #pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                  __stcg(reinterpret_cast<float4*>(dst + j),
-                         make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                                     __uint_as_float(v[j + 3])));
-              } else {
-                for (int j = 0; j < 32; ++j)
-                  if (col0 + c + j < p.n_out) dst[j] = __uint_as_float(v[j]);
-              }
+              for (int j = 0; j < 32; j += 4)
+                __stcg(reinterpret_cast<float4*>(dst + j),
+                       make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
+                                   __uint_as_float(v[j + 3])));
             } else {
-              float* dst = p.ws + vox * p.ldo + col0 + c;
-              if (p.vec_ok && col0 + c + 32 <= p.n_out) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "f"(__uint_as_float(v[j])),
-                               "f"(__uint_as_float(v[j + 1])), "f"(__uint_as_float(v[j + 2])),
-                               "f"(__uint_as_float(v[j + 3]))
-                               : "memory");
-              } else {
-                for (int j = 0; j < 32; ++j)
-                  if (col0 + c + j < p.n_out) atomicAdd(dst + j, __uint_as_float(v[j]));
-              }
+              for (int j = 0; j < 32; ++j)
+                if (col0 + c + j < p.n_out) dst[j] = __uint_as_float(v[j]);
             }
           }
         }
@@ -433,10 +336,6 @@ __global__ void __launch_bounds__(kThreads, 1)
               if (p.bias1) b += __ldg(p.bias1 + col);
             }
             bias_s[j] = b;
-            if (p.red_S) {
-              coef_s[j] = col < p.n_out ? __ldg(p.red_A + (long long)tc.n0 * p.n_out + col) : 0.f;
-              coef_s[256 + j] = col < p.n_out ? __ldg(p.red_B + (long long)tc.n0 * p.n_out + col) : 0.f;
-            }
           }
           asm volatile("bar.sync 1, 128;" ::: "memory");
         }
@@ -469,69 +368,13 @@ __global__ void __launch_bounds__(kThreads, 1)
             v0[j] = __float_as_uint(__uint_as_float(v0[j]) + bias_s[c + j]);
             v1[j] = __float_as_uint(__uint_as_float(v1[j]) + bias_s[c + 32 + j]);
           }
-          if (p.gn_sums || p.red_S) {
-            if (p.gn_sums && row_ok) {
+          if (p.gn_sums && row_ok) {
 #pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const float r0 = __bfloat162float(__float2bfloat16_rn(__uint_as_float(v0[j])));
-                const float r1 = __bfloat162float(__float2bfloat16_rn(__uint_as_float(v1[j])));
-                st_s += r0 + r1;
-                st_ss = fmaf(r0, r0, fmaf(r1, r1, st_ss));
-              }
-            }
-            if (p.red_S) {
-              float d1[64], d2[64];
-              const uint4* xp = reinterpret_cast<const uint4*>(p.red_x + vox * p.ldo + col0 + c);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                uint4 u = make_uint4(0, 0, 0, 0);
-                if (row_ok) u = __ldg(xp + j);
-                const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 xf = __bfloat1622float2(hh[e]);
-#pragma unroll
-                  for (int q2 = 0; q2 < 2; ++q2) {
-                    const int idx = 8 * j + 2 * e + q2;
-                    const float xv = q2 ? xf.y : xf.x;
-                    const uint32_t raw = idx < 32 ? v0[idx] : v1[idx - 32];
-                    float dv = __bfloat162float(__float2bfloat16_rn(__uint_as_float(raw)));  // what bwd_apply will read
-                    if (p.red_act == 1) {
-                      const float pre = fmaf(xv, coef_s[c + idx], coef_s[256 + c + idx]);
-                      const float sg = 1.f / (1.f + __expf(-pre));
-                      dv *= sg * (1.f + pre * (1.f - sg));
-                    } else if (p.red_act >= 2) {  // LeakyReLU(0.01) / ReLU (act codes of norm_act.cu)
-                      const float pre = fmaf(xv, coef_s[c + idx], coef_s[256 + c + idx]);
-                      if (pre <= 0.f) dv *= (p.red_act == 2 ? 0.01f : 0.f);
-                    }
-                    if (!row_ok) dv = 0.f;
-                    d1[idx] = dv;
-                    d2[idx] = dv * xv;
-                  }
-                }
-              }
-              // warp transpose-reduce: afterwards lane l holds the 32-row sums of columns l and l+32
-#pragma unroll
-              for (int half = 0; half < 2; ++half) {
-#pragma unroll
-                for (int w = 0; w < 2; ++w) {
-                  float* arr = (w == 0 ? d1 : d2) + half * 32;
-#pragma unroll
-                  for (int off = 16; off >= 1; off >>= 1) {
-                    const bool up = (lane & off) != 0;
-#pragma unroll
-                    for (int j = 0; j < off; ++j) {
-                      const float send = up ? arr[j] : arr[j + off];
-                      const float keep = up ? arr[j + off] : arr[j];
-                      arr[j] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-                    }
-                  }
-                }
-              }
-              atomicAdd(&red_s[2 * (c + lane)], d1[0]);
-              atomicAdd(&red_s[2 * (c + lane) + 1], d2[0]);
-              atomicAdd(&red_s[2 * (c + 32 + lane)], d1[32]);
-              atomicAdd(&red_s[2 * (c + 32 + lane) + 1], d2[32]);
+            for (int j = 0; j < 32; ++j) {
+              const float r0 = __bfloat162float(__float2bfloat16_rn(__uint_as_float(v0[j])));
+              const float r1 = __bfloat162float(__float2bfloat16_rn(__uint_as_float(v1[j])));
+              st_s += r0 + r1;
+              st_ss = fmaf(r0, r0, fmaf(r1, r1, st_ss));
             }
           }
 #pragma unroll
@@ -618,134 +461,19 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
       }
       } while (0);
-      if (p.splits > 1 && p.tile_ctr) {
-        // ---- fused split-K finish: the last of the `splits` items of this tile to arrive reduces nothing more — all
-        // partial sums are already in `ws` (L2 reductions) — it reads the tile back, adds the bias, rounds, stores, emits
-        // the GroupNorm sums and zeroes the tile for the next launch. Replaces a memset, a finish launch and a stats pass.
-        __threadfence();
+      if (p.fast_store && p.splits == 1 && p.gn_sums) {
+        // flush this tile's GroupNorm sums (all rows of a CTA tile belong to one sample: host-checked)
+        const TileCoord tcf = decode_m_tile(p, m_super);
+        for (int o = 16; o > 0; o >>= 1) {
+          fl_s += __shfl_xor_sync(0xffffffffu, fl_s, o);
+          fl_ss += __shfl_xor_sync(0xffffffffu, fl_ss, o);
+        }
+        if (lane == 0) {
+          atomicAdd(&stat_s[0], (double)fl_s);
+          atomicAdd(&stat_s[1], (double)fl_ss);
+        }
         asm volatile("bar.sync 1, 128;" ::: "memory");
         if (et == 0) {
-          const unsigned int old = atomicAdd(p.tile_ctr + tile, 1u);
-          const int last = old == (unsigned int)(p.splits - 1);
-          if (last) p.tile_ctr[tile] = 0u;
-          flag_s[0] = last;
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (flag_s[0]) {
-          __threadfence();
-          float fs = 0.f, fss = 0.f;
-          int n_of_tile = 0;
-          // a warp walks its 32 rows one at a time, its lanes spread over the row's columns (8 per lane): every access is a
-          // coalesced 1 KB row segment (the first version gave each thread a whole row: 32 scattered 32-byte pieces per
-          // warp instruction made the finishing CTA 50 us slower than the separate finish launch it replaced)
-          {
-            const TileCoord tc = decode_m_tile(p, m_super);
-            n_of_tile = tc.n0;
-            const int col0 = n_tile * p.block_n;
-#pragma unroll 4
-            for (int rr = 0; rr < 32; ++rr) {
-              const int r = q * 32 + rr;
-              const int dw = r & ((1 << p.bw_log2) - 1);
-              const int dh = (r >> p.bw_log2) & ((1 << p.bh_log2) - 1);
-              const int dt = (r >> (p.bw_log2 + p.bh_log2)) & ((1 << p.bt_log2) - 1);
-              const int dn = r >> (p.bw_log2 + p.bh_log2 + p.bt_log2);
-              const int vn = tc.n0 + dn, vt = tc.t0 + dt, vh = tc.h0 + dh, vw = tc.w0 + dw;
-              if (!(vn < p.N && vt < p.T && vh < p.H && vw < p.W)) continue;
-              const long long vox = (((long long)vn * p.OT + vt) * p.OH + vh) * p.OW + vw;
-              for (int c = lane * 8; c < p.block_n; c += 256) {
-                const int col = col0 + c;
-                if (col >= p.n_out) break;
-                float* wp = p.ws + vox * p.ldo + col;
-                float f[8];
-                if (p.vec_ok && col + 8 <= p.n_out) {
-                  const float4 a = __ldcg(reinterpret_cast<const float4*>(wp)), b = __ldcg(reinterpret_cast<const float4*>(wp) + 1);
-                  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-                  __stcg(reinterpret_cast<float4*>(wp), make_float4(0.f, 0.f, 0.f, 0.f));
-                  __stcg(reinterpret_cast<float4*>(wp) + 1, make_float4(0.f, 0.f, 0.f, 0.f));
-                } else {
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) {
-                    f[j] = (col + j < p.n_out) ? __ldcg(wp + j) : 0.f;
-                    if (col + j < p.n_out) __stcg(wp + j, 0.f);
-                  }
-                }
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  if (col + j < p.n_out) {
-                    if (p.bias0) f[j] += __ldg(p.bias0 + col + j);
-                    if (p.bias1) f[j] += __ldg(p.bias1 + col + j);
-                  }
-                }
-                if (p.out_f32) {
-                  float* o = reinterpret_cast<float*>(p.out) + vox * p.ldo + col;
-                  if (p.vec_ok && col + 8 <= p.n_out) {
-                    *reinterpret_cast<float4*>(o) = make_float4(f[0], f[1], f[2], f[3]);
-                    *reinterpret_cast<float4*>(o + 4) = make_float4(f[4], f[5], f[6], f[7]);
-                  } else {
-                    for (int j = 0; j < 8; ++j)
-                      if (col + j < p.n_out) o[j] = f[j];
-                  }
-                } else {
-                  __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + vox * p.ldo + col;
-                  if (p.gn_sums) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                      if (col + j < p.n_out) {
-                        const float rv = __bfloat162float(__float2bfloat16_rn(f[j]));
-                        fs += rv;
-                        fss = fmaf(rv, rv, fss);
-                      }
-                  }
-                  if (p.vec_ok && col + 8 <= p.n_out) {
-                    uint4 u;
-                    u.x = pack_bf16x2(f[0], f[1]);
-                    u.y = pack_bf16x2(f[2], f[3]);
-                    u.z = pack_bf16x2(f[4], f[5]);
-                    u.w = pack_bf16x2(f[6], f[7]);
-                    *reinterpret_cast<uint4*>(o) = u;
-                  } else {
-                    for (int j = 0; j < 8; ++j)
-                      if (col + j < p.n_out) o[j] = __float2bfloat16_rn(f[j]);
-                  }
-                }
-              }
-            }
-          }
-          if (p.gn_sums) {
-            for (int o = 16; o > 0; o >>= 1) {
-              fs += __shfl_xor_sync(0xffffffffu, fs, o);
-              fss += __shfl_xor_sync(0xffffffffu, fss, o);
-            }
-            if (lane == 0) {
-              atomicAdd(&p.gn_sums[(long long)n_of_tile * 2], (double)fs);
-              atomicAdd(&p.gn_sums[(long long)n_of_tile * 2 + 1], (double)fss);
-            }
-          }
-        }
-      }
-      if (p.fast_store && p.splits == 1 && (p.gn_sums || p.red_S)) {
-        // flush this tile's fused reductions (all rows of a CTA tile belong to one sample: host-checked)
-        const TileCoord tcf = decode_m_tile(p, m_super);
-        if (p.gn_sums) {
-          for (int o = 16; o > 0; o >>= 1) {
-            fl_s += __shfl_xor_sync(0xffffffffu, fl_s, o);
-            fl_ss += __shfl_xor_sync(0xffffffffu, fl_ss, o);
-          }
-          if (lane == 0) {
-            atomicAdd(&stat_s[0], (double)fl_s);
-            atomicAdd(&stat_s[1], (double)fl_ss);
-          }
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (p.red_S) {
-          const int col0f = n_tile * p.block_n;
-          for (int j = et; j < 2 * p.block_n; j += 128) {
-            const int col = col0f + (j >> 1);
-            if (col < p.n_out) atomicAdd(&p.red_S[((long long)tcf.n0 * p.n_out + col) * 2 + (j & 1)], red_s[j]);
-            red_s[j] = 0.f;
-          }
-        }
-        if (p.gn_sums && et == 0) {
           atomicAdd(&p.gn_sums[(long long)tcf.n0 * 2], stat_s[0]);
           atomicAdd(&p.gn_sums[(long long)tcf.n0 * 2 + 1], stat_s[1]);
           stat_s[0] = 0.0;
@@ -880,23 +608,7 @@ struct IgemmLaunch {
   void* workspace = nullptr;
   size_t workspace_bytes = 0;
   double* gn_sums = nullptr;
-  const void* red_x = nullptr;
-  const float* red_A = nullptr;
-  const float* red_B = nullptr;
-  int red_act = 0;
-  float* red_S = nullptr;
 };
-
-// workspaces prepared by og_workspace_init (all zero, magic in the tail): only those may use the in-kernel split-K finish
-static std::mutex g_ws_mutex;
-static std::vector<std::pair<const void*, size_t>> g_ws_prepared;
-static bool ws_prepared(const void* p, size_t bytes) {
-  std::lock_guard<std::mutex> lock(g_ws_mutex);
-  for (const auto& e : g_ws_prepared)
-    if (e.first == p && e.second == bytes) return true;
-  return false;
-}
-static constexpr size_t kWsTail = 4096;   // [0,256): scheduler state; [256,4096): per-tile arrival counters
 
 static IgemmSeg make_seg(int cin_blocks, int kt, int kh, int kw, int pt, int ph, int pw, int sgn) {
   IgemmSeg g;
@@ -951,10 +663,6 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   p.W = W;
   p.num_m_tiles = ((N + bn - 1) / bn) * p.tiles_w * p.tiles_h * p.tiles_t;
   p.block_n = pick_block_n(n_out, L.b_mn_major != 0);
-  if (const char* e = getenv("OG_IGEMM_BN")) {  // tuning experiments only
-    const int v = atoi(e);
-    if ((v == 16 || v == 32 || v == 64 || v == 128) && (!L.b_mn_major || v >= 64)) p.block_n = v;
-  }
   p.num_n_tiles = (n_out + p.block_n - 1) / p.block_n;
   p.n_out = n_out;
   p.ldo = n_out;
@@ -966,57 +674,21 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   p.residual = reinterpret_cast<const __nv_bfloat16*>(L.residual);
   const int stage_bytes = kABytes + p.block_n * kBlockK * 2;
   p.fast_store = (!L.out_f32 && n_out % 64 == 0 && p.block_n % 64 == 0) ? 1 : 0;
-  // dynamic tile scheduling: state lives in the last 256 bytes of the caller's workspace (og_workspace_init)
-  p.sched = nullptr;
-  size_t ws_usable = L.workspace_bytes;
-  unsigned int* tile_ctr = nullptr;
-  if (L.workspace && L.workspace_bytes >= 2 * kWsTail) {
-    const size_t off = (L.workspace_bytes - kWsTail) & ~(size_t)255;
-    ws_usable = off;
-    // in-kernel split-K finish: OFF by default. It removes the memset, finish and statistics launches of every split
-    // launch, but the last arriver's fence + read-back sits on the tail of the launch instead. OG_SPLITK_FUSED=1 enables it.
-    static const bool fused_finish_on = [] {
-      const char* e = getenv("OG_SPLITK_FUSED");
-      return e && atoi(e) == 1;
-    }();
-    if (fused_finish_on && ws_prepared(L.workspace, L.workspace_bytes))
-      tile_ctr = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(L.workspace) + off + 256);
-    // Dynamic tile assignment, OFF by default: it only helps when another kernel (a data-parallel all-reduce) holds SMs
-    // while this one launches. OG_IGEMM_DYNAMIC=1 enables it.
-    static const bool dyn_on = [] {
-      const char* e = getenv("OG_IGEMM_DYNAMIC");
-      return e && atoi(e) == 1;
-    }();
-    if (dyn_on) p.sched = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(L.workspace) + off);
-  }
-  // split-K when the tiles cannot fill the machine and each has a long K loop
+  // split-K when the tiles cannot fill the machine and each has a long K loop: every split stores into its own fp32 slab
+  // of the workspace, so the split shrinks to the slabs that fit and the launch runs unsplit below two
   p.splits = 1;
-  p.ws = nullptr;
-  p.ws_slab = 0;
-  p.dbg = 0;
-  if (const char* e = getenv("OG_IGEMM_DBG")) p.dbg = atoi(e);
   if (plain) {
     const long long tiles = (long long)p.num_m_tiles * p.num_n_tiles;
-    const size_t need = (size_t)N * T * H * W * n_out * sizeof(float);
-    if (tiles * 2 <= num_sms() && p.num_kb >= 32 && L.workspace && ws_usable >= need && !L.residual) {
+    const size_t need = (size_t)N * T * H * W * n_out * sizeof(float);   // one slab
+    if (tiles * 2 <= num_sms() && p.num_kb >= 32 && L.workspace && !L.residual) {
       int sp = (int)(num_sms() / tiles);
       if (sp > p.num_kb / 8) sp = p.num_kb / 8;
       if (sp > 16) sp = 16;
+      if ((size_t)sp > L.workspace_bytes / need) sp = (int)(L.workspace_bytes / need);
       if (sp >= 2) {
         p.splits = sp;
         p.ws = reinterpret_cast<float*>(L.workspace);
-        // one slab per split when the workspace holds them (plain stores, no memset); OG_SPLITK_SLABS=0: one zeroed slab
-        // that the items reduce into with red.global.add (the round-1 form, kept for small workspaces)
-        static const bool slabs_on = [] {
-          const char* e = getenv("OG_SPLITK_SLABS");
-          return !(e && atoi(e) == 0);
-        }();
-        if (tile_ctr && tiles <= (long long)((kWsTail - 256) / sizeof(unsigned int)))
-          p.tile_ctr = tile_ctr;     // prepared workspace: `ws` is zero on entry and is left zero (fused finish)
-        else if (slabs_on && ws_usable >= need * (size_t)sp)
-          p.ws_slab = (long long)(need / sizeof(float));
-        else
-          OG_CHECK_CUDA(cudaMemsetAsync(L.workspace, 0, need, stream));
+        p.ws_slab = (long long)(need / sizeof(float));
       }
     }
   }
@@ -1069,15 +741,9 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
     if (r != OG_OK) return r;
   }
 
-  // fused epilogue reductions need: staged bf16 stores, no split-K, every CTA tile inside one sample
+  // the fused GroupNorm sums need: staged bf16 stores, no split-K, every CTA tile inside one sample
   const bool can_fuse = plain && p.fast_store && p.splits == 1 && bn == 1 && n_out <= 65536;
-  const bool can_fuse_splitk = plain && p.splits > 1 && p.tile_ctr && bn == 1 && !L.out_f32;
-  p.gn_sums = (L.gn_sums && (can_fuse || can_fuse_splitk)) ? L.gn_sums : nullptr;
-  p.red_S = (L.red_S && can_fuse) ? L.red_S : nullptr;
-  p.red_x = reinterpret_cast<const __nv_bfloat16*>(L.red_x);
-  p.red_A = L.red_A;
-  p.red_B = L.red_B;
-  p.red_act = L.red_act;
+  p.gn_sums = (L.gn_sums && can_fuse) ? L.gn_sums : nullptr;
   const int total_tiles = p.num_m_tiles * p.num_n_tiles * p.splits;
   int grid = num_sms();
   if (grid > total_tiles) grid = total_tiles;
@@ -1094,9 +760,8 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   if (rc != OG_OK) return rc;
   g_launches.fetch_add(1);
   bool finish_did_stats = false;
-  if (p.splits > 1 && !p.tile_ctr) {
+  if (p.splits > 1) {
     const long long per_sample = (long long)T * H * W * n_out;
-    const int nslab = p.ws_slab ? p.splits : 1;
     finish_did_stats = L.gn_sums && !L.out_f32;
     double* gs = finish_did_stats ? L.gn_sums : nullptr;
     const int vec = (n_out % 4 == 0) ? 4 : 1;
@@ -1106,24 +771,18 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
     if (bx < 1) bx = 1;
     dim3 grid((unsigned)bx, (unsigned)N);
     if (vec == 4)
-      og_splitk_finish_kernel<4><<<grid, 256, 0, stream>>>(p.ws, p.ws_slab, nslab, L.bias0, L.bias1, L.out, L.out_f32,
+      og_splitk_finish_kernel<4><<<grid, 256, 0, stream>>>(p.ws, p.ws_slab, p.splits, L.bias0, L.bias1, L.out, L.out_f32,
                                                             n_out, per_sample, gs);
     else
-      og_splitk_finish_kernel<1><<<grid, 256, 0, stream>>>(p.ws, p.ws_slab, nslab, L.bias0, L.bias1, L.out, L.out_f32,
+      og_splitk_finish_kernel<1><<<grid, 256, 0, stream>>>(p.ws, p.ws_slab, p.splits, L.bias0, L.bias1, L.out, L.out_f32,
                                                             n_out, per_sample, gs);
     OG_CHECK_CUDA(cudaGetLastError());
     g_launches.fetch_add(1);
   }
-  // requested reductions that could not be fused: run the stand-alone passes on the stored output
+  // requested statistics that could not be fused: run the stand-alone pass on the stored output
   if (L.gn_sums && !p.gn_sums && !finish_did_stats) {
     OG_REQUIRE(!L.out_f32 && plain, "conv3d: GroupNorm statistics need a plain bf16 output");
     int r = og_gn_stats(L.out, N, (int64_t)T * H * W, n_out, 1, L.gn_sums, (og_stream_t)stream);
-    if (r != OG_OK) return r;
-  }
-  if (L.red_S && !p.red_S) {
-    OG_REQUIRE(!L.out_f32 && plain, "conv3d: fused backward reduction needs a plain bf16 output");
-    int r = og_affine_act_bwd_reduce(L.out, L.red_x, L.red_A, L.red_B, L.red_act, L.red_S, N, (int64_t)T * H * W, n_out, nullptr, 0,
-                                     (og_stream_t)stream);
     if (r != OG_OK) return r;
   }
   return OG_OK;
@@ -1137,7 +796,7 @@ extern "C" int og_conv3d_fwd(const void* x0, int c0, int kt, int kh, int kw, int
                              void* workspace, size_t workspace_bytes, double* gn_sums, og_stream_t stream) {
   using namespace og;
   OG_REQUIRE(x0 && w && out, "conv3d_fwd: null pointer");
-  OG_REQUIRE(c0 > 0 && c0 % 64 == 0, "conv3d_fwd: c0=%d must be a positive multiple of 64 (use the im2col path)", c0);
+  OG_REQUIRE(c0 > 0 && c0 % 64 == 0, "conv3d_fwd: c0=%d must be a positive multiple of 64", c0);
   OG_REQUIRE(!x1 || (c1 > 0 && c1 % 64 == 0), "conv3d_fwd: c1=%d must be a multiple of 64", c1);
   OG_REQUIRE(kt >= 1 && kh >= 1 && kw >= 1 && pt >= 0 && ph >= 0 && pw >= 0 && pt < kt && ph < kh && pw < kw,
              "conv3d_fwd: bad kernel/padding (%d,%d,%d)/(%d,%d,%d)", kt, kh, kw, pt, ph, pw);
@@ -1160,9 +819,7 @@ extern "C" int og_conv3d_fwd(const void* x0, int c0, int kt, int kh, int kw, int
 
 extern "C" int og_conv3d_dgrad(const void* dy, int cout, int w_rows, const void* w, int ldw, int k_off, int kt, int kh,
                                int kw, int pt, int ph, int pw, void* dx, int dx_f32, int N, int T, int H, int W,
-                               int cin, void* workspace, size_t workspace_bytes, const void* red_x,
-                               const float* red_A, const float* red_B, int red_act, float* red_S,
-                               og_stream_t stream) {
+                               int cin, void* workspace, size_t workspace_bytes, og_stream_t stream) {
   using namespace og;
   OG_REQUIRE(dy && w && dx, "conv3d_dgrad: null pointer");
   OG_REQUIRE(cout > 0 && cout % 64 == 0, "conv3d_dgrad: cout=%d must be a multiple of 64", cout);
@@ -1177,32 +834,7 @@ extern "C" int og_conv3d_dgrad(const void* dy, int cout, int w_rows, const void*
   L.out = dx; L.out_f32 = dx_f32;
   L.N = N; L.T = T; L.H = H; L.W = W; L.n_out = cin;
   L.workspace = workspace; L.workspace_bytes = workspace_bytes;
-  L.red_x = red_x; L.red_A = red_A; L.red_B = red_B; L.red_act = red_act; L.red_S = red_S;
   return launch_igemm(L, (cudaStream_t)stream);
-}
-
-// Prepares a workspace for og_conv3d_fwd / og_conv3d_dgrad: writes the dynamic tile scheduler's state {magic, 0, 0} into
-// its last 256 bytes. Call once after allocating (or re-allocating) the buffer; the kernels reset the state themselves.
-// A workspace that was not initialised (no magic) simply gets the static tile assignment.
-extern "C" int og_workspace_init(void* workspace, size_t workspace_bytes, og_stream_t stream) {
-  using namespace og;
-  OG_REQUIRE(workspace && workspace_bytes >= 2 * kWsTail, "workspace_init: need a workspace of at least %zu bytes", 2 * kWsTail);
-  const size_t off = (workspace_bytes - kWsTail) & ~(size_t)255;
-  char* tail = reinterpret_cast<char*>(workspace) + off;
-  OG_CHECK_CUDA(cudaMemsetAsync(workspace, 0, workspace_bytes, (cudaStream_t)stream));   // partial sums + counters: all zero
-  static const unsigned int magic = kSchedMagic;
-  OG_CHECK_CUDA(cudaMemcpyAsync(tail, &magic, sizeof(magic), cudaMemcpyHostToDevice, (cudaStream_t)stream));
-  {
-    std::lock_guard<std::mutex> lock(g_ws_mutex);
-    bool found = false;
-    for (auto& e : g_ws_prepared)
-      if (e.first == workspace) {
-        e.second = workspace_bytes;
-        found = true;
-      }
-    if (!found) g_ws_prepared.emplace_back(workspace, workspace_bytes);
-  }
-  return OG_OK;
 }
 
 static int out_extent(int in, int pad_front, int pad_back, int k, int s) { return (in + pad_front + pad_back - k) / s + 1; }

@@ -4,9 +4,6 @@
 //     everywhere; the product keeps NDHWC bf16 between kernels)
 //   * depth-to-space-time pixel shuffle 'b (c p q r) t h w -> b c (t p) (h q) (w r)' and its inverse
 //     (genie/module/video.py:403-408)
-//   * explicit im2col / col2im for the few layers the implicit-GEMM kernel does not take directly:
-//     strided CausalConv3d (SpaceTimeDownsample, video.py:477-483) and convs whose Cin is not a
-//     multiple of 64 (3 -> C input projections, 18 -> 512 decoder stem)
 //   * mse_loss forward / backward (tokenizer.py:364, action.py:166), bias gradient (column sums)
 #include "og_host.cuh"
 #include "og_ptx.cuh"
@@ -187,158 +184,6 @@ __global__ void __launch_bounds__(256)
 #pragma unroll
       for (int k = 0; k < PQR; ++k) xw[xoff + k] = a.v[k];
     }
-  }
-}
-
-// im2col: x NDHWC (bf16) -> col [M = N*To*Ho*Wo][kpad], k = tap*C + ci; zero for padding / OOB / k >= ntaps*C
-__global__ void og_im2col_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ col, int T, int H,
-                                 int W, int C, int To, int Ho, int Wo, int kt, int kh, int kw, int st, int sh, int sw,
-                                 int pt, int ph, int pw, int kpad, long long total) {
-  const int K = kt * kh * kw * C;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int k = (int)(i % kpad);
-    long long m = i / kpad;
-    __nv_bfloat16 val = __float2bfloat16_rn(0.f);
-    if (k < K) {
-      const int ci = k % C;
-      const int tap = k / C;
-      const int iw = tap % kw, ih = (tap / kw) % kh, it = tap / (kw * kh);
-      const int wo = (int)(m % Wo);
-      m /= Wo;
-      const int ho = (int)(m % Ho);
-      m /= Ho;
-      const int to = (int)(m % To);
-      const int n = (int)(m / To);
-      const int t = to * st + it - pt, h = ho * sh + ih - ph, w = wo * sw + iw - pw;
-      if (t >= 0 && t < T && h >= 0 && h < H && w >= 0 && w < W)
-        val = x[((((long long)n * T + t) * H + h) * W + w) * C + ci];
-    }
-    col[i] = val;
-  }
-}
-
-// 16-byte variant (C % 8 == 0, kpad % 8 == 0): one thread moves 8 channels of one tap
-__global__ void og_im2col_vec_kernel(const uint4* __restrict__ x, uint4* __restrict__ col, int T, int H, int W, int C,
-                                     int To, int Ho, int Wo, int kt, int kh, int kw, int st, int sh, int sw, int pt,
-                                     int ph, int pw, int kpad, long long total_vec) {
-  const int cv = C >> 3, kv = kpad >> 3, Kv = kt * kh * kw * cv;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total_vec;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int k = (int)(i % kv);
-    long long m = i / kv;
-    uint4 val = make_uint4(0, 0, 0, 0);
-    if (k < Kv) {
-      const int c8 = k % cv;
-      const int tap = k / cv;
-      const int iw = tap % kw, ih = (tap / kw) % kh, it = tap / (kw * kh);
-      const int wo = (int)(m % Wo);
-      m /= Wo;
-      const int ho = (int)(m % Ho);
-      m /= Ho;
-      const int to = (int)(m % To);
-      const int n = (int)(m / To);
-      const int t = to * st + it - pt, h = ho * sh + ih - ph, w = wo * sw + iw - pw;
-      if (t >= 0 && t < T && h >= 0 && h < H && w >= 0 && w < W)
-        val = __ldg(x + ((((long long)n * T + t) * H + h) * W + w) * cv + c8);
-    }
-    col[i] = val;
-  }
-}
-
-__global__ void og_col2im_vec_kernel(const uint4* __restrict__ dcol, uint4* __restrict__ dx, int T, int H, int W, int C,
-                                     int To, int Ho, int Wo, int kt, int kh, int kw, int st, int sh, int sw, int pt,
-                                     int ph, int pw, int kpad, long long total_vec) {
-  const int cv = C >> 3, kv = kpad >> 3;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total_vec;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int c8 = (int)(i % cv);
-    long long v = i / cv;
-    const int w = (int)(v % W);
-    v /= W;
-    const int h = (int)(v % H);
-    v /= H;
-    const int t = (int)(v % T);
-    const int n = (int)(v / T);
-    float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    for (int it = 0; it < kt; ++it) {
-      const int tn = t + pt - it;
-      if (tn < 0 || tn % st) continue;
-      const int to = tn / st;
-      if (to >= To) continue;
-      for (int ih = 0; ih < kh; ++ih) {
-        const int hn = h + ph - ih;
-        if (hn < 0 || hn % sh) continue;
-        const int ho = hn / sh;
-        if (ho >= Ho) continue;
-        for (int iw = 0; iw < kw; ++iw) {
-          const int wn = w + pw - iw;
-          if (wn < 0 || wn % sw) continue;
-          const int wo = wn / sw;
-          if (wo >= Wo) continue;
-          const long long m = (((long long)n * To + to) * Ho + ho) * Wo + wo;
-          const int tap = (it * kh + ih) * kw + iw;
-          const uint4 u = __ldg(dcol + m * kv + (long long)tap * cv + c8);
-          const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 f = __bfloat1622float2(hh[e]);
-            acc[2 * e] += f.x;
-            acc[2 * e + 1] += f.y;
-          }
-        }
-      }
-    }
-    uint4 o;
-    o.x = pack_bf16x2(acc[0], acc[1]);
-    o.y = pack_bf16x2(acc[2], acc[3]);
-    o.z = pack_bf16x2(acc[4], acc[5]);
-    o.w = pack_bf16x2(acc[6], acc[7]);
-    dx[i] = o;
-  }
-}
-
-// col2im (gather form, deterministic): dx[n,t,h,w,ci] = sum over taps/outputs that read this input element
-template <typename OutT>
-__global__ void og_col2im_kernel(const __nv_bfloat16* __restrict__ dcol, OutT* __restrict__ dx, int T, int H, int W,
-                                 int C, int To, int Ho, int Wo, int kt, int kh, int kw, int st, int sh, int sw, int pt,
-                                 int ph, int pw, int kpad, long long total) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int ci = (int)(i % C);
-    long long v = i / C;
-    const int w = (int)(v % W);
-    v /= W;
-    const int h = (int)(v % H);
-    v /= H;
-    const int t = (int)(v % T);
-    const int n = (int)(v / T);
-    float acc = 0.f;
-    for (int it = 0; it < kt; ++it) {
-      const int tn = t + pt - it;
-      if (tn < 0 || tn % st) continue;
-      const int to = tn / st;
-      if (to >= To) continue;
-      for (int ih = 0; ih < kh; ++ih) {
-        const int hn = h + ph - ih;
-        if (hn < 0 || hn % sh) continue;
-        const int ho = hn / sh;
-        if (ho >= Ho) continue;
-        for (int iw = 0; iw < kw; ++iw) {
-          const int wn = w + pw - iw;
-          if (wn < 0 || wn % sw) continue;
-          const int wo = wn / sw;
-          if (wo >= Wo) continue;
-          const long long m = (((long long)n * To + to) * Ho + ho) * Wo + wo;
-          const int tap = (it * kh + ih) * kw + iw;
-          acc += __bfloat162float(dcol[m * kpad + (long long)tap * C + ci]);
-        }
-      }
-    }
-    if constexpr (sizeof(OutT) == 2)
-      dx[i] = __float2bfloat16_rn(acc);
-    else
-      dx[i] = acc;
   }
 }
 
@@ -597,52 +442,6 @@ extern "C" int og_pixel_shuffle3d(const void* x, void* y, int inverse, int N, in
   else
     og_pixel_shuffle_kernel<<<ew_blocks(total, 256), 256, 0, (cudaStream_t)stream>>>(
         (const __nv_bfloat16*)x, (__nv_bfloat16*)y, T, H, W, c, p, q, r, total, inverse);
-  OG_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1);
-  return OG_OK;
-}
-
-extern "C" int og_im2col3d(const void* x, void* col, int N, int T, int H, int W, int C, int kt, int kh, int kw,
-                           int st, int sh, int sw, int pt, int ph, int pw, int kpad, og_stream_t stream) {
-  OG_REQUIRE(x && col, "im2col3d: null pointer");
-  OG_REQUIRE(kpad >= kt * kh * kw * C, "im2col3d: kpad=%d < %d", kpad, kt * kh * kw * C);
-  // causal "same" geometry of CausalConv3d (video.py:154-164): full front pad in time, symmetric in space
-  const int To = (T + pt - kt) / st + 1, Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
-  const long long total = (long long)N * To * Ho * Wo * kpad;
-  if (C % 8 == 0 && kpad % 8 == 0) {
-    og_im2col_vec_kernel<<<ew_blocks(total / 8, 256), 256, 0, (cudaStream_t)stream>>>(
-        (const uint4*)x, (uint4*)col, T, H, W, C, To, Ho, Wo, kt, kh, kw, st, sh, sw, pt, ph, pw, kpad, total / 8);
-    OG_CHECK_CUDA(cudaGetLastError());
-    g_launches.fetch_add(1);
-    return OG_OK;
-  }
-  og_im2col_kernel<<<ew_blocks(total, 256), 256, 0, (cudaStream_t)stream>>>(
-      (const __nv_bfloat16*)x, (__nv_bfloat16*)col, T, H, W, C, To, Ho, Wo, kt, kh, kw, st, sh, sw, pt, ph, pw, kpad,
-      total);
-  OG_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1);
-  return OG_OK;
-}
-
-extern "C" int og_col2im3d(const void* dcol, void* dx, int dx_f32, int N, int T, int H, int W, int C, int kt, int kh,
-                           int kw, int st, int sh, int sw, int pt, int ph, int pw, int kpad, og_stream_t stream) {
-  OG_REQUIRE(dcol && dx, "col2im3d: null pointer");
-  const int To = (T + pt - kt) / st + 1, Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
-  const long long total = (long long)N * T * H * W * C;
-  if (!dx_f32 && C % 8 == 0 && kpad % 8 == 0) {
-    og_col2im_vec_kernel<<<ew_blocks(total / 8, 256), 256, 0, (cudaStream_t)stream>>>(
-        (const uint4*)dcol, (uint4*)dx, T, H, W, C, To, Ho, Wo, kt, kh, kw, st, sh, sw, pt, ph, pw, kpad, total / 8);
-    OG_CHECK_CUDA(cudaGetLastError());
-    g_launches.fetch_add(1);
-    return OG_OK;
-  }
-  if (dx_f32)
-    og_col2im_kernel<float><<<ew_blocks(total, 256), 256, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16*)dcol, (float*)dx, T, H, W, C, To, Ho, Wo, kt, kh, kw, st, sh, sw, pt, ph, pw, kpad, total);
-  else
-    og_col2im_kernel<__nv_bfloat16><<<ew_blocks(total, 256), 256, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16*)dcol, (__nv_bfloat16*)dx, T, H, W, C, To, Ho, Wo, kt, kh, kw, st, sh, sw, pt, ph, pw,
-        kpad, total);
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   return OG_OK;

@@ -133,7 +133,7 @@ void choose_voxel_box(int vox, int N, int T, int H, int W, int* bw, int* bh, int
 
 extern "C" {
 const char* og_last_error(void) { return og::g_err; }
-int og_abi_version(void) { return 1; }
+int og_abi_version(void) { return 2; }
 int og_compiled_sm(void) { return 90; }
 uint64_t og_launch_count(void) { return og::g_launches.load(); }
 }

@@ -159,9 +159,7 @@ class StepScope:
         if t is None or t.numel() < nbytes:
             if self.frozen or (dev.type == 'cuda' and torch.cuda.is_current_stream_capturing()):
                 raise RuntimeError('open_genie_b200: split-K workspace of a captured training step would have to grow')
-            t = torch.empty(nbytes + 8192, dtype=torch.uint8, device=dev)
-            if dev.type == 'cuda':      # dynamic tile scheduler state in the buffer's tail (include/opengenie_b200.h)
-                _lib.call('og_workspace_init', t.data_ptr(), t.numel(), torch.cuda.current_stream(dev).cuda_stream)
+            t = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             self.ws[dev] = t
         return t
 
@@ -218,35 +216,15 @@ def _zeros(shape, dtype, device, recording: bool = False):
     return a.zeros(shape, dtype, device)
 
 
-# tuning switches (environment): fuse GroupNorm statistics / backward reductions into the GEMM epilogues
-import os as _os
-FUSE_STATS = _os.environ.get('OG_FUSE_STATS', '1') != '0'
-FUSE_RED = _os.environ.get('OG_FUSE_RED', '0') != '0'   # measured: costs more in the dgrad epilogue than the pass it saves
-FUSE_BIAS_GRAD = _os.environ.get('OG_FUSE_BIAS_GRAD', '1') != '0'   # bias gradient inside the weight-gradient launch
-
-
-# GroupNorm backward over sample GROUPS: reduce(group) then apply(group), so that the apply pass finds the group's dy / x in
-# L2 (126 MB) instead of streaming them from HBM a second time. Only for tensors that do not fit L2 as a whole; groups run
-# from the last sample to the first because the producing data-gradient kernel wrote the last samples last (still in L2).
-GN_BWD_GROUPS = int(_os.environ.get('OG_GN_BWD_GROUPS', '1'))
-GN_BWD_MIN_BYTES = int(_os.environ.get('OG_GN_BWD_MIN_MB', '96')) << 20
-
-
 def _gn_bwd(dy, x, A, Bc, S, mr, gamma, beta, G, act, add, dx, dgamma, dbeta, dx_colsum, B, V, C, s, reduce=True):
-    """og_affine_act_bwd_reduce + og_gn_act_bwd on bf16 [B, V, C] tensors (the ResidualBlock's GroupNorm(1, C) / SiLU
-    backward, genie/module/video.py:607-629), optionally split over sample groups (see GN_BWD_GROUPS)."""
-    groups = GN_BWD_GROUPS if (GN_BWD_GROUPS > 1 and B % GN_BWD_GROUPS == 0 and 2 * B * V * C >= GN_BWD_MIN_BYTES) else 1
-    nb = B // groups
-    for g in reversed(range(groups)):
-        n0 = g * nb
-        oa, oc, oS, om = n0 * V * C * 2, n0 * C * 4, n0 * C * 8, n0 * G * 8
-        if reduce:
-            _lib.call('og_affine_act_bwd_reduce', dy.data_ptr() + oa, x.data_ptr() + oa, A.data_ptr() + oc, Bc.data_ptr() + oc,
-                      act, S.data_ptr() + oS, nb, V, C, *_scratch(dy), s)
-        _lib.call('og_gn_act_bwd', dy.data_ptr() + oa, x.data_ptr() + oa, A.data_ptr() + oc, Bc.data_ptr() + oc,
-                  S.data_ptr() + oS, mr.data_ptr() + om, gamma.data_ptr(), beta.data_ptr(), None, G, act,
-                  (add.data_ptr() + oa) if add is not None else None, dx.data_ptr() + oa, dgamma.data_ptr(), dbeta.data_ptr(),
-                  None, None, dx_colsum.data_ptr() if dx_colsum is not None else None, nb, V, C, *_scratch(dy), s)
+    """og_affine_act_bwd_reduce (unless S already holds it) + og_gn_act_bwd on bf16 [B, V, C] tensors (the ResidualBlock's
+    GroupNorm(1, C) / SiLU backward, genie/module/video.py:607-629)."""
+    if reduce:
+        _lib.call('og_affine_act_bwd_reduce', dy.data_ptr(), x.data_ptr(), A.data_ptr(), Bc.data_ptr(), act, S.data_ptr(),
+                  B, V, C, *_scratch(dy), s)
+    _lib.call('og_gn_act_bwd', dy.data_ptr(), x.data_ptr(), A.data_ptr(), Bc.data_ptr(), S.data_ptr(), mr.data_ptr(),
+              gamma.data_ptr(), beta.data_ptr(), None, G, act, _ptr(add), dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(),
+              None, None, _ptr(dx_colsum), B, V, C, *_scratch(dy), s)
 
 
 def _scratch(t: Tensor):
@@ -257,7 +235,7 @@ def _scratch(t: Tensor):
 
 def _workspace(dev, nbytes: int):
     """Reusable fp32 scratch for split-K convolutions (small T*H*W, deep K). One buffer per device and step scope;
-    every use is stream-ordered (memset -> partial sums -> finish pass inside one og_conv3d_* call)."""
+    every use is stream-ordered (partial-sum slabs -> finish pass inside one og_conv3d_* call)."""
     return _SCOPE.workspace(dev, nbytes)
 
 
@@ -379,19 +357,17 @@ class ConvGeom:
         self.causal = causal
         self.ntaps = self.kt * self.kh * self.kw
         self.strided = stride != (1, 1, 1)
-        # Every convolution is an implicit GEMM: stride 1 (`direct`) or strided (`strided_implicit`: strided TMA boxes
-        # forward / weight gradient, residue-class decomposition for the data gradient). A k-block of the kernels is 64
-        # channels of one tap, so an input with Cin not in 64Z (the 3- and 18-channel stem convolutions) is zero-padded
-        # to `cin_pad` channels (a pass over a 3-channel tensor) and its packed weights likewise — for Cin = 3 that costs
-        # ~0.3 ms of extra tensor-core time per training step and replaces a 134 MB im2col buffer + its two passes.
-        # OG_STRIDED_IM2COL=1 keeps the explicit im2col + GEMM form of round 1 for strided / narrow layers (tests).
-        legacy = _os.environ.get('OG_STRIDED_IM2COL', '0') != '0' and causal and (self.strided or cin % 64 != 0)
-        self.cin_pad = cin if legacy else _round_up(cin, 64)
+        # Every convolution is an implicit GEMM: stride 1 (`direct`) or strided (strided TMA boxes forward / weight
+        # gradient, residue-class decomposition for the data gradient). A k-block of the kernels is 64 channels of one
+        # tap, so an input with Cin not in 64Z (the 3- and 18-channel stem convolutions) is zero-padded to `cin_pad`
+        # channels (a pass over a 3-channel tensor) and its packed weights likewise — for Cin = 3 that costs ~0.3 ms of
+        # extra tensor-core time per training step and replaces a 134 MB im2col buffer + its two passes.
+        self.cin_pad = _round_up(cin, 64)
         self.padded = self.cin_pad != cin
-        self.direct = (not self.strided) and not legacy
-        self.strided_implicit = self.strided and causal and not legacy
+        self.direct = not self.strided
+        self.strided_implicit = self.strided
         self.k_main = self.ntaps * cin                      # algorithmic reduction length (FLOP accounting)
-        self.kpad = self.ntaps * self.cin_pad if (self.direct or self.strided_implicit) else _round_up(self.k_main, 64)
+        self.kpad = self.ntaps * self.cin_pad
         if self.strided and not causal:
             raise NotImplementedError('strided convolutions implement CausalConv3d geometry only')
 
@@ -427,7 +403,7 @@ def _pad_input_channels(xi: Tensor, cpad: int) -> Tensor:
 
 
 class _Conv3dFn(torch.autograd.Function):
-    """y = conv(x; w, b) [+ conv1x1(x2; w2, b2)]   — og_conv3d_fwd / dgrad / wgrad, or im2col + the same kernels."""
+    """y = conv(x; w, b) [+ conv1x1(x2; w2, b2)]   — og_conv3d_fwd / dgrad / wgrad, or their strided forms."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, x2, weight2, bias2, packed, geom: ConvGeom, out_f32: bool, residual=None):
@@ -445,7 +421,6 @@ class _Conv3dFn(torch.autograd.Function):
         ldw = packed.shape[1]
         ws = _workspace(x.device, B * To * Ho * Wo * geom.cout * 4)
         x2i = None
-        col = None
         resi = None
         if residual is not None:     # out = conv(x) + residual, added in fp32 inside the GEMM epilogue (stride-1 convs)
             assert geom.direct and not out_f32, 'the fused residual add needs a stride-1 convolution with a bf16 output'
@@ -460,27 +435,18 @@ class _Conv3dFn(torch.autograd.Function):
                        'og_conv3d_fwd', xi.data_ptr(), Cp, geom.kt, geom.kh, geom.kw, geom.pt, geom.ph, geom.pw,
                       _ptr(x2i), c1, packed.data_ptr(), ldw, _ptr(bias), _ptr(bias2), _ptr(resi), y.data_ptr(), int(out_f32),
                       B, T, H, W, geom.cout, ws.data_ptr(), ws.numel(), None, s)
-        elif geom.strided_implicit:
+        else:
             assert x2 is None
             _conv_call('fwd', 2.0 * B * To * Ho * Wo * geom.cout * geom.k_main,
                        'og_conv3d_strided_fwd', xi.data_ptr(), Cp, geom.kt, geom.kh, geom.kw, geom.st, geom.sh, geom.sw,
                        geom.pt, geom.ph, geom.pw, packed.data_ptr(), ldw, _ptr(bias), y.data_ptr(), int(out_f32), B, T, H,
                        W, geom.cout, s)
-        else:
-            assert x2 is None
-            col = torch.empty((B * To * Ho * Wo, geom.kpad), dtype=bf16, device=x.device)
-            _lib.call('og_im2col3d', xi.data_ptr(), col.data_ptr(), B, T, H, W, C, geom.kt, geom.kh, geom.kw,
-                      geom.st, geom.sh, geom.sw, geom.pt, geom.ph, geom.pw, geom.kpad, s)
-            _conv_call('fwd', 2.0 * B * To * Ho * Wo * geom.cout * geom.k_main,
-                       'og_conv3d_fwd', col.data_ptr(), geom.kpad, 1, 1, 1, 0, 0, 0, None, 0, packed.data_ptr(), ldw,
-                      _ptr(bias), None, None, y.data_ptr(), int(out_f32), 1, 1, 1, B * To * Ho * Wo, geom.cout,
-                      ws.data_ptr(), ws.numel(), None, s)
         ctx.geom = geom
         ctx.in_shape = (B, C, T, H, W)
         ctx.has_bias = (bias is not None, bias2 is not None)
         ctx.has_residual = residual is not None
         ctx.w_shapes = (weight.shape, None if weight2 is None else weight2.shape)
-        ctx.save_for_backward(xi if (geom.direct or geom.strided_implicit) else col, x2i, packed)
+        ctx.save_for_backward(xi, x2i, packed)
         return y
 
     @staticmethod
@@ -510,7 +476,7 @@ class _Conv3dFn(torch.autograd.Function):
             g = _zeros((rows, kt * kh * kw * cin), f32, dev)
             real_cin = C if (geom.padded and cin == geom.cin_pad) else cin      # algorithmic FLOPs: no padding counted
             fl = 2.0 * dims[0] * dims[1] * dims[2] * dims[3] * cout * min(real_cin, geom.k_main) * kt * kh * kw
-            if want_db and FUSE_BIAS_GRAD and not fused_db[0]:
+            if want_db and not fused_db[0]:
                 fused_db[0] = True
                 _conv_call('wgrad', fl, 'og_conv3d_wgrad_bias', dyb.data_ptr(), cpad, xin.data_ptr(), cin, g.data_ptr(),
                            g.shape[1], kt, kh, kw, pt, ph, pw, dims[0], dims[1], dims[2], dims[3], dbs.data_ptr(), cout,
@@ -527,7 +493,7 @@ class _Conv3dFn(torch.autograd.Function):
                 _conv_call('dgrad', 2.0 * B * T * H * W * cout * geom.k_main,
                            'og_conv3d_dgrad', dyb.data_ptr(), cpad, cout, packed.data_ptr(), ldw, 0, geom.kt, geom.kh,
                            geom.kw, geom.pt, geom.ph, geom.pw, dx.data_ptr(), 0, B, T, H, W, Cp, ws.data_ptr(), ws.numel(),
-                           None, None, None, 0, None, s)
+                           s)
                 if geom.padded:
                     dx = dx[:, :C]
             if need[1]:
@@ -539,12 +505,11 @@ class _Conv3dFn(torch.autograd.Function):
                     dx2 = empty_internal(B, c1, T, H, W, bf16, dev)
                     _conv_call('dgrad', 2.0 * B * T * H * W * cout * c1,
                                'og_conv3d_dgrad', dyb.data_ptr(), cpad, cout, packed.data_ptr(), ldw, geom.k_main,
-                               1, 1, 1, 0, 0, 0, dx2.data_ptr(), 0, B, T, H, W, c1, ws.data_ptr(), ws.numel(),
-                               None, None, None, 0, None, s)
+                               1, 1, 1, 0, 0, 0, dx2.data_ptr(), 0, B, T, H, W, c1, ws.data_ptr(), ws.numel(), s)
                 if need[4]:
                     g = wgrad(x2i, c1, 1, 1, 1, 0, 0, 0, ctx.w_shapes[1], (B, T, H, W))
                     dw2 = g.view(cout, 1, 1, 1, c1).permute(0, 4, 1, 2, 3)
-        elif geom.strided_implicit:
+        else:
             if need[0]:
                 dx = empty_internal(B, Cp, T, H, W, bf16, dev)
                 _conv_call('dgrad', 2.0 * B * To * Ho * Wo * cout * geom.k_main,
@@ -560,19 +525,6 @@ class _Conv3dFn(torch.autograd.Function):
                            geom.kt, geom.kh, geom.kw, geom.st, geom.sh, geom.sw, geom.pt, geom.ph, geom.pw, B, T, H, W,
                            *_scratch(dyb), s)
                 dw = g[:cout].view(cout, geom.kt, geom.kh, geom.kw, Cp)[..., :C].permute(0, 4, 1, 2, 3)
-        else:
-            col = xs
-            if need[0]:
-                dcol = torch.empty_like(col)
-                _conv_call('dgrad', 2.0 * B * To * Ho * Wo * cout * geom.k_main,
-                           'og_conv3d_dgrad', dyb.data_ptr(), cpad, cout, packed.data_ptr(), ldw, 0, 1, 1, 1, 0, 0, 0,
-                           dcol.data_ptr(), 0, 1, 1, 1, B * To * Ho * Wo, geom.kpad, None, 0, None, None, None, 0, None, s)
-                dx = empty_internal(B, C, T, H, W, bf16, dev)
-                _lib.call('og_col2im3d', dcol.data_ptr(), dx.data_ptr(), 0, B, T, H, W, C, geom.kt, geom.kh, geom.kw,
-                          geom.st, geom.sh, geom.sw, geom.pt, geom.ph, geom.pw, geom.kpad, s)
-            if need[1]:
-                g = wgrad(col, geom.kpad, 1, 1, 1, 0, 0, 0, ctx.w_shapes[0], (1, 1, 1, B * To * Ho * Wo))
-                dw = g[:, :geom.k_main].reshape(cout, geom.kt, geom.kh, geom.kw, C).permute(0, 4, 1, 2, 3)
         if want_db:
             if not fused_db[0]:
                 _lib.call('og_colsum', dyb.data_ptr(), B * To * Ho * Wo, cout, cpad, dbs.data_ptr(), s)
@@ -940,8 +892,6 @@ def _rope_table(freq: Tensor, npos: int) -> Optional[Tensor]:
     tensor object (per sequence length; rebuilt if the tensor is modified in place), so it lives and dies with the module's
     `freq` parameter. Never built while a CUDA graph is being captured: a captured step uses the tables its warm-up steps
     created, or none (the passes then evaluate sincosf per element — same values)."""
-    if _os.environ.get('OG_ROPE_TABLE', '1') == '0':
-        return None
     cache = getattr(freq, '_og_rope_tables', None)
     if cache is None or cache[0] != (freq.data_ptr(), freq._version):
         cache = ((freq.data_ptr(), freq._version), {})
@@ -1103,10 +1053,12 @@ class _FfnFn(torch.autograd.Function):
         ws = _workspace(dev, B * V * C * 4)
         dh = torch.empty_like(x)
         S = _zeros((B, C, 2), f32, dev)
-        # data gradient with the GroupNorm backward reduction fused into its epilogue
+        # data gradient, then the GroupNorm backward reduction over it
         _conv_call('dgrad', 2.0 * B * V * C * geom.k_main, 'og_conv3d_dgrad', dy.data_ptr(), C, C, packed.data_ptr(),
                    packed.shape[1], 0, geom.kt, geom.kh, geom.kw, geom.pt, geom.ph, geom.pw, dh.data_ptr(), 0, B, T, H,
-                   W, C, ws.data_ptr(), ws.numel(), x.data_ptr(), A.data_ptr(), Bc.data_ptr(), 0, S.data_ptr(), s)
+                   W, C, ws.data_ptr(), ws.numel(), s)
+        _lib.call('og_affine_act_bwd_reduce', dh.data_ptr(), x.data_ptr(), A.data_ptr(), Bc.data_ptr(), 0, S.data_ptr(),
+                  B, V, C, *_scratch(dh), s)
         g = _zeros((C, geom.ntaps * C), f32, dev)
         _conv_call('wgrad', 2.0 * B * V * C * geom.k_main, 'og_conv3d_wgrad', dy.data_ptr(), C, hn.data_ptr(), C,
                    g.data_ptr(), g.shape[1], geom.kt, geom.kh, geom.kw, geom.pt, geom.ph, geom.pw, B, T, H, W,
@@ -1247,7 +1199,6 @@ def maskgit_sample(logits_last: Tensor, uniforms: Tensor, schedule: Tensor, temp
 class _ResBlockFn(torch.autograd.Function):
     """One autograd node for the whole block (genie/module/video.py:539-656) so that
       * GroupNorm statistics of each conv output come out of the producing GEMM's epilogue (gn_sums),
-      * the GroupNorm backward reductions come out of the data-gradient GEMM's epilogue (red_S),
       * the shortcut's data gradient is added inside the last backward apply pass (no stand-alone add),
     leaving per block: 2 apply passes forward, 2 apply passes backward, 2 column-sum passes, and the GEMMs."""
 
@@ -1272,7 +1223,7 @@ class _ResBlockFn(torch.autograd.Function):
         _lib.call('og_gn_act_fwd', xi.data_ptr(), x_sums.data_ptr(), g1w.data_ptr(), g1b.data_ptr(), None, None, eps, G, act,
                   a1.data_ptr(), A1.data_ptr(), B1.data_ptr(), mr[0].data_ptr(), B, V, C0, s)
         ws = _workspace(dev, B * V * C1 * 4)
-        fuse_stats = G == 1 and FUSE_STATS
+        fuse_stats = G == 1
         sums2 = _zeros((B, G, 2), torch.float64, dev, rec)
         h1 = empty_internal(B, C1, T, H, W, bf16, dev)
         _conv_call('fwd', 2.0 * B * V * C1 * geom1.k_main, 'og_conv3d_fwd', a1.data_ptr(), C0, geom1.kt, geom1.kh,
@@ -1289,9 +1240,7 @@ class _ResBlockFn(torch.autograd.Function):
         _conv_call('fwd', 2.0 * B * V * C1 * (geom2.k_main + C0), 'og_conv3d_fwd', a2.data_ptr(), C1, geom2.kt, geom2.kh,
                    geom2.kw, geom2.pt, geom2.ph, geom2.pw, xi.data_ptr(), C0, packed2.data_ptr(), packed2.shape[1],
                    _ptr(b2), _ptr(bres), None, y.data_ptr(), 0, B, T, H, W, C1, ws.data_ptr(), ws.numel(),
-                   y_sums.data_ptr() if FUSE_STATS else None, s)
-        if not FUSE_STATS:
-            _lib.call('og_gn_stats', y.data_ptr(), B, V, C1, 1, y_sums.data_ptr(), s)
+                   y_sums.data_ptr(), s)
         ctx.cfg = (geom1, geom2, G, b1 is not None, b2 is not None, bres is not None, act)
         ctx.save_for_backward(xi, a1, h1, a2, A1, B1, A2, B2, mr, g1w, g1b, g2w, g2b, packed1, packed2)
         ctx.mark_non_differentiable(y_sums)
@@ -1326,51 +1275,34 @@ class _ResBlockFn(torch.autograd.Function):
         gone = ConvGeom(C0, C1, (1, 1, 1))
         db2 = _zeros(C1, f32, dev)
         dw2 = wgrad(dyb, C1, a2, C1, geom2)
-        dwres = wgrad(dyb, C1, xi, C0, gone, dbias=db2 if FUSE_BIAS_GRAD else None)   # 1 tap: spare accumulator columns
-        if not FUSE_BIAS_GRAD:
-            _lib.call('og_colsum', dyb.data_ptr(), B * V, C1, C1, db2.data_ptr(), s)
-        # conv2 data gradient + fused GN2 backward reduction
+        dwres = wgrad(dyb, C1, xi, C0, gone, dbias=db2)   # 1 tap: spare accumulator columns
+        # conv2 data gradient, then the GN2 backward
         S2 = _zeros((B, C1, 2), f32, dev)
         d_a2 = empty_internal(B, C1, T, H, W, bf16, dev)
         _conv_call('dgrad', 2.0 * B * V * C1 * geom2.k_main, 'og_conv3d_dgrad', dyb.data_ptr(), C1, C1, packed2.data_ptr(),
                    ld2, 0, geom2.kt, geom2.kh, geom2.kw, geom2.pt, geom2.ph, geom2.pw, d_a2.data_ptr(), 0, B, T, H, W, C1,
-                   ws.data_ptr(), ws.numel(), *((h1.data_ptr(), A2.data_ptr(), B2.data_ptr(), act, S2.data_ptr())
-                                                if FUSE_RED else (None, None, None, 0, None)), s)
+                   ws.data_ptr(), ws.numel(), s)
         small = _zeros((3, C1), f32, dev)              # dgamma2, dbeta2, db1 in one fill
         dg2w, dg2b, db1 = small[0], small[1], small[2]
         d_h1 = empty_internal(B, C1, T, H, W, bf16, dev)
-        _gn_bwd(d_a2, h1, A2, B2, S2, mr[1], g2w, g2b, G, act, None, d_h1, dg2w, dg2b, db1 if has_b1 else None, B, V, C1, s,
-                reduce=not FUSE_RED)
+        _gn_bwd(d_a2, h1, A2, B2, S2, mr[1], g2w, g2b, G, act, None, d_h1, dg2w, dg2b, db1 if has_b1 else None, B, V, C1, s)
         dw1 = wgrad(d_h1, C1, a1, C0, geom1)
         dx = None
         dg1w, dg1b = _zeros(C0, f32, dev), _zeros(C0, f32, dev)
         dx_res = empty_internal(B, C0, T, H, W, bf16, dev)
-
-        def shortcut_dgrad():
-            _conv_call('dgrad', 2.0 * B * V * C1 * C0, 'og_conv3d_dgrad', dyb.data_ptr(), C1, C1, packed2.data_ptr(), ld2,
-                       geom2.k_main, 1, 1, 1, 0, 0, 0, dx_res.data_ptr(), 0, B, T, H, W, C0, ws.data_ptr(), ws.numel(),
-                       None, None, None, 0, None, s)
-
-        grouped = GN_BWD_GROUPS > 1      # reduce + apply per sample group must be adjacent: the shortcut gradient goes first
-        if grouped:
-            shortcut_dgrad()
-        # conv1 data gradient (+ fused GN1 backward reduction); shortcut data gradient; GN1 backward apply adds both
+        # conv1 data gradient; GN1 backward reduction; shortcut data gradient; GN1 backward apply adds both
         S1 = _zeros((B, C0, 2), f32, dev)
         d_a1 = empty_internal(B, C0, T, H, W, bf16, dev)
         _conv_call('dgrad', 2.0 * B * V * C1 * geom1.k_main, 'og_conv3d_dgrad', d_h1.data_ptr(), C1, C1,
                    packed1.data_ptr(), packed1.shape[1], 0, geom1.kt, geom1.kh, geom1.kw, geom1.pt, geom1.ph, geom1.pw,
-                   d_a1.data_ptr(), 0, B, T, H, W, C0, ws.data_ptr(), ws.numel(),
-                   *((xi.data_ptr(), A1.data_ptr(), B1.data_ptr(), act, S1.data_ptr()) if FUSE_RED
-                     else (None, None, None, 0, None)), s)
-        if not grouped:
-            if not FUSE_RED:
-                _lib.call('og_affine_act_bwd_reduce', d_a1.data_ptr(), xi.data_ptr(), A1.data_ptr(), B1.data_ptr(), act,
-                          S1.data_ptr(), B, V, C0, *_scratch(d_a1), s)
-            shortcut_dgrad()
+                   d_a1.data_ptr(), 0, B, T, H, W, C0, ws.data_ptr(), ws.numel(), s)
+        _lib.call('og_affine_act_bwd_reduce', d_a1.data_ptr(), xi.data_ptr(), A1.data_ptr(), B1.data_ptr(), act,
+                  S1.data_ptr(), B, V, C0, *_scratch(d_a1), s)
+        _conv_call('dgrad', 2.0 * B * V * C1 * C0, 'og_conv3d_dgrad', dyb.data_ptr(), C1, C1, packed2.data_ptr(), ld2,
+                   geom2.k_main, 1, 1, 1, 0, 0, 0, dx_res.data_ptr(), 0, B, T, H, W, C0, ws.data_ptr(), ws.numel(), s)
         # (the input gradient is always produced: its pass is also what emits dgamma1 / dbeta1)
         dx = empty_internal(B, C0, T, H, W, bf16, dev)
-        _gn_bwd(d_a1, xi, A1, B1, S1, mr[0], g1w, g1b, G, act, dx_res, dx, dg1w, dg1b, None, B, V, C0, s,
-                reduce=grouped and not FUSE_RED)
+        _gn_bwd(d_a1, xi, A1, B1, S1, mr[0], g1w, g1b, G, act, dx_res, dx, dg1w, dg1b, None, B, V, C0, s, reduce=False)
         return (dx, None, dg1w, dg1b, dw1, db1 if has_b1 else None, dg2w, dg2b, dw2, db2 if has_b2 else None, dwres,
                 (db2.clone() if has_b2 else db2) if has_bres else None, None, None, None, None, None, None, None)
 

@@ -48,8 +48,7 @@ def run(name, model, step_fn, frames, steps=3, warm=2):
     torch.cuda.synchronize()
     out = {'config': name, 'ms_per_step': round(ms, 2), 'frames_per_s': round(frames / ms * 1e3, 1), 'loss': float(loss),
            'params': sum(p.numel() for p in params), 'mem_gb': round(torch.cuda.max_memory_allocated() / 2**30, 1),
-           'tensor_core_kernels': flop_table(steps), 'kernels_ms': kernel_table(steps),
-           'temporal_mma': os.environ.get('OG_TEMPORAL_MMA', '0')}
+           'tensor_core_kernels': flop_table(steps), 'kernels_ms': kernel_table(steps)}
     ops.PROFILE, _lib.TIMING = None, None
     print(json.dumps(out), flush=True)
 

@@ -227,7 +227,7 @@ static bool run_case(const Case& c, bool do_dgrad, bool do_wgrad) {
     CK(cudaMalloc(&dxr, V * c.c0 * 4));
     CK(cudaMemset(dx, 0xFF, V * c.c0 * 4));
     r = og_conv3d_dgrad(dy, c.cout, c.cout, w, ldw, 0, c.kt, c.kh, c.kw, c.pt, c.ph, c.pw, dx, 1, c.N, c.T, c.H, c.W,
-                        c.c0, g_ws, g_ws_bytes, nullptr, nullptr, nullptr, 0, nullptr, 0);
+                        c.c0, g_ws, g_ws_bytes, 0);
     if (r != 0) {
       printf("  og_conv3d_dgrad failed: %d %s\n", r, og_last_error());
       ok = false;
@@ -247,7 +247,7 @@ static bool run_case(const Case& c, bool do_dgrad, bool do_wgrad) {
       CK(cudaMalloc(&dxb, (V * c.c0 + 64) * 2));
       CK(cudaMemset(dxb, 0x7F, (V * c.c0 + 64) * 2));  // canary after the tensor
       r = og_conv3d_dgrad(dy, c.cout, c.cout, w, ldw, 0, c.kt, c.kh, c.kw, c.pt, c.ph, c.pw, dxb, 0, c.N, c.T, c.H, c.W,
-                          c.c0, g_ws, g_ws_bytes, nullptr, nullptr, nullptr, 0, nullptr, 0);
+                          c.c0, g_ws, g_ws_bytes, 0);
       CK(cudaDeviceSynchronize());
       std::vector<__nv_bfloat16> hb(V * c.c0 + 64);
       std::vector<float> hr(V * c.c0);
@@ -266,7 +266,7 @@ static bool run_case(const Case& c, bool do_dgrad, bool do_wgrad) {
       float *dx1, *dx1r;
       CK(cudaMalloc(&dx1, V * c.c1 * 4));
       CK(cudaMalloc(&dx1r, V * c.c1 * 4));
-      r = og_conv3d_dgrad(dy, c.cout, c.cout, w, ldw, ntaps * c.c0, 1, 1, 1, 0, 0, 0, dx1, 1, c.N, c.T, c.H, c.W, c.c1, g_ws, g_ws_bytes, nullptr, nullptr, nullptr, 0, nullptr, 0);
+      r = og_conv3d_dgrad(dy, c.cout, c.cout, w, ldw, ntaps * c.c0, 1, 1, 1, 0, 0, 0, dx1, 1, c.N, c.T, c.H, c.W, c.c1, g_ws, g_ws_bytes, 0);
       if (r != 0) {
         printf("  og_conv3d_dgrad(shortcut) failed: %d %s\n", r, og_last_error());
         ok = false;
@@ -360,7 +360,7 @@ static void bench_case(const Case& c, int iters) {
                           c.N, c.T, c.H, c.W, c.cout, g_ws, g_ws_bytes, nullptr, 0);
       else if (which == 1)
         r = og_conv3d_dgrad(dy, c.cout, c.cout, w, ldw, 0, c.kt, c.kh, c.kw, c.pt, c.ph, c.pw, dx, 0, c.N, c.T, c.H,
-                            c.W, c.c0, g_ws, g_ws_bytes, nullptr, nullptr, nullptr, 0, nullptr, 0);
+                            c.W, c.c0, g_ws, g_ws_bytes, 0);
       else
         r = og_conv3d_wgrad(dy, c.cout, x0, c.c0, dw, (int64_t)ntaps * c.c0, c.kt, c.kh, c.kw, c.pt, c.ph, c.pw, c.N,
                             c.T, c.H, c.W, g_scratch, g_scratch_bytes, 0);
