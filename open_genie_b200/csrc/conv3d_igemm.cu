@@ -15,12 +15,16 @@
 // MN-major B operand (k = cout rows of 64, n = cin contiguous) with mirrored taps, so no transposed
 // weight copy ever exists.
 //
-// Warp roles (256 threads, 1 CTA / SM, persistent over tiles):
-//   warp 0    TMA producer (one elected lane)
-//   warps 1-3 idle (they only complete the first warpgroup: wgmma needs an aligned one)
-//   warps 4-7 one warpgroup: wgmma main loop (128 x BN accumulator = two m64 halves in registers, BN <= 128),
-//             then the epilogue: registers -> fp32 tile in shared memory -> one row per thread -> (+bias) -> global.
-//             The producer keeps filling the stage ring with the next tile's operands meanwhile.
+// Warp roles (384 threads, 1 CTA / SM, persistent over work items; "ping-pong" consumers):
+//   warpgroup 0  producer: warp 0 issues the TMA loads (one elected lane); warps 1-3 only complete the warpgroup.
+//                It gives its registers to the consumers (setmaxnreg 40 / 232).
+//   warpgroups 1, 2  consumers: the CTA's i-th work item belongs to consumer i % 2, which runs its whole wgmma main
+//                loop (128 x BN accumulator = two m64 halves in registers, BN <= 128) and then its epilogue straight
+//                from the accumulator fragments. The main loops run strictly in item order (see kOrderBar), so one
+//                consumer's epilogue overlaps the other consumer's MMAs.
+// Both consumers read ONE stage ring, filled in item order. A consumer steps its ring position over the k-blocks of
+// the other consumer's items; since an mbarrier parity wait cannot tell phase k from k + 2, it may only wait on a
+// `full` barrier once every earlier item's stages have been filled, which the ordering of the main loops guarantees.
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 
@@ -75,25 +79,18 @@ struct IgemmParams {
 static constexpr int kBlockM = 128;
 static constexpr int kBlockK = 64;                       // 64 bf16 = one 128-byte swizzle row
 static constexpr int kABytes = kBlockM * kBlockK * 2;    // 16 KiB
-static constexpr int kMaxStages = 8;
-static constexpr int kThreads = 256;
-// barriers (256) + bias (1024) + 4 warps x 4 KiB store staging + GroupNorm sums (256); the fp32 accumulator tile follows
-static constexpr int kTailBytes = 256 + 1024 + 4 * 4096 + 256;
-__host__ __device__ constexpr int acc_ld(int bn) { return bn + 4; }   // fp32 row stride: conflict-free float4 row reads
-
-template <int NV>
-__device__ __forceinline__ void ld_acc_row(const float* src, uint32_t (&v)[32]) {
-#pragma unroll
-  for (int i = 0; i < NV / 4; ++i) {
-    const float4 f = reinterpret_cast<const float4*>(src)[i];
-    v[4 * i] = __float_as_uint(f.x);
-    v[4 * i + 1] = __float_as_uint(f.y);
-    v[4 * i + 2] = __float_as_uint(f.z);
-    v[4 * i + 3] = __float_as_uint(f.w);
-  }
-#pragma unroll
-  for (int i = NV; i < 32; ++i) v[i] = 0u;
-}
+// Deeper rings fit in shared memory now that the epilogue needs no fp32 tile, but on H100 they measured slower: at
+// BN = 128, 3, 5 and 6 stages all ran the large forward and data-gradient shapes 5-20% slower than 4.
+static constexpr int kMaxStages = 4;
+static constexpr int kThreads = 384;
+// per consumer: bias row of the N tile (BN <= 128 floats) + 4 warps x 4 KiB store staging + GroupNorm sums (2 doubles)
+// + GroupNorm sums of each of the 128 tile rows (float2)
+static constexpr int kConsumerTail = 512 + 4 * 4096 + 64 + 128 * 8;
+// barriers (256), then the two consumers' tails
+static constexpr int kTailBytes = 256 + 2 * kConsumerTail;
+// named barriers: 0 = __syncthreads, 1 + wg = consumer wg's own epilogue, kOrderBar + wg = "consumer wg may start its
+// next main loop" (bar.arrive by the other consumer after it has issued its item's last MMA, bar.sync by wg)
+static constexpr int kOrderBar = 3;
 
 struct TileCoord {
   int n0, t0, h0, w0;
@@ -115,6 +112,35 @@ __device__ __forceinline__ TileCoord decode_m_tile(const IgemmParams& p, int m_t
   return c;
 }
 
+// Output voxel (row index of the output tensor) of row `row` of the M tile at `tc`; false for rows of a partial box.
+// (generalised store position: a strided data gradient writes one residue class of the input grid per launch)
+__device__ __forceinline__ bool tile_row(const IgemmParams& p, const TileCoord& tc, int row, long long& vox) {
+  const int dw = row & ((1 << p.bw_log2) - 1);
+  const int dh = (row >> p.bw_log2) & ((1 << p.bh_log2) - 1);
+  const int dt = (row >> (p.bw_log2 + p.bh_log2)) & ((1 << p.bt_log2) - 1);
+  const int dn = row >> (p.bw_log2 + p.bh_log2 + p.bt_log2);
+  const int vn = tc.n0 + dn, vt = tc.t0 + dt, vh = tc.h0 + dh, vw = tc.w0 + dw;
+  vox = (((long long)vn * p.OT + vt * p.om[0] + p.oo[0]) * p.OH + vh * p.om[1] + p.oo[1]) * p.OW + vw * p.om[2] + p.oo[2];
+  return vn < p.N && vt < p.T && vh < p.H && vw < p.W;
+}
+
+// bias0 + bias1 of output column col (0 past n_out), summed as the epilogues always have: (0 + bias0) + bias1
+__device__ __forceinline__ float bias_at(const IgemmParams& p, int col) {
+  float b = 0.f;
+  if (col < p.n_out) {
+    if (p.bias0) b += __ldg(p.bias0 + col);
+    if (p.bias1) b += __ldg(p.bias1 + col);
+  }
+  return b;
+}
+
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 template <int BN, int BMN>
 __global__ void __launch_bounds__(kThreads, 1)
     og_conv_igemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
@@ -128,10 +154,6 @@ __global__ void __launch_bounds__(kThreads, 1)
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.num_stages * stage_bytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + kMaxStages;
-  float* bias_s = reinterpret_cast<float*>(bars + 32);                    // [256] bias0+bias1 of the current N tile
-  uint8_t* stage_s = reinterpret_cast<uint8_t*>(bars + 32) + 1024;        // 4 warps x 32 rows x 128 B store staging
-  double* stat_s = reinterpret_cast<double*>(stage_s + 4 * 4096);         // [2]
-  float* acc_s = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + kTailBytes);  // [128][acc_ld(BN)] fp32
 
   const int warp = warp_idx_uniform();
   const int lane = threadIdx.x & 31;
@@ -143,16 +165,17 @@ __global__ void __launch_bounds__(kThreads, 1)
     tma_prefetch_desc(&mapB);
     for (int s = 0; s < p.num_stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 4);   // one arrival per consumer warp
+      mbar_init(&empty[s], 4);   // one arrival per warp of the consumer that used the stage
     }
     fence_mbar_init();
   }
   __syncthreads();
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================================== TMA producer =====================================
-    // (all 32 lanes run the loop converged; one elected lane issues — see elect_one() in og_ptx.cuh)
-    {
+    // (all 32 lanes of warp 0 run the loop converged; one elected lane issues — see elect_one() in og_ptx.cuh)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
@@ -218,28 +241,46 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
       }
     }
-  } else if (warp >= 4) {
-    // ============================ wgmma main loop + epilogue (one warpgroup) ============================
-    const int q = warp & 3;  // warp of the warpgroup: wgmma rows 16q..16q+15 of each m64 half; epilogue rows 32q..32q+31
-    const int row = q * 32 + lane;
-    const int et = threadIdx.x - 128;
+  } else {
+    // ============================ consumers: wgmma main loop + epilogue ============================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int wg = (warp >> 2) - 1;   // consumer 0 or 1: the CTA's items i with i % 2 == wg
+    const int q = warp & 3;           // warp of the warpgroup: wgmma rows 16q..16q+15 of each m64 half
+    const int et = threadIdx.x - 128 * (wg + 1);
+    const int epi_bar = 1 + wg;
+    uint8_t* tail = reinterpret_cast<uint8_t*>(bars) + 256 + wg * kConsumerTail;
+    float* bias_s = reinterpret_cast<float*>(tail);                       // [BN] bias0 + bias1 of the current N tile
+    uint8_t* my_stage = tail + 512 + q * 4096;                            // this warp's 32 rows x 128 B store staging
+    double* stat_s = reinterpret_cast<double*>(tail + 512 + 4 * 4096);   // [2]
+    float2* row_s = reinterpret_cast<float2*>(tail + 512 + 4 * 4096 + 64);   // [128] GroupNorm sums of each tile row
+    const int cl = 2 * (lane & 3);   // first of the two columns this thread holds in every 8-column group
     int stage = 0;
     uint32_t phase = 0;
     float fl_s = 0.f, fl_ss = 0.f;
     if (et == 0) stat_s[0] = stat_s[1] = 0.0;
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
+    named_bar_sync(epi_bar, 128);
+    int i = 0;
+    for (int item = blockIdx.x; item < total_tiles; item += gridDim.x, ++i) {
       const int tile = item / p.splits;
       const int split = item - tile * p.splits;
-      const int m_super = tile / p.num_n_tiles;
-      const int n_tile = tile - m_super * p.num_n_tiles;
       const int nkb = (int)(((long long)p.num_kb * (split + 1)) / p.splits) -
                       (int)(((long long)p.num_kb * split) / p.splits);
+      if ((i & 1) != wg) {   // the other consumer's item: step over its k-blocks of the ring
+        stage += nkb;
+        const int wraps = stage / p.num_stages;
+        stage -= wraps * p.num_stages;
+        phase ^= wraps & 1;
+        continue;
+      }
+      const int m_super = tile / p.num_n_tiles;
+      const int n_tile = tile - m_super * p.num_n_tiles;
+      // wait until the other consumer has issued the previous item's last MMA, i.e. waited for all of its stages
+      if (i > 0) named_bar_sync(kOrderBar + wg, 256);
       float acc[2][BN / 2];
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[hh][i] = 0.f;
+        for (int j = 0; j < BN / 2; ++j) acc[hh][j] = 0.f;
       int prev = -1;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(&full[stage], phase);
@@ -265,221 +306,182 @@ __global__ void __launch_bounds__(kThreads, 1)
           phase ^= 1;
         }
       }
+      if (item + gridDim.x < total_tiles) named_bar_arrive(kOrderBar + (wg ^ 1), 256);   // the next item's turn
       wgmma_wait<0>();
       reg_fence(acc[0]);
       reg_fence(acc[1]);
-      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-      // accumulator fragments -> fp32 tile in shared memory; the epilogue below reads one row per thread
-      asm volatile("bar.sync 1, 128;" ::: "memory");   // the previous tile's epilogue is done with acc_s
-      {
-        const int r0 = q * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+      if (lane == 0) mbar_arrive(&empty[prev]);
+
+      // ---- epilogue from the fragments: acc[hh][4j + 2h8 + {0,1}] = tile row hh*64 + 16q + lane/4 + 8h8,
+      //      columns 8j + cl + {0,1}
+      const TileCoord tc = decode_m_tile(p, m_super);
+      const int col0 = n_tile * p.block_n;
+      if (p.splits > 1) {
+        // split-K: store this item's partial sums into its own slab of the fp32 workspace; bias / cast happen in the
+        // finish pass
+        float* ws = p.ws + (long long)split * p.ws_slab + col0;
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            float* d0 = acc_s + (hh * 64 + r0) * acc_ld(BN) + j * 8 + c0;
-            *reinterpret_cast<float2*>(d0) = make_float2(acc[hh][4 * j], acc[hh][4 * j + 1]);
-            *reinterpret_cast<float2*>(d0 + 8 * acc_ld(BN)) = make_float2(acc[hh][4 * j + 2], acc[hh][4 * j + 3]);
-          }
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      const float* acc_row = acc_s + row * acc_ld(BN);
-
-      do {  // one pass; `continue` below leaves it for the tile's common tail
-      const TileCoord tc = decode_m_tile(p, m_super);
-      const int dw = row & ((1 << p.bw_log2) - 1);
-      const int dh = (row >> p.bw_log2) & ((1 << p.bh_log2) - 1);
-      const int dt = (row >> (p.bw_log2 + p.bh_log2)) & ((1 << p.bt_log2) - 1);
-      const int dn = row >> (p.bw_log2 + p.bh_log2 + p.bt_log2);
-      const int vn = tc.n0 + dn, vt = tc.t0 + dt, vh = tc.h0 + dh, vw = tc.w0 + dw;
-      const bool row_ok = vn < p.N && vt < p.T && vh < p.H && vw < p.W;  // partial boxes: masked store
-      // (generalised store position: a strided data gradient writes one residue class of the input grid per launch)
-      const long long vox = (((long long)vn * p.OT + vt * p.om[0] + p.oo[0]) * p.OH + vh * p.om[1] + p.oo[1]) * p.OW +
-                            vw * p.om[2] + p.oo[2];
-      const int col0 = n_tile * p.block_n;
-
-      if (p.splits > 1) {
-        // split-K: store this item's partial sums into its own slab of the fp32 workspace with plain stores (each thread
-        // fills one 128-byte line of its row per chunk); bias / cast happen in the finish pass
-        for (int c = 0; c < p.block_n; c += 32) {
-          if (col0 + c >= p.n_out) break;
-          uint32_t v[32];
-          ld_acc_row<32>(acc_row + c, v);
-          if (row_ok) {
-            float* dst = p.ws + (long long)split * p.ws_slab + vox * p.ldo + col0 + c;
-            if (p.vec_ok && col0 + c + 32 <= p.n_out) {
+          for (int h8 = 0; h8 < 2; ++h8) {
+            long long vox;
+            if (!tile_row(p, tc, hh * 64 + q * 16 + (lane >> 2) + 8 * h8, vox)) continue;
+            float* dst = ws + vox * p.ldo;
 #pragma unroll
-              for (int j = 0; j < 32; j += 4)
-                __stcg(reinterpret_cast<float4*>(dst + j),
-                       make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                                   __uint_as_float(v[j + 3])));
-            } else {
-              for (int j = 0; j < 32; ++j)
-                if (col0 + c + j < p.n_out) dst[j] = __uint_as_float(v[j]);
-            }
-          }
-        }
-        continue;
-      }
-
-      if (p.fast_store) {
-        // bf16 output, whole 64-column chunks: registers -> (bias) -> bf16 -> swizzled smem staging -> the warp
-        // writes 4 full 128-byte row segments per instruction (the row-per-thread accumulator layout would otherwise
-        // scatter 16-byte pieces over 32 different lines per store).
-        {
-          asm volatile("bar.sync 1, 128;" ::: "memory");  // previous tile's bias readers are done
-          for (int j = et; j < p.block_n; j += 128) {
-            const int col = col0 + j;
-            float b = 0.f;
-            if (col < p.n_out) {
-              if (p.bias0) b += __ldg(p.bias0 + col);
-              if (p.bias1) b += __ldg(p.bias1 + col);
-            }
-            bias_s[j] = b;
-          }
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-        }
-        float st_s = 0.f, st_ss = 0.f;
-        uint8_t* my_stage = stage_s + q * 4096;
-        __nv_bfloat16* outp = reinterpret_cast<__nv_bfloat16*>(p.out);
-        for (int c = 0; c < p.block_n; c += 64) {
-          if (col0 + c >= p.n_out) break;  // partial last N tile (n_out % 64 == 0, so chunks are all-or-nothing)
-          uint32_t v0[32], v1[32];
-          ld_acc_row<32>(acc_row + c, v0);
-          ld_acc_row<32>(acc_row + c + 32, v1);
-          if (p.residual && row_ok) {  // fp32 add before the single bf16 rounding
-            const uint4* rp = reinterpret_cast<const uint4*>(p.residual + vox * p.ldo + col0 + c);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const uint4 u = __ldg(rp + j);
-              const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float2 f = __bfloat1622float2(hh[e]);
-                uint32_t* dst = (j < 4) ? &v0[8 * j + 2 * e] : &v1[8 * (j - 4) + 2 * e];
-                dst[0] = __float_as_uint(__uint_as_float(dst[0]) + f.x);
-                dst[1] = __float_as_uint(__uint_as_float(dst[1]) + f.y);
+            for (int j = 0; j < BN / 8; ++j) {
+              const int col = col0 + 8 * j + cl;
+              const float v0 = acc[hh][4 * j + 2 * h8], v1 = acc[hh][4 * j + 2 * h8 + 1];
+              if (p.vec_ok && col + 1 < p.n_out) {
+                __stcg(reinterpret_cast<float2*>(dst + 8 * j + cl), make_float2(v0, v1));
+              } else {
+                if (col < p.n_out) dst[8 * j + cl] = v0;
+                if (col + 1 < p.n_out) dst[8 * j + cl + 1] = v1;
               }
             }
           }
-          // fold the bias in: from here on v0 / v1 are the final fp32 outputs of this row
+      } else if (p.fast_store) {
+        // bf16 output, whole 64-column chunks: fragments (+ residual) + bias -> bf16 -> this warp's swizzled staging
+        // rows -> the warp writes 4 full 128-byte row segments per instruction. Staging row lr (0..31) is tile row
+        // (lr / 16) * 64 + 16q + lr % 16, so the 32 rows are exactly those whose fragments this warp holds.
+        named_bar_sync(epi_bar, 128);   // the previous tile's bias readers are done
+        for (int j = et; j < p.block_n; j += 128) bias_s[j] = bias_at(p, col0 + j);
+        named_bar_sync(epi_bar, 128);
+        long long my_vox;   // lane L: staging row L
+        const int my_ok = tile_row(p, tc, (lane >> 4) * 64 + q * 16 + (lane & 15), my_vox);
+        __nv_bfloat16* outp = reinterpret_cast<__nv_bfloat16*>(p.out) + col0;
+        const __nv_bfloat16* resp = p.residual + col0;
+        const int chunk = lane & 7;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            v0[j] = __float_as_uint(__uint_as_float(v0[j]) + bias_s[c + j]);
-            v1[j] = __float_as_uint(__uint_as_float(v1[j]) + bias_s[c + 32 + j]);
+        for (int c = 0; c < BN; c += 64) {
+          if (col0 + c >= p.n_out) break;   // partial last N tile (n_out % 64 == 0, so chunks are all-or-nothing)
+          if (p.residual) {   // the residual's row segments, coalesced, into the staging rows
+#pragma unroll
+            for (int it = 0; it < 8; ++it) {
+              const int r = it * 4 + (lane >> 3);
+              const long long rvox = __shfl_sync(0xffffffffu, my_vox, r);
+              const int rok = __shfl_sync(0xffffffffu, my_ok, r);
+              uint4 u = make_uint4(0u, 0u, 0u, 0u);
+              if (rok) u = __ldg(reinterpret_cast<const uint4*>(resp + rvox * p.ldo + c + chunk * 8));
+              *reinterpret_cast<uint4*>(my_stage + r * 128 + ((chunk ^ (r & 7)) << 4)) = u;
+            }
+            __syncwarp();
           }
-          if (p.gn_sums && row_ok) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float r0 = __bfloat162float(__float2bfloat16_rn(__uint_as_float(v0[j])));
-              const float r1 = __bfloat162float(__float2bfloat16_rn(__uint_as_float(v1[j])));
-              st_s += r0 + r1;
-              st_ss = fmaf(r0, r0, fmaf(r1, r1, st_ss));
+          for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+            for (int h8 = 0; h8 < 2; ++h8) {
+              const int lr = hh * 16 + h8 * 8 + (lane >> 2);   // lr & 7 == lane >> 2
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj) {
+                const int j = c / 8 + jj;
+                // the staging word of columns c + 8jj + cl + {0,1}: the residual is read from it and the output
+                // written back to it by the same thread
+                uint32_t* w = reinterpret_cast<uint32_t*>(my_stage + lr * 128 + ((jj ^ (lane >> 2)) << 4)) + (lane & 3);
+                float v0 = acc[hh][4 * j + 2 * h8], v1 = acc[hh][4 * j + 2 * h8 + 1];
+                if (p.residual) {   // fp32 add before the single bf16 rounding
+                  const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(w));
+                  v0 += r.x;
+                  v1 += r.y;
+                }
+                const float2 b = *reinterpret_cast<const float2*>(bias_s + c + 8 * jj + cl);
+                *w = pack_bf16x2(v0 + b.x, v1 + b.y);
+              }
+            }
+          __syncwarp();
+          if (p.gn_sums && my_ok) {
+            // GroupNorm(1, C) sums of the bf16-rounded output: lane L sums its staging row L, columns c + j and
+            // c + 32 + j in turn (j < 32). Row by row in this order, then a warp sum over 32 consecutive tile rows
+            // (below), the sums come out with the same bits whatever the warp layout of the accumulators.
+#pragma unroll
+            for (int jc = 0; jc < 4; ++jc) {
+              const uint4 u0 = *reinterpret_cast<const uint4*>(my_stage + lane * 128 + ((jc ^ (lane & 7)) << 4));
+              const uint4 u1 = *reinterpret_cast<const uint4*>(my_stage + lane * 128 + (((jc + 4) ^ (lane & 7)) << 4));
+              const __nv_bfloat162* h0 = reinterpret_cast<const __nv_bfloat162*>(&u0);
+              const __nv_bfloat162* h1 = reinterpret_cast<const __nv_bfloat162*>(&u1);
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const float2 f0 = __bfloat1622float2(h0[e]), f1 = __bfloat1622float2(h1[e]);
+                fl_s += f0.x + f1.x;
+                fl_ss = fmaf(f0.x, f0.x, fmaf(f1.x, f1.x, fl_ss));
+                fl_s += f0.y + f1.y;
+                fl_ss = fmaf(f0.y, f0.y, fmaf(f1.y, f1.y, fl_ss));
+              }
             }
           }
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint4 u;
-            u.x = pack_bf16x2(__uint_as_float(v0[8 * j + 0]), __uint_as_float(v0[8 * j + 1]));
-            u.y = pack_bf16x2(__uint_as_float(v0[8 * j + 2]), __uint_as_float(v0[8 * j + 3]));
-            u.z = pack_bf16x2(__uint_as_float(v0[8 * j + 4]), __uint_as_float(v0[8 * j + 5]));
-            u.w = pack_bf16x2(__uint_as_float(v0[8 * j + 6]), __uint_as_float(v0[8 * j + 7]));
-            *reinterpret_cast<uint4*>(my_stage + lane * 128 + ((j ^ (lane & 7)) << 4)) = u;
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint4 u;
-            u.x = pack_bf16x2(__uint_as_float(v1[8 * j + 0]), __uint_as_float(v1[8 * j + 1]));
-            u.y = pack_bf16x2(__uint_as_float(v1[8 * j + 2]), __uint_as_float(v1[8 * j + 3]));
-            u.z = pack_bf16x2(__uint_as_float(v1[8 * j + 4]), __uint_as_float(v1[8 * j + 5]));
-            u.w = pack_bf16x2(__uint_as_float(v1[8 * j + 6]), __uint_as_float(v1[8 * j + 7]));
-            *reinterpret_cast<uint4*>(my_stage + lane * 128 + (((j + 4) ^ (lane & 7)) << 4)) = u;
-          }
-          __syncwarp();
-          const int chunk = lane & 7;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int r = i * 4 + (lane >> 3);
-            const long long rvox = __shfl_sync(0xffffffffu, vox, r);
-            const int rok = __shfl_sync(0xffffffffu, (int)row_ok, r);
+          for (int it = 0; it < 8; ++it) {
+            const int r = it * 4 + (lane >> 3);
+            const long long rvox = __shfl_sync(0xffffffffu, my_vox, r);
+            const int rok = __shfl_sync(0xffffffffu, my_ok, r);
             const uint4 u = *reinterpret_cast<const uint4*>(my_stage + r * 128 + ((chunk ^ (r & 7)) << 4));
-            if (rok) *reinterpret_cast<uint4*>(outp + rvox * p.ldo + col0 + c + chunk * 8) = u;
+            if (rok) *reinterpret_cast<uint4*>(outp + rvox * p.ldo + c + chunk * 8) = u;
           }
           __syncwarp();
         }
-        fl_s += st_s;
-        fl_ss += st_ss;
-        continue;
-      }
-
-      for (int c = 0; c < p.block_n; c += 32) {
-        uint32_t v[32];
-        if (BN >= 32)
-          ld_acc_row<32>(acc_row + c, v);
-        else
-          ld_acc_row<16>(acc_row + c, v);
-        const int cbase = col0 + c;
-        if (cbase >= p.n_out || !row_ok) continue;
-        float f[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          float b = 0.f;
-          const int col = cbase + j;
-          if (col < p.n_out) {
-            if (p.bias0) b += __ldg(p.bias0 + col);
-            if (p.bias1) b += __ldg(p.bias1 + col);
+        if (p.gn_sums) {
+          // flush this tile's GroupNorm sums (all rows of a CTA tile belong to one sample: host-checked). The row
+          // sums go through shared memory so that warp w adds those of tile rows 32w .. 32w + 31.
+          row_s[(lane >> 4) * 64 + q * 16 + (lane & 15)] = make_float2(fl_s, fl_ss);
+          named_bar_sync(epi_bar, 128);
+          const float2 rs = row_s[q * 32 + lane];
+          fl_s = rs.x;
+          fl_ss = rs.y;
+          for (int o = 16; o > 0; o >>= 1) {
+            fl_s += __shfl_xor_sync(0xffffffffu, fl_s, o);
+            fl_ss += __shfl_xor_sync(0xffffffffu, fl_ss, o);
           }
-          f[j] = __uint_as_float(v[j]) + b;
-          if (p.residual && col < p.n_out && row_ok) f[j] += __bfloat162float(p.residual[vox * p.ldo + col]);
+          if (lane == 0) {
+            atomicAdd(&stat_s[0], (double)fl_s);
+            atomicAdd(&stat_s[1], (double)fl_ss);
+          }
+          named_bar_sync(epi_bar, 128);
+          if (et == 0) {
+            atomicAdd(&p.gn_sums[(long long)tc.n0 * 2], stat_s[0]);
+            atomicAdd(&p.gn_sums[(long long)tc.n0 * 2 + 1], stat_s[1]);
+            stat_s[0] = 0.0;
+            stat_s[1] = 0.0;
+          }
+          fl_s = fl_ss = 0.f;
         }
-        if (p.out_f32) {
-          float* o = reinterpret_cast<float*>(p.out) + vox * p.ldo + cbase;
-          if (p.vec_ok && cbase + 32 <= p.n_out) {
+      } else {
+        // fp32 output, BN < 64 or n_out not a multiple of 64: masked stores straight from the fragments,
+        // (acc + bias) + residual
 #pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              *reinterpret_cast<float4*>(o + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-          } else {
-            for (int j = 0; j < 32; ++j)
-              if (cbase + j < p.n_out) o[j] = f[j];
-          }
-        } else {
-          __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + vox * p.ldo + cbase;
-          if (p.vec_ok && cbase + 32 <= p.n_out) {
+        for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-              uint4 u;
-              u.x = pack_bf16x2(f[j], f[j + 1]);
-              u.y = pack_bf16x2(f[j + 2], f[j + 3]);
-              u.z = pack_bf16x2(f[j + 4], f[j + 5]);
-              u.w = pack_bf16x2(f[j + 6], f[j + 7]);
-              *reinterpret_cast<uint4*>(o + j) = u;
+          for (int h8 = 0; h8 < 2; ++h8) {
+            long long vox;
+            if (!tile_row(p, tc, hh * 64 + q * 16 + (lane >> 2) + 8 * h8, vox)) continue;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+              const int col = col0 + 8 * j + cl;
+              if (col >= p.n_out) continue;
+              const bool two = col + 1 < p.n_out;
+              float f0 = acc[hh][4 * j + 2 * h8] + bias_at(p, col);
+              float f1 = acc[hh][4 * j + 2 * h8 + 1] + bias_at(p, col + 1);
+              if (p.residual) {
+                f0 += __bfloat162float(p.residual[vox * p.ldo + col]);
+                if (two) f1 += __bfloat162float(p.residual[vox * p.ldo + col + 1]);
+              }
+              if (p.out_f32) {
+                float* o = reinterpret_cast<float*>(p.out) + vox * p.ldo + col;
+                if (p.vec_ok && two) {
+                  *reinterpret_cast<float2*>(o) = make_float2(f0, f1);
+                } else {
+                  o[0] = f0;
+                  if (two) o[1] = f1;
+                }
+              } else {
+                __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + vox * p.ldo + col;
+                if (p.vec_ok && two) {
+                  *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(f0, f1);
+                } else {
+                  o[0] = __float2bfloat16_rn(f0);
+                  if (two) o[1] = __float2bfloat16_rn(f1);
+                }
+              }
             }
-          } else {
-            for (int j = 0; j < 32; ++j)
-              if (cbase + j < p.n_out) o[j] = __float2bfloat16_rn(f[j]);
           }
-        }
-      }
-      } while (0);
-      if (p.fast_store && p.splits == 1 && p.gn_sums) {
-        // flush this tile's GroupNorm sums (all rows of a CTA tile belong to one sample: host-checked)
-        const TileCoord tcf = decode_m_tile(p, m_super);
-        for (int o = 16; o > 0; o >>= 1) {
-          fl_s += __shfl_xor_sync(0xffffffffu, fl_s, o);
-          fl_ss += __shfl_xor_sync(0xffffffffu, fl_ss, o);
-        }
-        if (lane == 0) {
-          atomicAdd(&stat_s[0], (double)fl_s);
-          atomicAdd(&stat_s[1], (double)fl_ss);
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (et == 0) {
-          atomicAdd(&p.gn_sums[(long long)tcf.n0 * 2], stat_s[0]);
-          atomicAdd(&p.gn_sums[(long long)tcf.n0 * 2 + 1], stat_s[1]);
-          stat_s[0] = 0.0;
-          stat_s[1] = 0.0;
-        }
-        fl_s = fl_ss = 0.f;
       }
     }
   }
@@ -692,11 +694,10 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
       }
     }
   }
-  const int tail_bytes = kTailBytes + kBlockM * acc_ld(p.block_n) * 4 /*fp32 accumulator tile*/;
-  int stages = (227 * 1024 - 1024 /*align slack*/ - tail_bytes) / stage_bytes;
+  int stages = (227 * 1024 - 1024 /*align slack*/ - kTailBytes) / stage_bytes;
   if (stages > kMaxStages) stages = kMaxStages;
   p.num_stages = stages;
-  const size_t smem_bytes = (size_t)stages * stage_bytes + 1024 + tail_bytes;
+  const size_t smem_bytes = (size_t)stages * stage_bytes + 1024 + kTailBytes;
 
   CUtensorMap mapA0, mapA1, mapB;
   {
