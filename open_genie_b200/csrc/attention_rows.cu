@@ -829,8 +829,13 @@ extern "C" int og_temporal_attn_fwd(const void* q, const void* k, const void* v,
                                     og_stream_t stream) {
   OG_REQUIRE(q && k && v && out, "temporal_attn_fwd: null pointer");
   OG_REQUIRE(T >= 1 && T <= 32, "temporal_attn_fwd: T=%d must be in [1,32]", T);
+  OG_REQUIRE(B >= 1 && P >= 1, "temporal_attn_fwd: empty problem (B=%d, P=%lld)", B, (long long)P);
   OG_REQUIRE(n_head >= 1 && C % n_head == 0, "temporal_attn_fwd: C=%d not divisible by n_head=%d", C, n_head);
   const int D = C / n_head;
+  if (D != 32 && D != 64) {
+    set_error("temporal_attn_fwd: d_head=%d not supported (32 or 64)", D);
+    return OG_ERR_UNSUPPORTED_SHAPE;
+  }
   if (temporal_mma_enabled(D, T, C))
     return launch_temporal_fwd_mma(q, k, v, residual, out, B, T, P, C, n_head, scale, kv_bcast, (cudaStream_t)stream);
   const long long ntask = (long long)B * P * n_head;
@@ -841,14 +846,10 @@ extern "C" int og_temporal_attn_fwd(const void* q, const void* k, const void* v,
     og_temporal_attn_fwd_kernel<64><<<(unsigned)grid, 128, smem, (cudaStream_t)stream>>>(
         (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)residual,
         (__nv_bfloat16*)out, B, T, P, C, n_head, scale, kv_bcast);
-  else if (D == 32)
+  else
     og_temporal_attn_fwd_kernel<32><<<(unsigned)grid, 128, smem, (cudaStream_t)stream>>>(
         (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)residual,
         (__nv_bfloat16*)out, B, T, P, C, n_head, scale, kv_bcast);
-  else {
-    set_error("temporal_attn_fwd: d_head=%d not supported (32 or 64)", D);
-    return OG_ERR_UNSUPPORTED_SHAPE;
-  }
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   return OG_OK;
@@ -860,8 +861,13 @@ extern "C" int og_temporal_attn_bwd(const void* q, const void* k, const void* v,
   OG_REQUIRE(q && k && v && dout && dq, "temporal_attn_bwd: null pointer");
   OG_REQUIRE(kv_bcast ? (dk_bcast && dv_bcast) : (dk && dv), "temporal_attn_bwd: missing dk/dv buffers");
   OG_REQUIRE(T >= 1 && T <= 32, "temporal_attn_bwd: T=%d must be in [1,32]", T);
+  OG_REQUIRE(B >= 1 && P >= 1, "temporal_attn_bwd: empty problem (B=%d, P=%lld)", B, (long long)P);
   OG_REQUIRE(n_head >= 1 && C % n_head == 0, "temporal_attn_bwd: C=%d not divisible by n_head=%d", C, n_head);
   const int D = C / n_head;
+  if (D != 32 && D != 64) {
+    set_error("temporal_attn_bwd: d_head=%d not supported (32 or 64)", D);
+    return OG_ERR_UNSUPPORTED_SHAPE;
+  }
   if (temporal_mma_enabled(D, T, C))
     return launch_temporal_bwd_mma(q, k, v, dout, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale, kv_bcast,
                                    (cudaStream_t)stream);
@@ -881,7 +887,7 @@ extern "C" int og_temporal_attn_bwd(const void* q, const void* k, const void* v,
         (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)dout,
         (__nv_bfloat16*)dq, (__nv_bfloat16*)dk, (__nv_bfloat16*)dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale,
         kv_bcast);
-  } else if (D == 32) {
+  } else {
     static bool attr = false;
     if (!attr) {
       OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_bwd_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -892,9 +898,6 @@ extern "C" int og_temporal_attn_bwd(const void* q, const void* k, const void* v,
         (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)dout,
         (__nv_bfloat16*)dq, (__nv_bfloat16*)dk, (__nv_bfloat16*)dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale,
         kv_bcast);
-  } else {
-    set_error("temporal_attn_bwd: d_head=%d not supported (32 or 64)", D);
-    return OG_ERR_UNSUPPORTED_SHAPE;
   }
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);

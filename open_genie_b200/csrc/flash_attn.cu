@@ -431,6 +431,8 @@ extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, co
                                  int C, int n_head, float scale, og_stream_t stream) {
   OG_REQUIRE(q && k && v && out && dout && lse && delta_ws && dq && dk && dv, "flash_attn_bwd: null pointer");
   OG_REQUIRE(n_head >= 1 && C == n_head * kD, "flash_attn_bwd: needs d_head = 64 (C=%d, n_head=%d)", C, n_head);
+  OG_REQUIRE(nseq > 0 && S > 0, "flash_attn_bwd: empty problem");
+  OG_REQUIRE(scale > 0.f, "flash_attn_bwd: scale must be positive (as in the forward pass)");
   cudaStream_t s = (cudaStream_t)stream;
   const long long rows = (long long)nseq * S;
   {

@@ -1,6 +1,8 @@
 // temporal_attn_mma.cu — tensor-core form of the temporal (causal, T <= 16, d_head = 64) attention.
 //
-// STATUS: checked by tests/test_gpu_attention.py and the full-size LatentAction / Dynamics parity tests; the default path; OG_TEMPORAL_MMA=0 falls back to the per-lane kernels in attention_rows.cu.
+// STATUS: checked by tests/test_gpu_attention.py, tests/test_gpu_attention_paths.py and the full-size LatentAction /
+// Dynamics parity tests; always used for d_head = 64, T <= 16 (temporal_mma_enabled in attention_rows.cu), the per-lane
+// kernels there cover the other shapes.
 // SASS: LDSM / HMMA.16816.F32.BF16.
 //
 // Why: one (batch, pixel, head) task is a 16 x 16 x 64 score tile and a 16 x 64 x 16 value product. The per-lane
@@ -416,7 +418,7 @@ __global__ void __launch_bounds__(128)
 
 }  // namespace tmma
 
-// launchers used by og_temporal_attn_fwd / og_temporal_attn_bwd (attention_rows.cu) when OG_TEMPORAL_MMA=1
+// launchers used by og_temporal_attn_fwd / og_temporal_attn_bwd (attention_rows.cu) for d_head = 64, T <= 16
 int launch_temporal_fwd_mma(const void* q, const void* k, const void* v, const void* residual, void* out, int B, int T,
                             long long P, int C, int n_head, float scale, int kv_bcast, cudaStream_t stream) {
   const long long ntask = (long long)B * P * n_head;
