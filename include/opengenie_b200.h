@@ -132,7 +132,7 @@ int og_conv3d_strided_wgrad(const void* dy, int cout, const void* x, int cin, fl
  * ---------------------------------------------------------------------------------------------- */
 
 /* sums[n][g] = (sum x, sum x^2) over the group, accumulated in fp64 (caller zeroes sums: N*G*2 doubles).
- * x: bf16 [N,V,C]; C % 8 == 0, (C/G) % 8 == 0, G <= 64. */
+ * x: bf16 [N,V,C]; C % 8 == 0, C <= 2048, 1 <= G <= 64, C % G == 0 ((C/G) % 8 != 0 takes a per-channel kernel). */
 int og_gn_stats(const void* x, int N, int64_t V, int C, int G, double* sums, og_stream_t stream);
 
 /* Folds statistics, affine (gamma, beta: fp32 [C] or NULL) and the optional AdaGN modulation
@@ -177,7 +177,11 @@ int og_adagn_cond_bwd(const float* dscale, const float* dshift, const float* cba
                       const float* w_shift, int N, int64_t V, int D, int C, float* dw_scale, float* db_scale,
                       float* dw_shift, float* db_shift, float* dcond, og_stream_t stream);
 
-/* One-launch forms of the two pairs above, used on the training hot path (same math, same outputs):
+/* One-launch forms of the two pairs above, used on the training hot path. Same math, but not bit for bit: A, B,
+ * mean_rstd, dgamma, dbeta and dcond_* come out identical to the two-launch forms, and so does y except for SiLU
+ * (h (1 + tanh h) with h = pre/2 against pre * sigmoid(pre): at most one bf16 ulp apart). dx is formed as
+ * fma(A, dpre, fma(Q, x, R)) rather than A*dpre + (Q*x + R), so its last bits can differ, by many ulps where dx
+ * nearly cancels; both forms stay within the same error bound (tests/test_gpu_norm_act_paths.py).
  * og_gn_act_fwd  = og_gn_finalize + og_affine_act_fwd  (A, B, mean_rstd are still written for backward);
  * og_gn_act_bwd  = og_gn_bwd_finalize + og_affine_act_bwd_apply, S/mean_rstd NULL => pure activation backward.
  * dx_colsum (optional, float[C], ACCUMULATED) receives sum over rows of dx — the bias gradient of the
