@@ -25,6 +25,20 @@
 // Both consumers read ONE stage ring, filled in item order. A consumer steps its ring position over the k-blocks of
 // the other consumer's items; since an mbarrier parity wait cannot tell phase k from k + 2, it may only wait on a
 // `full` barrier once every earlier item's stages have been filled, which the ordering of the main loops guarantees.
+//
+// Wide tiles (WIDE = true, 128 voxels x 256 channels, for the layers with 256 or more output channels; launch_igemm
+// says which): both consumers work on every item, consumer wg on tile rows 64wg..64wg+63 against the whole 256-column B
+// tile (m64n256k16, 128 fp32 accumulators per thread). A stage is 16 KiB of A + 32 KiB of B, and the A box and B tile
+// are read from shared memory once per 128 x 256 outputs instead of once per 128 x 128 (B) or twice (A, when two N tiles
+// cover 256 channels). The epilogues then no longer overlap the other consumer's MMAs: only the producer runs ahead.
+// The k-blocks are added in the same order as in the ping-pong kernel, so the output has the same bits.
+//
+// Swapped tiles (SWAP = true, for 128 output channels over many voxels): a layer with 128 output channels has no second
+// N tile to widen, so the tile grows along the voxels instead, with the operands swapped: D^T[channel][voxel] =
+// W[channel][k] . X[voxel][k]^T. The weights are the wgmma A operand (consumer wg: channels 64wg..64wg+63; in the data
+// gradient they are MN-major and read with the A-transpose bit), and a 256-voxel activation box, K-major as it lands
+// from TMA, is B (m64n256k16). The epilogue transposes the [channel][voxel] fragments with stmatrix.trans through a
+// shared buffer so that every row store is a whole 256-byte NDHWC row.
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 
@@ -88,6 +102,15 @@ static constexpr int kThreads = 384;
 static constexpr int kConsumerTail = 512 + 4 * 4096 + 64 + 128 * 8;
 // barriers (256), then the two consumers' tails
 static constexpr int kTailBytes = 256 + 2 * kConsumerTail;
+// wide tile (kWideN = 256 columns, both consumers on every item), per consumer: bias row of the N tile (256 floats) +
+// 4 warps x 2 KiB store staging + GroupNorm sums (2 doubles) + GroupNorm sums of its 64 tile rows per column half (float2)
+static constexpr int kWideN = 256;
+static constexpr int kWideConsumerTail = 1024 + 4 * 2048 + 64 + 2 * 64 * 8;
+static constexpr int kWideTailBytes = 256 + 2 * kWideConsumerTail;
+// swapped tile (256 voxels x 128 channels): barriers, a [64 voxels][128 channels] bf16 transpose buffer shared by both
+// consumers, GroupNorm sums (2 doubles)
+static constexpr int kSwapVox = 256;
+static constexpr int kSwapTailBytes = 256 + 64 * 256 + 64;
 // named barriers: 0 = __syncthreads, 1 + wg = consumer wg's own epilogue, kOrderBar + wg = "consumer wg may start its
 // next main loop" (bar.arrive by the other consumer after it has issued its item's last MMA, bar.sync by wg)
 static constexpr int kOrderBar = 3;
@@ -141,15 +164,19 @@ __device__ __forceinline__ void named_bar_arrive(int id, int count) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
-template <int BN, int BMN>
+// WIDE: 128 x 256 tiles, both consumers on every item (see the file header); BN = kWideN, unsplit launches with bf16
+// staged stores only (launch_igemm). SWAP (with WIDE): 256 voxels x 128 output channels with the operands swapped,
+// D^T[channel][voxel] = W[channel][k] . X[voxel][k]^T; the activation box (256 voxels) is the wgmma B operand.
+template <int BN, int BMN, bool WIDE, bool SWAP = false>
 __global__ void __launch_bounds__(kThreads, 1)
     og_conv_igemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
                          const __grid_constant__ CUtensorMap mapB, const IgemmParams p) {
+  static_assert(!SWAP || WIDE, "the swapped tile is a wide tile");
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment: required by the 128-byte swizzle pattern shared by TMA and the wgmma descriptors
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int b_bytes = p.block_n * kBlockK * 2;
-  const int a_bytes = kABytes;
+  const int b_bytes = p.block_n * kBlockK * 2;                 // weights
+  const int a_bytes = SWAP ? kSwapVox * kBlockK * 2 : kABytes;   // activation box
   const int stage_bytes = a_bytes + b_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.num_stages * stage_bytes);
   uint64_t* full = bars;
@@ -165,7 +192,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     tma_prefetch_desc(&mapB);
     for (int s = 0; s < p.num_stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 4);   // one arrival per warp of the consumer that used the stage
+      mbar_init(&empty[s], WIDE ? 8 : 4);   // one arrival per warp of the consumer(s) that used the stage
     }
     fence_mbar_init();
   }
@@ -203,8 +230,10 @@ __global__ void __launch_bounds__(kThreads, 1)
           const int dt = sg.sh0[0] + jt * sg.shstep[0], dh = sg.sh0[1] + jh * sg.shstep[1],
                     dw = sg.sh0[2] + jw * sg.shstep[2];
           mbar_wait(&empty[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * stage_bytes;
-          uint8_t* sb = sa + a_bytes;
+          // stage = [activation box][weights], or [weights][activation box] for the swapped tile (the weights are then
+          // the wgmma A operand, whose m64 halves start 8 KiB apart)
+          uint8_t* sa = smem + stage * stage_bytes + (SWAP ? b_bytes : 0);
+          uint8_t* sb = smem + stage * stage_bytes + (SWAP ? 0 : a_bytes);
           if (elect_one()) {
             mbar_expect_tx(&full[stage], (uint32_t)stage_bytes);
             tma_load_5d(sa, mapA, &full[stage], cb * kBlockK, aw0 + dw, ah0 + dh, at0 + dt, tc.n0);
@@ -239,6 +268,260 @@ __global__ void __launch_bounds__(kThreads, 1)
             }
           }
         }
+      }
+    }
+  } else if constexpr (SWAP) {
+    // ====== swapped tile: consumer wg = output channels 64wg..64wg+63 x all 256 voxels (m64n256), then the epilogue ======
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int wg = (warp >> 2) - 1;
+    const int q = warp & 3;
+    const int ct = threadIdx.x - 128;   // 0..255 over both consumers
+    uint8_t* tbuf = reinterpret_cast<uint8_t*>(bars) + 256;                  // [64 voxels][128 channels] bf16, swizzled
+    double* stat_s = reinterpret_cast<double*>(tbuf + 64 * 256);            // [2]
+    // this thread's two channel rows: 64wg + 16q + lane/4 (+ 8)
+    const int ch0 = 64 * wg + 16 * q + (lane >> 2);
+    const float bias_lo = bias_at(p, ch0), bias_hi = bias_at(p, ch0 + 8);
+    int stage = 0;
+    uint32_t phase = 0;
+    if (ct == 0) stat_s[0] = stat_s[1] = 0.0;
+    for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
+      float acc[BN / 2];
+#pragma unroll
+      for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t w_addr = smem_u32(smem + stage * stage_bytes) + wg * 8192;   // this consumer's 64 channels
+        const uint32_t x_addr = smem_u32(smem + stage * stage_bytes) + b_bytes;     // [256 voxels][64 k]
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) {
+          // weights: K-major [128 channel rows][64 k] (forward), or MN-major [64 k rows][64 channels] per 64-channel
+          // panel (data gradient: w[co][tap][ci] has ci contiguous), read with the A-transpose bit
+          const uint64_t adesc = BMN ? gmma_desc_sw128(w_addr + k * 2048, 64 * 128, 1024)
+                                     : gmma_desc_sw128(w_addr + k * 32, 16, 1024);
+          wgmma_ss<BN, BMN, 0>(acc, adesc, gmma_desc_sw128(x_addr + k * 32, 16, 1024), 1);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == p.num_stages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (lane == 0) mbar_arrive(&empty[prev]);
+
+      // ---- epilogue (no residual: host-checked): acc[4j + 2h8 + {0,1}] = channel ch0 + 8h8, voxels 8j + 2(lane%4) +
+      //      {0,1}. Per 64-voxel chunk both consumers transpose their fragments + bias into tbuf with stmatrix.trans,
+      //      then all 256 threads store whole 256-byte NDHWC rows. 16-byte chunk c of row r sits at chunk c ^ (r % 8):
+      //      the 8 rows of one 8x8 matrix then fall in 8 different bank groups.
+      const TileCoord tc = decode_m_tile(p, item);
+      float fl_s = 0.f, fl_ss = 0.f;
+#pragma unroll
+      for (int vc = 0; vc < 4; ++vc) {
+        named_bar_sync(1, 256);   // the previous chunk's rows have been read out of tbuf
+#pragma unroll
+        for (int jp = 0; jp < 4; ++jp) {
+          const int j = 8 * vc + 2 * jp;   // matrices m = 0..3: (voxel group j + m/2, channel half m%2)
+          const int m = lane >> 3, r = 16 * jp + 8 * (m >> 1) + (lane & 7), c16 = 8 * wg + 2 * q + (m & 1);
+          stmatrix_x4_trans(smem_u32(tbuf + r * 256 + ((c16 ^ (r & 7)) << 4)),
+                            pack_bf16x2(acc[4 * j] + bias_lo, acc[4 * j + 1] + bias_lo),
+                            pack_bf16x2(acc[4 * j + 2] + bias_hi, acc[4 * j + 3] + bias_hi),
+                            pack_bf16x2(acc[4 * j + 4] + bias_lo, acc[4 * j + 5] + bias_lo),
+                            pack_bf16x2(acc[4 * j + 6] + bias_hi, acc[4 * j + 7] + bias_hi));
+        }
+        named_bar_sync(1, 256);
+#pragma unroll
+        for (int it = 0; it < 4; ++it) {
+          const int idx = it * 256 + ct, r = idx >> 4, c16 = idx & 15;
+          long long vox;
+          if (!tile_row(p, tc, vc * 64 + r, vox)) continue;
+          const uint4 u = *reinterpret_cast<const uint4*>(tbuf + r * 256 + ((c16 ^ (r & 7)) << 4));
+          reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + vox * p.ldo)[c16] = u;
+          if (p.gn_sums) {   // GroupNorm(1, C) sums of the bf16-rounded output
+            const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float2 f = __bfloat1622float2(h[e]);
+              fl_s += f.x + f.y;
+              fl_ss = fmaf(f.x, f.x, fmaf(f.y, f.y, fl_ss));
+            }
+          }
+        }
+      }
+      if (p.gn_sums) {   // all voxels of a tile belong to one sample (host-checked)
+        for (int o = 16; o > 0; o >>= 1) {
+          fl_s += __shfl_xor_sync(0xffffffffu, fl_s, o);
+          fl_ss += __shfl_xor_sync(0xffffffffu, fl_ss, o);
+        }
+        if (lane == 0) {
+          atomicAdd(&stat_s[0], (double)fl_s);
+          atomicAdd(&stat_s[1], (double)fl_ss);
+        }
+        named_bar_sync(1, 256);
+        if (ct == 0) {
+          atomicAdd(&p.gn_sums[(long long)tc.n0 * 2], stat_s[0]);
+          atomicAdd(&p.gn_sums[(long long)tc.n0 * 2 + 1], stat_s[1]);
+          stat_s[0] = 0.0;
+          stat_s[1] = 0.0;
+        }
+      }
+    }
+  } else if constexpr (WIDE) {
+    // ================= wide tile: both consumers on every item, m64n256 each, then the epilogue =================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int wg = (warp >> 2) - 1;   // tile rows 64 wg .. 64 wg + 63
+    const int q = warp & 3;           // wgmma rows 16q..16q+15 of this consumer's m64 half
+    const int et = threadIdx.x - 128 * (wg + 1);
+    const int epi_bar = 1 + wg;
+    uint8_t* tail = reinterpret_cast<uint8_t*>(bars) + 256 + wg * kWideConsumerTail;
+    float* bias_s = reinterpret_cast<float*>(tail);                        // [BN] bias0 + bias1 of the current N tile
+    uint8_t* my_stage = tail + 1024 + q * 2048;                            // this warp's 16 rows x 128 B store staging
+    double* stat_s = reinterpret_cast<double*>(tail + 1024 + 4 * 2048);   // [2]
+    float2* row_s = reinterpret_cast<float2*>(tail + 1024 + 4 * 2048 + 64);   // [2 column halves][64 tile rows]
+    const int cl = 2 * (lane & 3);
+    int stage = 0;
+    uint32_t phase = 0;
+    float fl_s[2] = {0.f, 0.f}, fl_ss[2] = {0.f, 0.f};   // GroupNorm row sums of columns 0-127 and 128-255
+    if (et == 0) stat_s[0] = stat_s[1] = 0.0;
+    for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
+      const int m_super = item / p.num_n_tiles;
+      const int n_tile = item - m_super * p.num_n_tiles;
+      float acc[BN / 2];
+#pragma unroll
+      for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t a_addr = smem_u32(smem + stage * stage_bytes) + wg * 8192;   // this consumer's 64 A rows
+        const uint32_t b_addr = smem_u32(smem + stage * stage_bytes) + a_bytes;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) {
+          const uint64_t bdesc = BMN ? gmma_desc_sw128(b_addr + k * 2048, 64 * 128, 1024)
+                                     : gmma_desc_sw128(b_addr + k * 32, 16, 1024);
+          wgmma_ss<BN, 0, BMN>(acc, gmma_desc_sw128(a_addr + k * 32, 16, 1024), bdesc, 1);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous k-block's MMAs are done: its stage goes back to the producer
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == p.num_stages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (lane == 0) mbar_arrive(&empty[prev]);
+
+      // ---- epilogue: acc[4j + 2h8 + {0,1}] = tile row 64 wg + 16q + lane/4 + 8h8, columns 8j + cl + {0,1}. Per
+      //      64-column chunk: fragments (+ residual) + bias -> bf16 -> this warp's 16 swizzled staging rows (staging
+      //      row lr = tile row 64 wg + 16q + lr) -> 128-byte row segments, 2 rows per lane and instruction.
+      const TileCoord tc = decode_m_tile(p, m_super);
+      const int col0 = n_tile * BN;
+      named_bar_sync(epi_bar, 128);   // the previous tile's bias readers are done
+      for (int j = et; j < BN; j += 128) bias_s[j] = bias_at(p, col0 + j);
+      named_bar_sync(epi_bar, 128);
+      long long my_vox;   // lanes L and L + 16: staging row L % 16
+      const int my_ok = tile_row(p, tc, wg * 64 + q * 16 + (lane & 15), my_vox);
+      __nv_bfloat16* outp = reinterpret_cast<__nv_bfloat16*>(p.out) + col0;
+      const __nv_bfloat16* resp = p.residual + col0;
+      const int chunk = lane & 7;
+#pragma unroll
+      for (int c = 0; c < BN; c += 64) {
+        if (col0 + c >= p.n_out) break;   // partial last N tile (n_out % 64 == 0, so chunks are all-or-nothing)
+        if (p.residual) {
+#pragma unroll
+          for (int it = 0; it < 4; ++it) {
+            const int r = it * 4 + (lane >> 3);
+            const long long rvox = __shfl_sync(0xffffffffu, my_vox, r);
+            const int rok = __shfl_sync(0xffffffffu, my_ok, r);
+            uint4 u = make_uint4(0u, 0u, 0u, 0u);
+            if (rok) u = __ldg(reinterpret_cast<const uint4*>(resp + rvox * p.ldo + c + chunk * 8));
+            *reinterpret_cast<uint4*>(my_stage + r * 128 + ((chunk ^ (r & 7)) << 4)) = u;
+          }
+          __syncwarp();
+        }
+#pragma unroll
+        for (int h8 = 0; h8 < 2; ++h8) {
+          const int lr = h8 * 8 + (lane >> 2);   // lr & 7 == lane >> 2
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = c / 8 + jj;
+            uint32_t* w = reinterpret_cast<uint32_t*>(my_stage + lr * 128 + ((jj ^ (lane >> 2)) << 4)) + (lane & 3);
+            float v0 = acc[4 * j + 2 * h8], v1 = acc[4 * j + 2 * h8 + 1];
+            if (p.residual) {   // fp32 add before the single bf16 rounding
+              const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(w));
+              v0 += r.x;
+              v1 += r.y;
+            }
+            const float2 b = *reinterpret_cast<const float2*>(bias_s + c + 8 * jj + cl);
+            *w = pack_bf16x2(v0 + b.x, v1 + b.y);
+          }
+        }
+        __syncwarp();
+        if (p.gn_sums && my_ok && lane < 16) {
+          // GroupNorm(1, C) sums of the bf16-rounded output: lane L < 16 sums staging row L in the order of the
+          // ping-pong epilogue, one row sum per 128-column half (that kernel's N tile), so the sums keep their bits
+          const int hf = c >> 7;
+#pragma unroll
+          for (int jc = 0; jc < 4; ++jc) {
+            const uint4 u0 = *reinterpret_cast<const uint4*>(my_stage + lane * 128 + ((jc ^ (lane & 7)) << 4));
+            const uint4 u1 = *reinterpret_cast<const uint4*>(my_stage + lane * 128 + (((jc + 4) ^ (lane & 7)) << 4));
+            const __nv_bfloat162* h0 = reinterpret_cast<const __nv_bfloat162*>(&u0);
+            const __nv_bfloat162* h1 = reinterpret_cast<const __nv_bfloat162*>(&u1);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float2 f0 = __bfloat1622float2(h0[e]), f1 = __bfloat1622float2(h1[e]);
+              fl_s[hf] += f0.x + f1.x;
+              fl_ss[hf] = fmaf(f0.x, f0.x, fmaf(f1.x, f1.x, fl_ss[hf]));
+              fl_s[hf] += f0.y + f1.y;
+              fl_ss[hf] = fmaf(f0.y, f0.y, fmaf(f1.y, f1.y, fl_ss[hf]));
+            }
+          }
+        }
+#pragma unroll
+        for (int it = 0; it < 4; ++it) {
+          const int r = it * 4 + (lane >> 3);
+          const long long rvox = __shfl_sync(0xffffffffu, my_vox, r);
+          const int rok = __shfl_sync(0xffffffffu, my_ok, r);
+          const uint4 u = *reinterpret_cast<const uint4*>(my_stage + r * 128 + ((chunk ^ (r & 7)) << 4));
+          if (rok) *reinterpret_cast<uint4*>(outp + rvox * p.ldo + c + chunk * 8) = u;
+        }
+        __syncwarp();
+      }
+      if (p.gn_sums) {
+        // flush this tile's sums (all rows of a CTA tile belong to one sample: host-checked). Warp q adds the row sums
+        // of column half q / 2 over 32 consecutive tile rows, exactly as the ping-pong kernel does per N tile; the
+        // double sum of those fp32 partials does not depend on their order.
+        if (lane < 16) {
+          row_s[q * 16 + lane] = make_float2(fl_s[0], fl_ss[0]);
+          row_s[64 + q * 16 + lane] = make_float2(fl_s[1], fl_ss[1]);
+        }
+        named_bar_sync(epi_bar, 128);
+        const float2 rs = row_s[(q >> 1) * 64 + (q & 1) * 32 + lane];
+        float s = rs.x, ss = rs.y;
+        for (int o = 16; o > 0; o >>= 1) {
+          s += __shfl_xor_sync(0xffffffffu, s, o);
+          ss += __shfl_xor_sync(0xffffffffu, ss, o);
+        }
+        if (lane == 0) {
+          atomicAdd(&stat_s[0], (double)s);
+          atomicAdd(&stat_s[1], (double)ss);
+        }
+        named_bar_sync(epi_bar, 128);
+        if (et == 0) {
+          atomicAdd(&p.gn_sums[(long long)tc.n0 * 2], stat_s[0]);
+          atomicAdd(&p.gn_sums[(long long)tc.n0 * 2 + 1], stat_s[1]);
+          stat_s[0] = 0.0;
+          stat_s[1] = 0.0;
+        }
+        fl_s[0] = fl_s[1] = fl_ss[0] = fl_ss[1] = 0.f;
       }
     }
   } else {
@@ -573,16 +856,16 @@ static int pick_block_n(int n_out, bool mn_major) {
   return bn;
 }
 
-template <int BN, int BMN>
+template <int BN, int BMN, bool WIDE = false, bool SWAP = false>
 static int launch_igemm_kernel(int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& mapA0,
                                const CUtensorMap& mapA1, const CUtensorMap& mapB, const IgemmParams& p) {
   static bool attr_set = false;
   if (!attr_set) {
-    OG_CHECK_CUDA(cudaFuncSetAttribute(og_conv_igemm_kernel<BN, BMN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       227 * 1024));
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_conv_igemm_kernel<BN, BMN, WIDE, SWAP>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  og_conv_igemm_kernel<BN, BMN><<<grid, kThreads, smem_bytes, stream>>>(mapA0, mapA1, mapB, p);
+  og_conv_igemm_kernel<BN, BMN, WIDE, SWAP><<<grid, kThreads, smem_bytes, stream>>>(mapA0, mapA1, mapB, p);
   OG_CHECK_CUDA(cudaGetLastError());
   return OG_OK;
 }
@@ -632,8 +915,16 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   const int N = L.N, T = L.T, H = L.H, W = L.W, n_out = L.n_out;
   OG_REQUIRE(N > 0 && T > 0 && H > 0 && W > 0 && n_out > 0, "conv3d: empty problem");
   const bool plain = (L.OT == 0) && L.astride[0] == 1 && L.astride[1] == 1 && L.astride[2] == 1;
+  // 128 output channels over many voxels: 256-voxel x 128-channel tiles with the operands swapped (see the kernel), when
+  // there are at least four such tiles per SM (then the launch would not be split either). scripts/bench_conv_gemm.py,
+  // ms per launch, ping-pong -> swapped, H100 SXM at 700 W: fwd 256->128 @16x64x64 1.464 -> 1.394, 128->128 + sc256
+  // 0.797 -> 0.751, 128->128 0.720 -> 0.717; data gradient 128<-3 (the tail) 0.941 -> 0.566, 128<-128 0.722 -> 0.718.
+  // With a residual it measured slower (fwd 128->128 0.726 -> 0.783: the residual tile is read in the unoverlapped
+  // epilogue), so residual launches keep the ping-pong kernel.
+  const bool swap = plain && !L.out_f32 && !L.residual && n_out == 128 &&
+                    (long long)N * T * H * W >= 4LL * kSwapVox * num_sms();
   int bw, bh, bt, bn;
-  choose_voxel_box(kBlockM, N, T, H, W, &bw, &bh, &bt, &bn);
+  choose_voxel_box(swap ? kSwapVox : kBlockM, N, T, H, W, &bw, &bh, &bt, &bn);
   IgemmParams p;
   memset(&p, 0, sizeof(p));
   p.nseg = L.nseg;
@@ -674,7 +965,6 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   p.bias0 = L.bias0;
   p.bias1 = L.bias1;
   p.residual = reinterpret_cast<const __nv_bfloat16*>(L.residual);
-  const int stage_bytes = kABytes + p.block_n * kBlockK * 2;
   p.fast_store = (!L.out_f32 && n_out % 64 == 0 && p.block_n % 64 == 0) ? 1 : 0;
   // split-K when the tiles cannot fill the machine and each has a long K loop: every split stores into its own fp32 slab
   // of the workspace, so the split shrinks to the slabs that fit and the launch runs unsplit below two
@@ -694,10 +984,29 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
       }
     }
   }
-  int stages = (227 * 1024 - 1024 /*align slack*/ - kTailBytes) / stage_bytes;
+  // 128 x 256 tiles (both consumers on each item) for unsplit, plain launches with staged bf16 stores and >= 256 output
+  // channels; everything else keeps the ping-pong kernel with BN <= 128. scripts/bench_conv_gemm.py, ms per launch,
+  // ping-pong -> wide, H100 SXM at a 400 W power limit (two alternated runs agreed within a few percent):
+  //   forward  256->1024 @16x32x32 4.02 -> 3.22, 256->2048 @8x16x16 0.99 -> 0.78, 512->4096 @4x8x8 0.58 -> 0.41,
+  //            512->256 @8x16x16 0.213 -> 0.176, 256->256 @16x32x32 0.794 -> 0.757, +sc128 0.826 -> 0.781,
+  //            128->256 @16x32x32 0.414 -> 0.398, 256->256 @8x16x16 0.108 -> 0.106
+  //   data gradient (MN-major weights) 256<-1024 @16x32x32 3.56 -> 3.04, 256<-128 @16x64x64 1.77 -> 1.64,
+  //            256<-256 @16x32x32 0.777 -> 0.743, 256<-256 @8x16x16 0.114 -> 0.102; but slower with 512 outputs
+  //            (512<-256 @8x16x16 0.204 -> 0.224) and with 2048-channel dy boxes (256<-2048 @8x16x16 0.763 -> 0.886),
+  //            so the data gradient takes the wide tile only for 256 outputs over at most 1024 channels.
+  const bool wide = plain && p.splits == 1 && p.fast_store && n_out >= kWideN &&
+                    (!L.b_mn_major || (n_out == kWideN && L.c0 <= 1024));
+  if (wide) {
+    p.block_n = kWideN;
+    p.num_n_tiles = (n_out + kWideN - 1) / kWideN;
+  }
+  OG_REQUIRE(!swap || (p.splits == 1 && p.fast_store && p.num_n_tiles == 1), "conv3d: bad swapped-tile launch");
+  const int stage_bytes = (swap ? kSwapVox * kBlockK * 2 : kABytes) + p.block_n * kBlockK * 2;
+  const int tail_bytes = swap ? kSwapTailBytes : wide ? kWideTailBytes : kTailBytes;
+  int stages = (227 * 1024 - 1024 /*align slack*/ - tail_bytes) / stage_bytes;
   if (stages > kMaxStages) stages = kMaxStages;
   p.num_stages = stages;
-  const size_t smem_bytes = (size_t)stages * stage_bytes + 1024 + kTailBytes;
+  const size_t smem_bytes = (size_t)stages * stage_bytes + 1024 + tail_bytes;
 
   CUtensorMap mapA0, mapA1, mapB;
   {
@@ -749,7 +1058,13 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   int grid = num_sms();
   if (grid > total_tiles) grid = total_tiles;
   int rc;
-  switch (p.block_n * 2 + p.b_mn_major) {
+  if (swap) {
+    rc = p.b_mn_major ? launch_igemm_kernel<kSwapVox, 1, true, true>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p)
+                      : launch_igemm_kernel<kSwapVox, 0, true, true>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p);
+  } else if (wide) {
+    rc = p.b_mn_major ? launch_igemm_kernel<kWideN, 1, true>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p)
+                      : launch_igemm_kernel<kWideN, 0, true>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p);
+  } else switch (p.block_n * 2 + p.b_mn_major) {
     case 16 * 2: rc = launch_igemm_kernel<16, 0>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p); break;
     case 32 * 2: rc = launch_igemm_kernel<32, 0>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p); break;
     case 64 * 2: rc = launch_igemm_kernel<64, 0>(grid, smem_bytes, stream, mapA0, mapA1, mapB, p); break;

@@ -222,4 +222,13 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// Four 8x8 b16 matrices from registers to shared memory, transposed: lane 8m + i gives the address of row i of matrix m
+// in memory, and register m of thread t holds elements (t/4, 2(t%4) + {0,1}) of the transpose of matrix m — the
+// accumulator fragment layout of mma / wgmma, so an [M][N] fragment lands as [N][M] rows of 16 bytes.
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
+
 }  // namespace og

@@ -44,6 +44,15 @@ SHAPES = [
     ('dgrad 256<-256 k3 @8x16x16', 'dgrad', dict(cin=256, cout=256, k=3, grid=(8, 16, 16))),
     ('dgrad 512<-512 k3 @4x8x8 split-K', 'dgrad', dict(cin=512, cout=512, k=3, grid=(4, 8, 8))),
     ('strided dgrad 128<-128 k3 s(1,2,2) @16x64x64', 'sdgrad', dict(cin=128, cout=128, k=3, s=(1, 2, 2), grid=(16, 64, 64))),
+    # the remaining classes with 256 or more output channels: decoder up-convolutions and channel changes
+    ('fwd 128->256 k3 @16x32x32 bias+gn', 'fwd', dict(cin=128, cout=256, k=3, grid=(16, 32, 32), bias=1, gn=True)),
+    ('fwd 256->256 k3 +sc128 @16x32x32 bias2+gn', 'fwd',
+     dict(cin=256, cout=256, k=3, grid=(16, 32, 32), sc=128, bias=2, gn=True)),
+    ('fwd 512->256 k3 @8x16x16 bias+gn', 'fwd', dict(cin=512, cout=256, k=3, grid=(8, 16, 16), bias=1, gn=True)),
+    ('fwd 256->2048 k3 @8x16x16 bias', 'fwd', dict(cin=256, cout=2048, k=3, grid=(8, 16, 16), bias=1)),
+    ('fwd 512->4096 k3 @4x8x8 bias', 'fwd', dict(cin=512, cout=4096, k=3, grid=(4, 8, 8), bias=1)),
+    ('dgrad 256<-2048 k3 @8x16x16', 'dgrad', dict(cin=256, cout=2048, k=3, grid=(8, 16, 16))),
+    ('dgrad 512<-256 k3 @8x16x16', 'dgrad', dict(cin=512, cout=256, k=3, grid=(8, 16, 16))),
 ]
 
 
