@@ -312,7 +312,8 @@ int og_flash_attn_bwd(const void* q, const void* k, const void* v, const void* o
                       const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq, int S, int C,
                       int n_head, float scale, og_stream_t stream);
 
-/* Temporal attention, is_causal=True (attention.py:347-371, 423): one sequence per (batch, pixel), T <= 32.
+/* Temporal attention, is_causal=True (attention.py:347-371, 423): one sequence per (batch, pixel), T <= 32
+ * (longer clips: og_temporal_attn_long_fwd / bwd below).
  * q/out rows ((b*T + t)*P + p); k,v either the same layout (kv_bcast=0) or [B][T][C] shared by all pixels
  * (kv_bcast=1: latent-action conditioning through to_k/to_v, attention.py:127-129,362-363). */
 int og_temporal_attn_fwd(const void* q, const void* k, const void* v, const void* residual, void* out, int B, int T,
@@ -321,6 +322,23 @@ int og_temporal_attn_fwd(const void* q, const void* k, const void* v, const void
 int og_temporal_attn_bwd(const void* q, const void* k, const void* v, const void* dout, void* dq, void* dk, void* dv,
                          float* dk_bcast, float* dv_bcast, int B, int T, int64_t P, int C, int n_head, float scale,
                          int kv_bcast, og_stream_t stream);
+
+/* Temporal attention for clips of any length (T >= 1; the modules call it for T > 32), d_head = 64 only: the same
+ * causal attention and layouts as og_temporal_attn_fwd / bwd, FlashAttention-2 style on mma.sync tensor cores (64-row
+ * query and key tiles, online softmax), with the forward / backward contract of og_flash_attn_fwd / bwd.
+ * out: bf16 like q (always written: the backward pass needs it). residual / out_res (optional, both or neither):
+ * out_res = out + residual, added in fp32 before the rounding.
+ * lse: fp32 log-sum-exp of the scaled scores, B*T*P*n_head values laid out [B][n_head][P][T]
+ * (index ((b*n_head + h)*P + p)*T + t); delta_ws: fp32 scratch of the same size and layout. */
+int og_temporal_attn_long_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
+                              void* out_res, float* lse, int B, int T, int64_t P, int C, int n_head, float scale,
+                              int kv_bcast, og_stream_t stream);
+/* kv_bcast=0: dk, dv bf16 like k, v. kv_bcast=1: dk_bcast, dv_bcast fp32 [B][T][C], ACCUMULATED (+=): each CTA adds the
+ * sum over its chunk of pixels with fp32 atomics, so the order of the additions (and the last bits) is not fixed. */
+int og_temporal_attn_long_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout,
+                              const float* lse, float* delta_ws, void* dq, void* dk, void* dv, float* dk_bcast,
+                              float* dv_bcast, int B, int T, int64_t P, int C, int n_head, float scale, int kv_bcast,
+                              og_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * DynamicsModel rows (genie/dynamics.py)

@@ -955,6 +955,10 @@ class _SpaceAttnFn(torch.autograd.Function):
         return dx, None, dgamma, dbeta, None, None, None
 
 
+# Longest clip of the per-pixel temporal kernels (og_temporal_attn_fwd / bwd); longer ones take the tiled kernels.
+_TIME_ATTN_SHORT_T = 32
+
+
 class _TimeAttnFn(torch.autograd.Function):
     """y = SDPA_causal(q, k, v; scale) + x over t for every pixel; q = LayerNorm(RoPE1d(x)); k = v = q, or the
     projected latent-action conditioning (B, T, C) shared by all pixels (attention.py:347-371, 471)."""
@@ -976,15 +980,23 @@ class _TimeAttnFn(torch.autograd.Function):
             vc = v_cond.detach().to(bf16).contiguous()
         else:
             kc = vc = q
-        _lib.call('og_temporal_attn_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), x.data_ptr(), y.data_ptr(), B, T,
-                  P, C, n_head, scale, int(bcast), s)
+        o = lse = None
+        if T <= _TIME_ATTN_SHORT_T:
+            _lib.call('og_temporal_attn_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), x.data_ptr(), y.data_ptr(),
+                      B, T, P, C, n_head, scale, int(bcast), s)
+        else:
+            # longer clips: the tiled kernels, which keep the attention output and log-sum-exp for the backward pass
+            o = torch.empty_like(x)
+            lse = torch.empty((B, n_head, P, T), dtype=f32, device=x.device)
+            _lib.call('og_temporal_attn_long_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), o.data_ptr(),
+                      x.data_ptr(), y.data_ptr(), lse.data_ptr(), B, T, P, C, n_head, scale, int(bcast), s)
         ctx.cfg = (n_head, scale, eps, bcast)
-        ctx.save_for_backward(x, q, kc if bcast else None, vc if bcast else None, freq, gamma)
+        ctx.save_for_backward(x, q, kc if bcast else None, vc if bcast else None, freq, gamma, o, lse)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, q, kc, vc, freq, gamma = ctx.saved_tensors
+        x, q, kc, vc, freq, gamma, o, lse = ctx.saved_tensors
         n_head, scale, eps, bcast = ctx.cfg
         B, T, H, W, C = x.shape
         P = H * W
@@ -992,16 +1004,27 @@ class _TimeAttnFn(torch.autograd.Function):
         dy = _rows_bf16(dy)
         dq = torch.empty_like(x)
         dkc = dvc = None
+        delta = None if lse is None else torch.empty_like(lse)
         if bcast:
             dkc = _zeros((B, T, C), f32, x.device)
             dvc = _zeros((B, T, C), f32, x.device)
-            _lib.call('og_temporal_attn_bwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), dy.data_ptr(), dq.data_ptr(),
-                      None, None, dkc.data_ptr(), dvc.data_ptr(), B, T, P, C, n_head, scale, 1, s)
+            if lse is None:
+                _lib.call('og_temporal_attn_bwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), dy.data_ptr(),
+                          dq.data_ptr(), None, None, dkc.data_ptr(), dvc.data_ptr(), B, T, P, C, n_head, scale, 1, s)
+            else:
+                _lib.call('og_temporal_attn_long_bwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), o.data_ptr(),
+                          dy.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), None, None,
+                          dkc.data_ptr(), dvc.data_ptr(), B, T, P, C, n_head, scale, 1, s)
             g1 = g2 = None
         else:
             dk, dv = torch.empty_like(x), torch.empty_like(x)
-            _lib.call('og_temporal_attn_bwd', q.data_ptr(), q.data_ptr(), q.data_ptr(), dy.data_ptr(), dq.data_ptr(),
-                      dk.data_ptr(), dv.data_ptr(), None, None, B, T, P, C, n_head, scale, 0, s)
+            if lse is None:
+                _lib.call('og_temporal_attn_bwd', q.data_ptr(), q.data_ptr(), q.data_ptr(), dy.data_ptr(),
+                          dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), None, None, B, T, P, C, n_head, scale, 0, s)
+            else:
+                _lib.call('og_temporal_attn_long_bwd', q.data_ptr(), q.data_ptr(), q.data_ptr(), o.data_ptr(),
+                          dy.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(),
+                          dk.data_ptr(), dv.data_ptr(), None, None, B, T, P, C, n_head, scale, 0, s)
             g1, g2 = dk, dv
         dx = torch.empty_like(x)
         dgamma = _zeros(C, f32, x.device)
