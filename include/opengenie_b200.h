@@ -366,13 +366,15 @@ int og_masked_ce_bwd(const void* logits, const int64_t* target, const uint8_t* m
  * og_maskgit_sample runs EVERY iteration of lines 136-163 in one launch (one CTA per batch row): inverse-CDF draw with
  * the supplied uniforms (torch.multinomial's role, line 145) -> confidence = prob[pred] (146) -> -inf on already
  * predicted positions (151) -> top-k of `schedule[s]` (152) -> scatter into code / mask (159-160).
- * logits: [rows = B*P][V] bf16 or fp32; cdf: fp32 [rows][V]; uniforms: fp32 [steps][B][P] in [0,1);
- * schedule: int32 [steps] (device); code: int64 [B][P] in/out (initialised to masked_tok); mask: uint8 [B][P] in/out
- * (1 = still to predict). P <= 4096. */
+ * logits: [rows = B*P][V] bf16 or fp32; cdf: fp32 [rows][V], non-decreasing along each row; row_stats: fp32 [rows][2]
+ * = (max, 1 / sum) of the scaled row, from which og_maskgit_sample recomputes prob[pred] (NULL in og_softmax_cdf:
+ * not written); uniforms: fp32 [steps][B][P] in [0,1); schedule: int32 [steps] (device); code: int64 [B][P] in/out
+ * (initialised to masked_tok); mask: uint8 [B][P] in/out (1 = still to predict). P <= 4096. */
 int og_softmax_cdf(const void* logits, int logits_f32, int64_t rows, int V, float inv_temp, float* cdf,
-                   og_stream_t stream);
-int og_maskgit_sample(const float* cdf, const float* uniforms, const int* schedule, int steps, int B, int P, int V,
-                      int64_t* code, uint8_t* mask, og_stream_t stream);
+                   float* row_stats, og_stream_t stream);
+int og_maskgit_sample(const float* cdf, const void* logits, int logits_f32, float inv_temp, const float* row_stats,
+                      const float* uniforms, const int* schedule, int steps, int B, int P, int V, int64_t* code,
+                      uint8_t* mask, og_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * fused multi-tensor AdamW (genie/tokenizer.py:437-442) + bf16 operand refresh

@@ -132,17 +132,22 @@ __global__ void og_masked_ce_bwd_kernel(const __nv_bfloat16* __restrict__ logits
 // confidence -> mask already-predicted positions to -inf -> top-k -> scatter into code / mask).
 // ------------------------------------------------------------------------------------------------
 
-// cdf[row][j] = sum_{i<=j} softmax(logits[row] * inv_temp)[i], fp32; one warp per row.
+// logits[row][j] * inv_temp in fp32, for bf16 or fp32 logits
+__device__ __forceinline__ float scaled_logit(const void* __restrict__ logits, int logits_f32, long long i,
+                                              float inv_temp) {
+  return (logits_f32 ? reinterpret_cast<const float*>(logits)[i]
+                     : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(logits)[i])) * inv_temp;
+}
+
+// cdf[row][j] = sum_{i<=j} softmax(logits[row] * inv_temp)[i], fp32; one warp per row. row_stats[row] = (max, 1/sum):
+// prob[j] = expf(logit[j] * inv_temp - max) * (1/sum) is the exact fp32 value the CDF is summed from.
 __global__ void og_softmax_cdf_kernel(const void* __restrict__ logits, int logits_f32, long long rows, int V, float inv_temp,
-                                      float* __restrict__ cdf) {
+                                      float* __restrict__ cdf, float2* __restrict__ row_stats) {
   const int lane = threadIdx.x & 31;
   const long long w0 = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
   for (long long row = w0; row < rows; row += nw) {
-    auto at = [&](int j) -> float {
-      return (logits_f32 ? reinterpret_cast<const float*>(logits)[row * V + j]
-                         : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(logits)[row * V + j])) * inv_temp;
-    };
+    auto at = [&](int j) -> float { return scaled_logit(logits, logits_f32, row * V + j, inv_temp); };
     float m = -INFINITY;
     for (int j = lane; j < V; j += 32) m = fmaxf(m, at(j));
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -150,6 +155,7 @@ __global__ void og_softmax_cdf_kernel(const void* __restrict__ logits, int logit
     for (int j = lane; j < V; j += 32) s += expf(at(j) - m);
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     const float inv = 1.f / s;
+    if (row_stats && lane == 0) row_stats[row] = make_float2(m, inv);
     float carry = 0.f;
     for (int j0 = 0; j0 < V; j0 += 32) {
       const int j = j0 + lane;
@@ -159,6 +165,15 @@ __global__ void og_softmax_cdf_kernel(const void* __restrict__ logits, int logit
         if (lane >= o) p += t;
       }
       p += carry;
+      // Each lane sums its prefix in a different order, so two adjacent sums can come out in the wrong order (at
+      // logits of standard deviation 4, most rows of 1024 have such a step). A running maximum makes every row
+      // non-decreasing, which the inverse-CDF search needs; since the exact prefix sums are non-decreasing, no entry
+      // moves further from its exact value than the largest error of the sums before it. carry is at most every p of
+      // the next chunk.
+      for (int o = 1; o < 32; o <<= 1) {
+        const float t = __shfl_up_sync(0xffffffffu, p, o);
+        if (lane >= o) p = fmaxf(p, t);
+      }
       if (j < V) cdf[row * V + j] = p;
       carry = __shfl_sync(0xffffffffu, p, 31);
     }
@@ -167,8 +182,10 @@ __global__ void og_softmax_cdf_kernel(const void* __restrict__ logits, int logit
 
 // One CTA (1024 threads) per batch row; P = h*w positions (P <= 4096).
 __global__ void __launch_bounds__(1024)
-    og_maskgit_sample_kernel(const float* __restrict__ cdf, const float* __restrict__ uniforms, const int* __restrict__ schedule,
-                             int steps, int B, int P, int V, long long* __restrict__ code, unsigned char* __restrict__ mask) {
+    og_maskgit_sample_kernel(const float* __restrict__ cdf, const void* __restrict__ logits, int logits_f32,
+                             float inv_temp, const float2* __restrict__ row_stats, const float* __restrict__ uniforms,
+                             const int* __restrict__ schedule, int steps, int B, int P, int V, long long* __restrict__ code,
+                             unsigned char* __restrict__ mask) {
   extern __shared__ unsigned char smem_mg[];
   int Pp = 1;
   while (Pp < P) Pp <<= 1;
@@ -190,7 +207,8 @@ __global__ void __launch_bounds__(1024)
     for (int p = threadIdx.x; p < Pp; p += blockDim.x) {
       float c = -INFINITY;
       if (p < P) {
-        const float* row = cdf + ((long long)b * P + p) * V;
+        const long long r = (long long)b * P + p;
+        const float* row = cdf + r * V;
         const float u = uniforms[((long long)s * B + b) * P + p] * row[V - 1];
         int lo = 0, hi = V - 1;                             // first j with cdf[j] > u
         while (lo < hi) {
@@ -198,7 +216,10 @@ __global__ void __launch_bounds__(1024)
           if (row[mid] > u) hi = mid; else lo = mid + 1;
         }
         pred[p] = lo;
-        const float pr = row[lo] - (lo > 0 ? row[lo - 1] : 0.f);
+        // confidence = prob[pred] (line 146), recomputed from the row's (max, 1/sum). The difference of two CDF
+        // entries would carry an absolute error of about one ulp of the running sum, which reorders unlikely draws.
+        const float2 st = row_stats[r];
+        const float pr = expf(scaled_logit(logits, logits_f32, r * V + lo, inv_temp) - st.x) * st.y;
         c = mask[(long long)b * P + p] ? pr : -INFINITY;    // conf[~mask] = -inf (line 151)
       }
       key[p] = c;
@@ -302,17 +323,20 @@ extern "C" int og_masked_ce_bwd(const void* logits, const int64_t* target, const
 }
 
 extern "C" int og_softmax_cdf(const void* logits, int logits_f32, int64_t rows, int V, float inv_temp, float* cdf,
-                              og_stream_t stream) {
+                              float* row_stats, og_stream_t stream) {
   OG_REQUIRE(logits && cdf && rows > 0 && V > 0, "softmax_cdf: bad arguments");
-  og_softmax_cdf_kernel<<<grid_for(rows, 8, 8), 256, 0, (cudaStream_t)stream>>>(logits, logits_f32, rows, V, inv_temp, cdf);
+  og_softmax_cdf_kernel<<<grid_for(rows, 8, 8), 256, 0, (cudaStream_t)stream>>>(logits, logits_f32, rows, V, inv_temp, cdf,
+                                                                               reinterpret_cast<float2*>(row_stats));
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   return OG_OK;
 }
 
-extern "C" int og_maskgit_sample(const float* cdf, const float* uniforms, const int* schedule, int steps, int B, int P, int V,
-                                 int64_t* code, uint8_t* mask, og_stream_t stream) {
-  OG_REQUIRE(cdf && uniforms && schedule && code && mask && steps > 0 && B > 0 && V > 0, "maskgit_sample: bad arguments");
+extern "C" int og_maskgit_sample(const float* cdf, const void* logits, int logits_f32, float inv_temp,
+                                 const float* row_stats, const float* uniforms, const int* schedule, int steps, int B,
+                                 int P, int V, int64_t* code, uint8_t* mask, og_stream_t stream) {
+  OG_REQUIRE(cdf && logits && row_stats && uniforms && schedule && code && mask && steps > 0 && B > 0 && V > 0,
+             "maskgit_sample: bad arguments");
   OG_REQUIRE(P > 0 && P <= 4096, "maskgit_sample: P=%d positions per frame must be in [1, 4096]", P);
   int Pp = 1;
   while (Pp < P) Pp <<= 1;
@@ -322,8 +346,9 @@ extern "C" int og_maskgit_sample(const float* cdf, const float* uniforms, const 
     OG_CHECK_CUDA(cudaFuncSetAttribute(og_maskgit_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     attr_set = true;
   }
-  og_maskgit_sample_kernel<<<B, 1024, smem, (cudaStream_t)stream>>>(cdf, uniforms, schedule, steps, B, P, V,
-                                                                   (long long*)code, mask);
+  og_maskgit_sample_kernel<<<B, 1024, smem, (cudaStream_t)stream>>>(
+      cdf, logits, logits_f32, inv_temp, reinterpret_cast<const float2*>(row_stats), uniforms, schedule, steps, B, P, V,
+      (long long*)code, mask);
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   return OG_OK;

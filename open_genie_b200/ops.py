@@ -1205,14 +1205,16 @@ def maskgit_sample(logits_last: Tensor, uniforms: Tensor, schedule: Tensor, temp
     dev = lg.device
     s = _stream()
     cdf = torch.empty((b * P, V), dtype=f32, device=dev)
-    _lib.call('og_softmax_cdf', lg.data_ptr(), int(lg.dtype == f32), b * P, V, 1.0 / float(temp), cdf.data_ptr(), s)
+    row_stats = torch.empty((b * P, 2), dtype=f32, device=dev)
+    lg_f32, inv_temp = int(lg.dtype == f32), 1.0 / float(temp)
+    _lib.call('og_softmax_cdf', lg.data_ptr(), lg_f32, b * P, V, inv_temp, cdf.data_ptr(), row_stats.data_ptr(), s)
     steps = int(schedule.numel())
     u = uniforms.detach().to(device=dev, dtype=f32).reshape(steps, b * P).contiguous()
     sch = schedule.detach().to(device=dev, dtype=torch.int32).contiguous()
     code = torch.full((b, P), int(masked_tok), dtype=torch.int64, device=dev)
     mask = torch.ones((b, P), dtype=torch.uint8, device=dev)
-    _lib.call('og_maskgit_sample', cdf.data_ptr(), u.data_ptr(), sch.data_ptr(), steps, b, P, V, code.data_ptr(),
-              mask.data_ptr(), s)
+    _lib.call('og_maskgit_sample', cdf.data_ptr(), lg.data_ptr(), lg_f32, inv_temp, row_stats.data_ptr(), u.data_ptr(),
+              sch.data_ptr(), steps, b, P, V, code.data_ptr(), mask.data_ptr(), s)
     return code.view(b, h, w), mask.view(b, h, w)
 
 

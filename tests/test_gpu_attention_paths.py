@@ -758,8 +758,13 @@ def test_space_attention_res_composed():
 # which kernel ran: one profiled call per dispatch class
 # ------------------------------------------------------------------------------------------------------------------
 def _kernels_run(fn):
+    """Names of the kernels two calls of `fn` launch. Late in a long test process the trace of a session sometimes
+    lacked the kernels of its first call (the library's launch counter showed that they had run); those of a second,
+    identical call were listed."""
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
         fn()
         torch.cuda.synchronize()
     return [e.name for e in prof.events()]
