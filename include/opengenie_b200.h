@@ -208,14 +208,16 @@ int og_ndhwc_to_ncdhw_f32(const void* x, int x_f32, float* y, int N, int C, int6
 
 /* Depth-to-space-time: Rearrange('b (c p q r) t h w -> b c (t p) (h q) (w r)') of
  * DepthToSpaceTimeUpsample (genie/module/video.py:403-408). x: bf16 [N,T,H,W,c*p*q*r] un-shuffled,
- * y: bf16 [N,T*p,H*q,W*r,c] shuffled. inverse=0 reads x writes y; inverse=1 reads y writes x (backward). */
+ * y: bf16 [N,T*p,H*q,W*r,c] shuffled. inverse=0 reads x writes y; inverse=1 reads y writes x (backward).
+ * Any c and alignment; the 16-byte vector kernels run when c % 8 == 0 and the pointers allow. */
 int og_pixel_shuffle3d(const void* x, void* y, int inverse, int N, int T, int H, int W, int c, int p, int q, int r,
                        og_stream_t stream);
 
 /* BlurPooling3d with num_groups == 1 (genie/module/video.py:487-537): every output channel is
  * blur_k(sum_c x[:, c]) with the normalised Pascal kernel, stride (st,sh,sw), padding (k-1)/2.
  * backward == 0: x [N,T,H,W,cin] -> y [N,To,Ho,Wo,cout], scratch >= N*T*H*W floats.
- * backward != 0: x = dy [N,To,Ho,Wo,cout] -> y = dx [N,T,H,W,cin], scratch >= N*To*Ho*Wo floats. */
+ * backward != 0: x = dy [N,To,Ho,Wo,cout] -> y = dx [N,T,H,W,cin], scratch >= N*To*Ho*Wo floats.
+ * cin, cout % 8 == 0; y 16-byte aligned; every padded extent (e.g. H + 2*pad) at least k. */
 int og_blurpool3d(const void* x, void* y, float* scratch, int backward, int N, int T, int H, int W, int cin, int cout,
                   int k, int st, int sh, int sw, og_stream_t stream);
 
@@ -235,16 +237,17 @@ int og_mse_bwd(const float* rec_ndhwc, const float* tgt_ncdhw, const float* gsca
 /* Perceptual-loss pieces that are not convolutions (genie/module/loss.py:34-107, torchvision vgg16.features):
  * nn.MaxPool2d(2, 2) on NHWC bf16 (C % 8 == 0), and out[0] += sum (a - b)^2 over n bf16 elements (n % 8 == 0) — the
  * feature-space mse_loss numerator (loss.py:100-103). The VGG convolutions / ReLUs run on og_conv3d_fwd (kt = 1) and
- * og_affine_act_fwd (act = 3). */
+ * og_affine_act_fwd (act = 3). The max-pool propagates NaN as nn.MaxPool2d does. x, y, a and b must be 16-byte
+ * aligned. */
 int og_maxpool2x2(const void* x, void* y, int N, int H, int W, int C, og_stream_t stream);
 int og_sqdiff_sum(const void* a, const void* b, int64_t n, float* out, og_stream_t stream);
 
-/* out[c] += sum_rows x[row][c] (conv bias gradient). x: bf16 [rows][ld]. */
+/* out[c] += sum_rows x[row][c] (conv bias gradient). x: bf16 [rows][ld], rows >= 1. */
 int og_colsum(const void* x, int64_t rows, int C, int ld, float* out, og_stream_t stream);
 /* y[row][0:cd] = x[row][0:cs] zero-padded / truncated; x fp32 or bf16, y bf16. */
 int og_pad_channels(const void* x, int x_f32, void* y, int64_t rows, int cs, int cd, og_stream_t stream);
 
-/* out = a - b on n bf16 elements (n % 8 == 0). */
+/* out = a - b on n bf16 elements (n % 8 == 0); a, b and out 16-byte aligned. */
 int og_sub_rows(const void* a, const void* b, void* out, int64_t n, og_stream_t stream);
 
 /* dst[row*dst_ld + c] = bf16(src[row*src_ld + c]) for c < cols: refreshes the bf16 operand copy of a
@@ -384,7 +387,9 @@ typedef struct og_adamw_tensor {
   const float* g;  /* fp32 gradient or NULL (then only the bf16 copy is refreshed) */
   float* m;        /* exp_avg */
   float* v;        /* exp_avg_sq */
-  void* p_bf16;    /* optional bf16 destination: element i -> [(i / row_len) * dst_ld + i % row_len] */
+  void* p_bf16;    /* optional bf16 destination: element i -> [(i / row_len) * dst_ld + i % row_len]. Any
+                    * alignment and pitch works; row_len % 4 == 0, dst_ld % 4 == 0 and an 8-byte aligned p_bf16
+                    * let full, 16-byte aligned chunks take the vector path */
   int64_t n;
   int64_t row_len;
   int64_t dst_ld;

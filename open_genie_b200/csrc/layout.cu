@@ -11,6 +11,8 @@
 namespace og {
 extern std::atomic<uint64_t> g_launches;
 
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 static int ew_blocks(long long total, int block) {
   long long g = (total + block - 1) / block;
   long long cap = (long long)num_sms() * 32;
@@ -234,7 +236,7 @@ __global__ void og_mse_bwd_kernel(const float* __restrict__ rec, const float* __
 // column sums (bias gradient): out[c] += sum_rows x[row][c]; x bf16 [rows][ld], first C columns
 __global__ void og_colsum_kernel(const __nv_bfloat16* __restrict__ x, long long rows, int C, int ld,
                                  float* __restrict__ out) {
-  // block handles 64 rows x all columns; thread t -> column t (loop), coalesced along c
+  // block handles 256 rows x all columns; thread t -> column t (loop), coalesced along c
   const long long r0 = (long long)blockIdx.x * 256;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float acc = 0.f;
@@ -365,6 +367,7 @@ using namespace og;
 
 extern "C" int og_sub_rows(const void* a, const void* b, void* out, int64_t n, og_stream_t stream) {
   OG_REQUIRE(a && b && out && n > 0 && n % 8 == 0, "sub_rows: bad arguments (n must be a multiple of 8)");
+  OG_REQUIRE(aligned16(a) && aligned16(b) && aligned16(out), "sub_rows: a, b and out must be 16-byte aligned");
   og_sub_rows_kernel<<<ew_blocks(n / 8, 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)a, (const uint4*)b,
                                                                              (uint4*)out, n / 8);
   OG_CHECK_CUDA(cudaGetLastError());
@@ -417,7 +420,9 @@ extern "C" int og_pixel_shuffle3d(const void* x, void* y, int inverse, int N, in
                                   int q, int r, og_stream_t stream) {
   OG_REQUIRE(x && y, "pixel_shuffle3d: null pointer");
   OG_REQUIRE(c >= 1 && p >= 1 && q >= 1 && r >= 1, "pixel_shuffle3d: bad shape (c=%d p=%d q=%d r=%d)", c, p, q, r);
-  if (c % 8 != 0) {
+  OG_REQUIRE(N >= 1 && T >= 1 && H >= 1 && W >= 1, "pixel_shuffle3d: bad extents (N=%d T=%d H=%d W=%d)", N, T, H, W);
+  // og_pixel_shuffle_kernel moves 8 channels of y as one 16-byte vector: a y off that alignment goes scalar
+  if (c % 8 != 0 || !aligned16(y)) {
     const long long tot = (long long)N * T * p * H * q * W * r * c;
     og_pixel_shuffle_scalar_kernel<<<ew_blocks(tot, 256), 256, 0, (cudaStream_t)stream>>>(
         (const __nv_bfloat16*)x, (__nv_bfloat16*)y, T, H, W, c, p, q, r, tot, inverse);
@@ -429,7 +434,7 @@ extern "C" int og_pixel_shuffle3d(const void* x, void* y, int inverse, int N, in
   // forward: x un-shuffled (read), y shuffled (written). inverse: y shuffled (read), x un-shuffled (written).
   const int pqr = p * q * r;
   const long long tv = (long long)N * T * H * W * (c / 8);
-  const bool aligned = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
+  const bool aligned = aligned16(x);   // y is 16-byte aligned here
   if (aligned && pqr == 8)
     og_pixel_shuffle_vec_kernel<8><<<ew_blocks(tv, 256), 256, 0, (cudaStream_t)stream>>>(
         (const uint4*)x, (uint4*)y, T, H, W, c, p, q, r, tv, inverse);
@@ -471,7 +476,8 @@ extern "C" int og_mse_bwd(const float* rec_ndhwc, const float* tgt_ncdhw, const 
 }
 
 extern "C" int og_colsum(const void* x, int64_t rows, int C, int ld, float* out, og_stream_t stream) {
-  OG_REQUIRE(x && out && C > 0 && ld >= C, "colsum: bad arguments");
+  OG_REQUIRE(x && out && rows > 0 && C > 0 && ld >= C, "colsum: bad arguments (rows=%lld C=%d ld=%d)", (long long)rows,
+             C, ld);
   if (ld % 8 == 0 && (ld <= 2048 || ld % 2048 == 0) && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
     const int col_blocks = (ld + 2047) / 2048;
     long long want = (4LL * num_sms() + col_blocks - 1) / col_blocks;
@@ -609,6 +615,12 @@ static int blurpool_launch(const void* x, void* y, float* scratch, int backward,
   OG_REQUIRE(x && y && scratch, "blurpool: null pointer");
   OG_REQUIRE(cin % 8 == 0 && cout % 8 == 0 && k >= 1 && k <= 7 && kt >= 1 && kt <= 7, "blurpool: need C %% 8 == 0 and k <= 7");
   OG_REQUIRE(pad_t >= 0 && pad >= 0 && st >= 1 && sh >= 1 && sw >= 1, "blurpool: bad stride / padding");
+  OG_REQUIRE(N >= 1 && T >= 1 && H >= 1 && W >= 1, "blurpool: bad extents (N=%d T=%d H=%d W=%d)", N, T, H, W);
+  // checked before the division below, which truncates towards zero and would turn a negative span into one output
+  OG_REQUIRE(T + 2 * pad_t >= kt && H + 2 * pad >= k && W + 2 * pad >= k,
+             "blurpool: padded input smaller than the kernel (T=%d H=%d W=%d k=%d)", T, H, W, k);
+  // the stencil kernels write 8 channels of y as one 16-byte vector
+  OG_REQUIRE(aligned16(y), "blurpool: y must be 16-byte aligned");
   const int To = (T + 2 * pad_t - kt) / st + 1, Ho = (H + 2 * pad - k) / sh + 1, Wo = (W + 2 * pad - k) / sw + 1;
   OG_REQUIRE(To >= 1 && Ho >= 1 && Wo >= 1, "blurpool: empty output");
   auto row_sum = [](int kk) {
@@ -732,7 +744,8 @@ __global__ void og_maxpool2x2_kernel(const uint4* __restrict__ x, uint4* __restr
     for (int e = 0; e < 4; ++e) {
       __nv_bfloat162 m = reinterpret_cast<const __nv_bfloat162*>(&q[0])[e];
 #pragma unroll
-      for (int k = 1; k < 4; ++k) m = __hmax2(m, reinterpret_cast<const __nv_bfloat162*>(&q[k])[e]);
+      // NaN-propagating, as nn.MaxPool2d: a NaN feature must reach the loss
+      for (int k = 1; k < 4; ++k) m = __hmax2_nan(m, reinterpret_cast<const __nv_bfloat162*>(&q[k])[e]);
       oh[e] = m;
     }
     y[i] = o;
@@ -764,6 +777,7 @@ extern "C" int og_maxpool2x2(const void* x, void* y, int N, int H, int W, int C,
   using namespace og;
   OG_REQUIRE(x && y && N > 0 && H >= 2 && W >= 2, "maxpool2x2: bad arguments");
   OG_REQUIRE(C % 8 == 0, "maxpool2x2: C=%d must be a multiple of 8", C);
+  OG_REQUIRE(aligned16(x) && aligned16(y), "maxpool2x2: x and y must be 16-byte aligned");
   const int Ho = H / 2, Wo = W / 2;
   const long long total = (long long)N * Ho * Wo * (C / 8);
   og_maxpool2x2_kernel<<<ew_blocks(total, 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)x, (uint4*)y, H, W, Ho, Wo, C / 8,
@@ -776,6 +790,7 @@ extern "C" int og_maxpool2x2(const void* x, void* y, int N, int H, int W, int C,
 extern "C" int og_sqdiff_sum(const void* a, const void* b, int64_t n, float* out, og_stream_t stream) {
   using namespace og;
   OG_REQUIRE(a && b && out && n > 0 && n % 8 == 0, "sqdiff_sum: bad arguments (n %% 8 == 0)");
+  OG_REQUIRE(aligned16(a) && aligned16(b), "sqdiff_sum: a and b must be 16-byte aligned");
   og_sqdiff_sum_kernel<<<ew_blocks(n / 8, 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)a, (const uint4*)b, n / 8, out);
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);

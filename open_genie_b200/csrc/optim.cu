@@ -33,7 +33,10 @@ __global__ void __launch_bounds__(256)
     const bool vec = (base + kChunk <= t.n) && ((reinterpret_cast<uintptr_t>(t.p + base) & 15) == 0) && t.g &&
                      ((reinterpret_cast<uintptr_t>(t.g + base) & 15) == 0) &&
                      ((reinterpret_cast<uintptr_t>(t.m + base) & 15) == 0) &&
-                     ((reinterpret_cast<uintptr_t>(t.v + base) & 15) == 0) && (t.row_len % 4 == 0);
+                     ((reinterpret_cast<uintptr_t>(t.v + base) & 15) == 0) && (t.row_len % 4 == 0) &&
+                     // the bf16 copy goes out as 8-byte stores: 4 elements never straddle a row, and every row
+                     // start must be 8-byte aligned
+                     (!t.p_bf16 || (((reinterpret_cast<uintptr_t>(t.p_bf16) & 7) == 0) && t.dst_ld % 4 == 0));
     if (vec) {
       // 16-byte path: 4 parameters per thread-iteration, bf16 copy written as one 8-byte store
       for (int e = threadIdx.x * 4; e < kChunk; e += 256 * 4) {

@@ -1,7 +1,38 @@
 """Shared helpers for the parity tests."""
+import math
+
 import torch
 
 from oracle import genie_oracle as O
+
+
+class Guarded:
+    """An output tensor placed `offset` elements into a buffer and followed by a guard of `guard` elements, all filled
+    with a NaN bit pattern: an element the kernel never writes fails the comparison, and a write past the end changes
+    the guard. `init` pre-fills the tensor itself (accumulated outputs start from non-zero values)."""
+    BITS = {torch.bfloat16: (torch.int16, 0x7FA5), torch.float32: (torch.int32, 0x7FC0A5A5),
+            torch.float64: (torch.int64, 0x7FF8A5A5A5A5A5A5)}
+
+    def __init__(self, shape, dtype, guard=64, init=None, offset=0, device='cuda'):
+        self.n = math.prod(shape) + offset
+        self.buf = torch.empty(self.n + guard, dtype=dtype, device=device)
+        ity, bits = self.BITS[dtype]
+        self.buf.view(ity).fill_(bits)
+        self.t = self.buf[offset:self.n].view(shape)
+        if init is not None:
+            self.t.copy_(init)
+
+    def ptr(self):
+        return self.t.data_ptr()
+
+    def untouched(self):
+        ity, bits = self.BITS[self.buf.dtype]
+        return bool((self.buf.view(ity) == bits).all())
+
+    def check_guard(self, name):
+        ity, bits = self.BITS[self.buf.dtype]
+        changed = int((self.buf[self.n:].view(ity) != bits).sum())
+        assert changed == 0, f'{name}: {changed} guard elements after the tensor were overwritten'
 
 
 def det_weights(module, gain=1.0):

@@ -8,11 +8,10 @@ Every tolerance is a per-element worst-case bound built from the rounding points
 (`attn_err`, `rope_ln_bwd_expect`). The `test_tolerance(s)_reject_*` tests run on the CPU and show that each bound
 still rejects the mistakes it exists to catch.
 """
-import math
-
 import pytest
 import torch
 
+from helpers import Guarded
 from oracle import genie_oracle as O
 
 GPU = pytest.mark.gpu
@@ -392,29 +391,6 @@ def _rand(shape, seed, amp=1.0):
 
 def _ptr(t):
     return None if t is None else t.data_ptr()
-
-
-class Guarded:
-    """An output tensor followed by a guard of `guard` elements, all filled with a NaN bit pattern: an element the
-    kernel never writes fails the comparison, and a write past the end changes the guard."""
-    BITS = {BF16: (torch.int16, 0x7FA5), F32T: (torch.int32, 0x7FC0A5A5)}
-
-    def __init__(self, shape, dtype, guard, init=None, offset=0):
-        self.n = math.prod(shape) + offset
-        self.buf = torch.empty(self.n + guard, dtype=dtype, device=DEV)
-        ity, bits = self.BITS[dtype]
-        self.buf.view(ity).fill_(bits)
-        self.t = self.buf[offset:self.n].view(shape)
-        if init is not None:
-            self.t.copy_(init)
-
-    def ptr(self):
-        return self.t.data_ptr()
-
-    def check_guard(self, name):
-        ity, bits = self.BITS[self.buf.dtype]
-        changed = int((self.buf[self.n:].view(ity) != bits).sum())
-        assert changed == 0, f'{name}: {changed} guard elements after the tensor were overwritten'
 
 
 def temporal_run(B, T, P, nh, d, bcast, seed, amp=1.0, aliased=False, do_mask=None, check_guards=True):

@@ -11,11 +11,11 @@ Every tolerance is a per-element worst-case bound built from the rounding points
 (`gn_expect`, `adagn_expect`). The `test_tolerance(s)_reject_*` tests run on the CPU and show that each bound still
 rejects the mistakes it exists to catch.
 """
-import math
-
 import pytest
 import torch
 import torch.nn.functional as F
+
+from helpers import Guarded
 
 GPU = pytest.mark.gpu
 DEV = 'cuda'
@@ -560,34 +560,6 @@ def _rand(shape, seed, amp=1.0, off=0.0, dtype=BF16):
 
 def _ptr(t):
     return None if t is None else (t.ptr() if isinstance(t, Guarded) else t.data_ptr())
-
-
-class Guarded:
-    """An output tensor followed by a guard of `guard` elements, all filled with a NaN bit pattern: an element the
-    kernel never writes fails the comparison, and a write past the end changes the guard. `init` pre-fills the
-    tensor itself (accumulated outputs start from non-zero values, S and the statistics from zero)."""
-    BITS = {BF16: (torch.int16, 0x7FA5), F32T: (torch.int32, 0x7FC0A5A5), F64T: (torch.int64, 0x7FF8A5A5A5A5A5A5)}
-
-    def __init__(self, shape, dtype, guard=64, init=None):
-        self.n = math.prod(shape)
-        self.buf = torch.empty(self.n + max(guard, 64), dtype=dtype, device=DEV)
-        ity, bits = self.BITS[dtype]
-        self.buf.view(ity).fill_(bits)
-        self.t = self.buf[:self.n].view(shape)
-        if init is not None:
-            self.t.copy_(init)
-
-    def ptr(self):
-        return self.t.data_ptr()
-
-    def untouched(self):
-        ity, bits = self.BITS[self.buf.dtype]
-        return bool((self.buf.view(ity) == bits).all())
-
-    def check_guard(self, name):
-        ity, bits = self.BITS[self.buf.dtype]
-        changed = int((self.buf[self.n:].view(ity) != bits).sum())
-        assert changed == 0, f'{name}: {changed} guard elements after the tensor were overwritten'
 
 
 _WS = {}
