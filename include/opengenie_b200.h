@@ -85,10 +85,12 @@ int og_conv3d_dgrad(const void* dy, int cout, int w_rows, const void* w, int ldw
                     int pt, int ph, int pw, void* dx, int dx_f32, int N, int T, int H, int W, int cin,
                     void* workspace, size_t workspace_bytes, og_stream_t stream);
 
-/* Weight gradient (autograd's conv3d backward-weight). ACCUMULATES into dw (caller zeroes it):
+/* Weight gradient (autograd's conv3d backward-weight). ACCUMULATES into dw (zero it for a plain gradient):
  *   dw[co][tap][ci] += sum_{n,t,h,w} dy[n,t,h,w,co] * x[n, t+it-pt, h+ih-ph, w+iw-pw, ci]
- * dy: bf16 [N,T,H,W,cout]; x: bf16 [N,T,H,W,cin] (cin % 64 == 0); dw: fp32, row stride ld_dw elements,
- * tap-major / channel-minor inside a row (the channels_last_3d order of the torch weight).
+ * dy: bf16 [N,T,H,W,cout] (cout % 8 == 0); x: bf16 [N,T,H,W,cin] (cin % 64 == 0); N, T, H, W > 0;
+ * 0 <= pt < kt (likewise ph, pw). dw: fp32, row stride ld_dw >= kt*kh*kw*cin elements (the words between rows are
+ * not touched), tap-major / channel-minor inside a row (the channels_last_3d order of the torch weight); any
+ * alignment (an odd ld_dw or a dw off 8 bytes takes scalar accesses).
  * workspace (may be NULL): fp32 scratch for the stream-K split over the SMs — up to two 128 x 256 partial tiles
  * (+ 128 bias partials) per SM, added in k order, so the result is the same every run; with less workspace the split
  * shrinks to what fits (whole tiles per CTA without a workspace). */
@@ -96,7 +98,8 @@ int og_conv3d_wgrad(const void* dy, int cout, const void* x, int cin, float* dw,
                     int kw, int pt, int ph, int pw, int N, int T, int H, int W, void* workspace,
                     size_t workspace_bytes, og_stream_t stream);
 /* og_conv3d_wgrad + the bias gradient of the same nn.Conv3d in one launch: dbias[c] += sum over voxels of dy[v][c] for
- * c < n_bias (1 <= n_bias <= cout; caller zeroes dbias). The sums come out of the same tensor-core pass (an extra N = 16
+ * c < n_bias (1 <= n_bias <= cout; dbias is not NULL and ACCUMULATES like dw: zero it for a plain gradient; dbias[c]
+ * for c >= n_bias is not touched). The sums come out of the same tensor-core pass (an extra N = 16
  * product against a tile of ones in the tiles that hold the first columns). Replaces the bias half of autograd's conv3d backward
  * (genie/module/video.py:178-192, 609-629). */
 int og_conv3d_wgrad_bias(const void* dy, int cout, const void* x, int cin, float* dw, int64_t ld_dw, int kt, int kh,
@@ -106,6 +109,9 @@ int og_conv3d_wgrad_bias(const void* dy, int cout, const void* x, int cin, float
 /* Strided CausalConv3d — SpaceTimeDownsample (genie/module/video.py:457-483) — as the SAME implicit GEMM, no im2col:
  * geometry of video.py:154-164 (time padded at the FRONT only by pt = (kt-1) + (1-st); space symmetrically by
  * ph = (kh-1)/2, pw = (kw-1)/2), output extents To = (T+pt-kt)/st+1, Ho = (H+2ph-kh)/sh+1, Wo likewise.
+ * N, T, H, W > 0, strides 1..8, and every padded extent at least the kernel (T+pt >= kt, H+2ph >= kh, W+2pw >= kw):
+ * a shorter input has no output, as in F.conv3d, and is rejected. The strided TMA boxes must span at most 256 input
+ * positions per dimension (fwd, wgrad); otherwise -1.
  *   fwd  : the A box of a tap is a TMA box with element strides (st,sh,sw); OOB zero fill is the padding.
  *   dgrad: input position i only receives taps == (i+pad) mod s, so the input grid splits into st*sh*sw residue
  *          classes; each is a stride-1 implicit GEMM over dy with its tap subset, stored at stride s into dx
@@ -113,7 +119,8 @@ int og_conv3d_wgrad_bias(const void* dy, int cout, const void* x, int cin, float
  *   wgrad: dY boxes on the output grid, x boxes strided on the input grid; ACCUMULATES into dw; workspace as
  *          og_conv3d_wgrad.
  * x / dx: bf16 [N,T,H,W,cin] (cin % 64 == 0); out: [N,To,Ho,Wo,cout]; dy: bf16 [N,To,Ho,Wo,cout] with cout % 64 == 0
- * (zero padded by the caller; w_rows = real weight rows); w: packed bf16 [cout][ldw] as for og_conv3d_fwd. */
+ * (zero padded by the caller; w_rows = real weight rows, the rows after them are never read); w: packed bf16
+ * [cout][ldw] as for og_conv3d_fwd (ldw >= kt*kh*kw*cin, ldw % 8 == 0). wgrad: dw as og_conv3d_wgrad. */
 int og_conv3d_strided_fwd(const void* x, int cin, int kt, int kh, int kw, int st, int sh, int sw, int pt, int ph, int pw,
                           const void* w, int ldw, const float* bias, void* out, int out_f32, int N, int T, int H, int W,
                           int cout, og_stream_t stream);

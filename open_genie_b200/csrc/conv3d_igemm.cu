@@ -1153,7 +1153,12 @@ extern "C" int og_conv3d_dgrad(const void* dy, int cout, int w_rows, const void*
   return launch_igemm(L, (cudaStream_t)stream);
 }
 
-static int out_extent(int in, int pad_front, int pad_back, int k, int s) { return (in + pad_front + pad_back - k) / s + 1; }
+// Output extent of a strided convolution; 0 when the padded input is shorter than the kernel (truncating division
+// would give such an input one output where F.conv3d raises).
+static int out_extent(int in, int pad_front, int pad_back, int k, int s) {
+  const int span = in + pad_front + pad_back - k;
+  return span < 0 ? 0 : span / s + 1;
+}
 
 // Strided CausalConv3d forward (SpaceTimeDownsample, genie/module/video.py:457-483; geometry video.py:154-164: time is
 // padded at the FRONT only by pt = kt-1 + (1-st), space symmetrically by (k-1)//2), as the SAME implicit GEMM: the A
@@ -1167,8 +1172,9 @@ extern "C" int og_conv3d_strided_fwd(const void* x, int cin, int kt, int kh, int
   OG_REQUIRE(kt >= 1 && kh >= 1 && kw >= 1 && st >= 1 && sh >= 1 && sw >= 1 && st <= 8 && sh <= 8 && sw <= 8 && pt >= 0 &&
                  ph >= 0 && pw >= 0, "conv3d_strided_fwd: bad kernel / stride / padding");
   OG_REQUIRE(ldw >= kt * kh * kw * cin && ldw % 8 == 0, "conv3d_strided_fwd: bad ldw=%d", ldw);
+  OG_REQUIRE(N > 0 && T > 0 && H > 0 && W > 0, "conv3d_strided_fwd: extents must be positive");
   const int To = out_extent(T, pt, 0, kt, st), Ho = out_extent(H, ph, ph, kh, sh), Wo = out_extent(W, pw, pw, kw, sw);
-  OG_REQUIRE(To >= 1 && Ho >= 1 && Wo >= 1, "conv3d_strided_fwd: empty output");
+  OG_REQUIRE(To >= 1 && Ho >= 1 && Wo >= 1, "conv3d_strided_fwd: empty output (padded input smaller than the kernel)");
   IgemmLaunch L;
   L.a0 = x; L.c0 = cin; L.aT = T; L.aH = H; L.aW = W;
   L.astride[0] = st; L.astride[1] = sh; L.astride[2] = sw;
@@ -1191,9 +1197,14 @@ extern "C" int og_conv3d_strided_dgrad(const void* dy, int cout, int w_rows, con
   using namespace og;
   OG_REQUIRE(dy && w && dx, "conv3d_strided_dgrad: null pointer");
   OG_REQUIRE(cout > 0 && cout % 64 == 0 && cin > 0 && cin % 64 == 0, "conv3d_strided_dgrad: channels must be multiples of 64");
-  OG_REQUIRE(w_rows > 0 && w_rows <= cout && ldw % 8 == 0, "conv3d_strided_dgrad: bad w_rows / ldw");
+  OG_REQUIRE(w_rows > 0 && w_rows <= cout && ldw % 8 == 0 && ldw >= kt * kh * kw * cin,
+             "conv3d_strided_dgrad: bad w_rows / ldw");
+  OG_REQUIRE(kt >= 1 && kh >= 1 && kw >= 1 && st >= 1 && sh >= 1 && sw >= 1 && st <= 8 && sh <= 8 && sw <= 8 && pt >= 0 &&
+                 ph >= 0 && pw >= 0, "conv3d_strided_dgrad: bad kernel / stride / padding");
+  // checked before the memset below, whose size they give
+  OG_REQUIRE(N > 0 && T > 0 && H > 0 && W > 0, "conv3d_strided_dgrad: extents must be positive");
   const int To = out_extent(T, pt, 0, kt, st), Ho = out_extent(H, ph, ph, kh, sh), Wo = out_extent(W, pw, pw, kw, sw);
-  OG_REQUIRE(To >= 1 && Ho >= 1 && Wo >= 1, "conv3d_strided_dgrad: empty output");
+  OG_REQUIRE(To >= 1 && Ho >= 1 && Wo >= 1, "conv3d_strided_dgrad: empty output (padded input smaller than the kernel)");
   const int k[3] = {kt, kh, kw}, s[3] = {st, sh, sw}, pd[3] = {pt, ph, pw}, in[3] = {T, H, W};
   bool any_empty = false;
   for (int d = 0; d < 3; ++d)

@@ -329,8 +329,14 @@ static int launch_wgrad(const void* dy, int cout, const void* x, int cin, float*
   OG_REQUIRE(kt >= 1 && kh >= 1 && kw >= 1 && pt >= 0 && ph >= 0 && pw >= 0 && pt < kt && ph < kh && pw < kw,
              "conv3d_wgrad: bad kernel/padding");
   OG_REQUIRE(st >= 1 && sh >= 1 && sw >= 1 && st <= 8 && sh <= 8 && sw <= 8, "conv3d_wgrad: bad stride");
+  OG_REQUIRE(N > 0 && T > 0 && H > 0 && W > 0 && Ti > 0 && Hi > 0 && Wi > 0,
+             "conv3d_wgrad: extents must be positive (N=%d T=%d H=%d W=%d)", N, T, H, W);
+  // rows closer than ncols would overlap, and two CTAs would add into the same words
+  OG_REQUIRE(ld_dw >= (int64_t)kt * kh * kw * cin, "conv3d_wgrad: ld_dw=%lld must be >= kt*kh*kw*cin = %d",
+             (long long)ld_dw, kt * kh * kw * cin);
   int bw, bh, bt, bn;
   choose_voxel_box(kVox, N, T, H, W, &bw, &bh, &bt, &bn);
+  OG_REQUIRE(bw * sw <= 256 && bh * sh <= 256 && bt * st <= 256, "conv3d_wgrad: strided box exceeds the TMA limit");
   WgradParams p;
   memset(&p, 0, sizeof(p));
   p.kt = kt; p.kh = kh; p.kw = kw; p.pt = pt; p.ph = ph; p.pw = pw;
@@ -382,7 +388,6 @@ static int launch_wgrad(const void* dy, int cout, const void* x, int cin, float*
                        (uint64_t)Ti * Hi * Wi * cin * 2};
     uint32_t box[5] = {64, (uint32_t)(bw * sw), (uint32_t)(bh * sh), (uint32_t)(bt * st), (uint32_t)bn};
     uint32_t es[5] = {1, (uint32_t)sw, (uint32_t)sh, (uint32_t)st, 1};
-    OG_REQUIRE(box[1] <= 256 && box[2] <= 256 && box[3] <= 256, "conv3d_wgrad: strided box exceeds the TMA limit");
     int r = make_tmap_bf16(&mapX, x, 5, dims, str, box, es);
     if (r != OG_OK) return r;
   }
@@ -433,11 +438,12 @@ extern "C" int og_conv3d_wgrad_bias(const void* dy, int cout, const void* x, int
 extern "C" int og_conv3d_strided_wgrad(const void* dy, int cout, const void* x, int cin, float* dw, int64_t ld_dw, int kt,
                                        int kh, int kw, int st, int sh, int sw, int pt, int ph, int pw, int N, int T, int H,
                                        int W, void* workspace, size_t workspace_bytes, og_stream_t stream) {
+  OG_REQUIRE(st >= 1 && sh >= 1 && sw >= 1, "conv3d_strided_wgrad: bad stride");
+  // a padded extent smaller than the kernel has no output (truncating division would give it one)
+  OG_REQUIRE(T + pt >= kt && H + 2 * ph >= kh && W + 2 * pw >= kw,
+             "conv3d_strided_wgrad: padded input (%d,%d,%d) smaller than the kernel (%d,%d,%d)", T + pt, H + 2 * ph,
+             W + 2 * pw, kt, kh, kw);
   const int To = (T + pt - kt) / st + 1, Ho = (H + 2 * ph - kh) / sh + 1, Wo = (W + 2 * pw - kw) / sw + 1;
-  if (To < 1 || Ho < 1 || Wo < 1) {
-    og::set_error("conv3d_strided_wgrad: empty output");
-    return OG_ERR_INVALID_ARGUMENT;
-  }
   return launch_wgrad(dy, cout, x, cin, dw, ld_dw, kt, kh, kw, pt, ph, pw, N, To, Ho, Wo, T, H, W, st, sh, sw, workspace,
                       workspace_bytes, stream);
 }

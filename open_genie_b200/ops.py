@@ -374,6 +374,11 @@ class ConvGeom:
     def out_dims(self, T, H, W):
         if self.direct:
             return T, H, W
+        padded = (T + self.pt, H + 2 * self.ph, W + 2 * self.pw)
+        if any(p < k for p, k in zip(padded, (self.kt, self.kh, self.kw))):
+            # F.conv3d raises here too; the kernels reject such a shape rather than compute an output for it
+            raise ValueError(f'strided conv: padded input {padded} (T,H,W = {(T, H, W)}) is smaller than the kernel '
+                             f'{(self.kt, self.kh, self.kw)}')
         return ((T + self.pt - self.kt) // self.st + 1, (H + 2 * self.ph - self.kh) // self.sh + 1,
                 (W + 2 * self.pw - self.kw) // self.sw + 1)
 
