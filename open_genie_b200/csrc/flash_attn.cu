@@ -3,7 +3,7 @@
 // Reference: F.scaled_dot_product_attention(q, k, v, scale = n_head * d_head**-0.5) reached from
 // SpatialAttention.forward -> Attention.forward (genie/module/attention.py:279-307, 199-239), with
 // q = k = v = LayerNorm(RoPE(x)) in the HEAD-valid configuration. Layout: [nseq][S][C] bf16 rows
-// (one sequence = the H*W tokens of one frame, contiguous in NDHWC), head h = columns [h*64, h*64+64).
+// (one sequence = the H*W tokens of one frame, contiguous in NDHWC), head h = columns [h*d, h*d+d), d = 64 or 128.
 //
 // Every kernel is one warpgroup (128 threads) owning a 64-row tile; thread 0 streams the other operand's 64-row tiles
 // through a two-stage TMA ring (rows beyond S are zero-filled by TMA and masked). Accumulators live in registers in the
@@ -20,15 +20,31 @@
 //             dQ_i += dS K_j                             (A = dS from registers, B = K_j MN-major)
 // with P = exp(S*scale - lse), dS = P * (dP - delta) * scale, delta = rowsum(dO * O).
 // No atomics, no fp32 gradient buffers; outputs are bf16 in the activation layout.
+//
+// d_head = 128 (og_flash_attn_fwd_d128_kernel, og_flash_attn_bwd_d128_kernel<MODE>, og_attn_delta_d128_kernel): the
+// same kernel bodies (flash_fwd / flash_bwd, templated on kH = d / 64). A 64 x 128 tile is two 64 x 64 half-tiles of
+// the 128-byte swizzle, 8 KiB apart, each its own TMA box (a SWIZZLE_128B box is at most 64 bf16 wide) on the same
+// mbarrier. The K-major score GEMMs walk 8 k16 slices, slices 4-7 from the second half. The MN-major B operands
+// (V in P V, dO and Q in MODE 0, K in MODE 1) are taken one half at a time: one m64n64k16 per half and slice into its
+// own m64n64 accumulator, through the same gemm_acc / descriptor as d = 64. That keeps one descriptor form for both
+// widths and lets MODE 0 split the head columns between warpgroups; the issue count equals one m64n128k16 per slice
+// with the atom stride in the descriptor.
+//   forward: O as two m64n64 fragments (64 registers); smem Q + 2 x (K, V) = 80 KiB.
+//   MODE 0: two warpgroups (256 threads) per key tile. Both compute the full S^T and dP^T (contracting over all 128
+//           dims: the score GEMMs run twice), warpgroup w keeps dV and dK for head columns [64w, 64w + 64), so a
+//           thread holds 2 x 32 accumulators as at d = 64. smem 2 + 2 x 2 tiles = 96 KiB.
+//   MODE 1: one warpgroup, dQ as two m64n64 fragments.
+// Registers (nvcc 12.9, -O3, sm_90a; no spills): d = 64: fwd 98, MODE 0 168, MODE 1 122; d = 128: fwd 130,
+// MODE 0 175 (256 threads), MODE 1 154.
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 
 namespace og {
 extern std::atomic<uint64_t> g_launches;
 
-static constexpr int kD = 64;            // head dim
+static constexpr int kD = 64;            // width of one 64-column half of a head (the whole head at d_head = 64)
 static constexpr int kTile = 64;         // rows per tile (queries or keys)
-static constexpr int kTileBytes = kTile * kD * 2;  // 8 KiB
+static constexpr int kTileBytes = kTile * kD * 2;  // 8 KiB: one 64 x 64 swizzled half-tile
 static constexpr int kFaThreads = 128;
 
 struct FaParams {
@@ -63,14 +79,19 @@ __device__ __forceinline__ void frag_to_a(const float (&x)[32], uint32_t (&a)[4]
   }
 }
 
-// D = X Y^T over the 64 head dims: both tiles K-major [64 rows][64 d] with the 128-byte swizzle
+// D = X Y^T over the 64 kH head dims: both tiles K-major, kH half-tiles [64 rows][64 d] with the 128-byte swizzle,
+// kTileBytes apart (k16 slices 4c .. 4c + 3 come from half c)
+template <int kH>
 __device__ __forceinline__ void gemm_rows(float (&d)[32], uint32_t x_addr, uint32_t y_addr) {
 #pragma unroll
-  for (int k = 0; k < kD / 16; ++k)
-    wgmma_ss<64, 0, 0>(d, gmma_desc_sw128(x_addr + k * 32, 16, 1024), gmma_desc_sw128(y_addr + k * 32, 16, 1024), k > 0);
+  for (int c = 0; c < kH; ++c)
+#pragma unroll
+    for (int k = 0; k < kD / 16; ++k)
+      wgmma_ss<64, 0, 0>(d, gmma_desc_sw128(x_addr + c * kTileBytes + k * 32, 16, 1024),
+                         gmma_desc_sw128(y_addr + c * kTileBytes + k * 32, 16, 1024), c > 0 || k > 0);
 }
 
-// D += A Y: A from registers (64 rows x 64 k), Y a [64 k rows][64 d] tile read MN-major
+// D += A Y: A from registers (64 rows x 64 k), Y a [64 k rows][64 d] half-tile read MN-major
 __device__ __forceinline__ void gemm_acc(float (&d)[32], const uint32_t (&a)[4][4], uint32_t y_addr) {
 #pragma unroll
   for (int kk = 0; kk < 4; ++kk) wgmma_rs_n64<1>(d, a[kk], gmma_desc_sw128(y_addr + kk * 2048, 8192, 1024), 1);
@@ -79,7 +100,7 @@ __device__ __forceinline__ void gemm_acc(float (&d)[32], const uint32_t (&a)[4][
 // 64 x 64 fragment (times `sc`) -> bf16 rows of [nseq][S][C] (rows >= S dropped)
 __device__ __forceinline__ void store_frag(const float (&d)[32], float sc, __nv_bfloat16* base, long long row0, int S,
                                            int row_in_seq0, int C) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
 #pragma unroll
   for (int rr = 0; rr < 2; ++rr) {
     const int r = warp * 16 + (lane >> 2) + rr * 8;
@@ -91,14 +112,24 @@ __device__ __forceinline__ void store_frag(const float (&d)[32], float sc, __nv_
   }
 }
 
-__global__ void __launch_bounds__(kFaThreads)
-    og_flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                             const __grid_constant__ CUtensorMap mapV, const FaParams p) {
+// rows row0 .. row0 + 63, head columns [h 64 kH, h 64 kH + 64 kH) of one sequence -> kH half-tiles
+template <int kH>
+__device__ __forceinline__ void load_rows(uint8_t* dst, const CUtensorMap* map, uint64_t* bar, int h, int row0, int seq) {
+#pragma unroll
+  for (int c = 0; c < kH; ++c) tma_load_3d(dst + c * kTileBytes, map, bar, (h * kH + c) * kD, row0, seq);
+}
+
+// Forward of one (sequence, head, 64-query tile); kH = d_head / 64 half-tiles per row tile, O as kH m64n64 fragments.
+template <int kH>
+__device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtensorMap* mapK, const CUtensorMap* mapV,
+                                          const FaParams& p) {
+  constexpr int kTB = kH * kTileBytes;   // one 64-row tile
+  constexpr int kDh = kH * kD;           // d_head
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                   // 8 KiB
-  uint8_t* sKV = smem + kTileBytes;     // 2 stages x (K 8 KiB + V 8 KiB)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + 4 * kTileBytes);
+  uint8_t* sQ = smem;                   // 1 tile
+  uint8_t* sKV = smem + kTB;            // 2 stages x (K, V)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + 4 * kTB);
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;  // [2]
 
@@ -111,9 +142,9 @@ __global__ void __launch_bounds__(kFaThreads)
   const int q0 = qt * kTile;
 
   if (tid == 0) {
-    tma_prefetch_desc(&mapQ);
-    tma_prefetch_desc(&mapK);
-    tma_prefetch_desc(&mapV);
+    tma_prefetch_desc(mapQ);
+    tma_prefetch_desc(mapK);
+    tma_prefetch_desc(mapV);
     mbar_init(q_full, 1);
     mbar_init(&kv_full[0], 1);
     mbar_init(&kv_full[1], 1);
@@ -121,30 +152,32 @@ __global__ void __launch_bounds__(kFaThreads)
   }
   __syncthreads();
   if (tid == 0) {
-    mbar_expect_tx(q_full, kTileBytes);
-    tma_load_3d(sQ, &mapQ, q_full, h * kD, q0, seq);
+    mbar_expect_tx(q_full, kTB);
+    load_rows<kH>(sQ, mapQ, q_full, h, q0, seq);
     for (int j = 0; j < 2 && j < p.kv_tiles; ++j) {
-      mbar_expect_tx(&kv_full[j], 2 * kTileBytes);
-      tma_load_3d(sKV + j * 2 * kTileBytes, &mapK, &kv_full[j], h * kD, j * kTile, seq);
-      tma_load_3d(sKV + j * 2 * kTileBytes + kTileBytes, &mapV, &kv_full[j], h * kD, j * kTile, seq);
+      mbar_expect_tx(&kv_full[j], 2 * kTB);
+      load_rows<kH>(sKV + j * 2 * kTB, mapK, &kv_full[j], h, j * kTile, seq);
+      load_rows<kH>(sKV + j * 2 * kTB + kTB, mapV, &kv_full[j], h, j * kTile, seq);
     }
   }
   // Online softmax in base 2 with the scale folded in: p = 2^(s*c - m), c = scale*log2(e). l is a per-thread partial
   // row sum (the quad's four partial sums are added once at the end).
   const float cl2 = p.scale * 1.4426950408889634f;
-  float o[32];
+  float o[kH][32];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  for (int c = 0; c < kH; ++c)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   const uint32_t q_addr = smem_u32(sQ);
   mbar_wait(q_full, 0);
   for (int j = 0; j < p.kv_tiles; ++j) {
     const int st = j & 1;
     mbar_wait(&kv_full[st], (j >> 1) & 1);
-    const uint32_t k_addr = smem_u32(sKV + st * 2 * kTileBytes), v_addr = k_addr + kTileBytes;
+    const uint32_t k_addr = smem_u32(sKV + st * 2 * kTB), v_addr = k_addr + kTB;
     float s[32];
     wgmma_fence();
-    gemm_rows(s, q_addr, k_addr);
+    gemm_rows<kH>(s, q_addr, k_addr);
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(s);
@@ -178,19 +211,23 @@ __global__ void __launch_bounds__(kFaThreads)
       l[rr] = l[rr] * alpha[rr] + ls;
     }
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+    for (int c = 0; c < kH; ++c)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o[c][i] *= alpha[(i >> 1) & 1];
     uint32_t a[4][4];
     frag_to_a(s, a);
     wgmma_fence();
-    gemm_acc(o, a, v_addr);
+#pragma unroll
+    for (int c = 0; c < kH; ++c) gemm_acc(o[c], a, v_addr + c * kTileBytes);
     wgmma_commit();
     wgmma_wait<0>();
-    reg_fence(o);
+#pragma unroll
+    for (int c = 0; c < kH; ++c) reg_fence(o[c]);
     __syncthreads();  // every warp is done with stage st
     if (tid == 0 && j + 2 < p.kv_tiles) {
-      mbar_expect_tx(&kv_full[st], 2 * kTileBytes);
-      tma_load_3d(sKV + st * 2 * kTileBytes, &mapK, &kv_full[st], h * kD, (j + 2) * kTile, seq);
-      tma_load_3d(sKV + st * 2 * kTileBytes + kTileBytes, &mapV, &kv_full[st], h * kD, (j + 2) * kTile, seq);
+      mbar_expect_tx(&kv_full[st], 2 * kTB);
+      load_rows<kH>(sKV + st * 2 * kTB, mapK, &kv_full[st], h, (j + 2) * kTile, seq);
+      load_rows<kH>(sKV + st * 2 * kTB + kTB, mapV, &kv_full[st], h, (j + 2) * kTile, seq);
     }
   }
 #pragma unroll
@@ -200,20 +237,26 @@ __global__ void __launch_bounds__(kFaThreads)
   }
   const float inv[2] = {1.f / l[0], 1.f / l[1]};
 #pragma unroll
-  for (int i = 0; i < 32; ++i) o[i] *= inv[(i >> 1) & 1];
+  for (int c = 0; c < kH; ++c)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[c][i] *= inv[(i >> 1) & 1];
   const long long row0 = (long long)seq * p.S + q0;
-  store_frag(o, 1.f, p.out + h * kD, row0, p.S, q0, p.C);
+#pragma unroll
+  for (int c = 0; c < kH; ++c) store_frag(o[c], 1.f, p.out + h * kDh + c * kD, row0, p.S, q0, p.C);
 #pragma unroll
   for (int rr = 0; rr < 2; ++rr) {
     const int r = warp * 16 + (lane >> 2) + rr * 8;
     if (q0 + r >= p.S) continue;
     if (p.res) {  // second output: attention + residual, added in fp32 before the rounding
-      const long long off = (row0 + r) * p.C + h * kD + 2 * (lane & 3);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.res + off + 8 * j));
-        *reinterpret_cast<uint32_t*>(p.out_res + off + 8 * j) =
-            pack_bf16x2(o[4 * j + 2 * rr] + t.x, o[4 * j + 2 * rr + 1] + t.y);
+      for (int c = 0; c < kH; ++c) {
+        const long long off = (row0 + r) * p.C + h * kDh + c * kD + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.res + off + 8 * j));
+          *reinterpret_cast<uint32_t*>(p.out_res + off + 8 * j) =
+              pack_bf16x2(o[c][4 * j + 2 * rr] + t.x, o[c][4 * j + 2 * rr + 1] + t.y);
+        }
       }
     }
     if (p.lse && (lane & 3) == 0)
@@ -221,27 +264,43 @@ __global__ void __launch_bounds__(kFaThreads)
   }
 }
 
+__global__ void __launch_bounds__(kFaThreads)
+    og_flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                             const __grid_constant__ CUtensorMap mapV, const FaParams p) {
+  flash_fwd<1>(&mapQ, &mapK, &mapV, p);
+}
+
+__global__ void __launch_bounds__(kFaThreads)
+    og_flash_attn_fwd_d128_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                  const __grid_constant__ CUtensorMap mapV, const FaParams p) {
+  flash_fwd<2>(&mapQ, &mapK, &mapV, p);
+}
+
 // ------------------------------------------------------------------------------------------------
 // backward (see the file header). The softmax scale is applied once per output element of dK / dQ, not per score.
+// kH = d_head / 64. MODE 0 at kH = 2 runs two warpgroups: both compute the full S^T and dP^T (contracting over all
+// 128 head dims), warpgroup w keeps dV and dK for head columns [64 w, 64 w + 64). MODE 1 keeps dQ as kH fragments.
 // ------------------------------------------------------------------------------------------------
-template <int MODE>
-__global__ void __launch_bounds__(kFaThreads)
-    og_flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                             const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
-                             const FaBwdParams p) {
+template <int MODE, int kH>
+__device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtensorMap* mapK, const CUtensorMap* mapV,
+                                          const CUtensorMap* mapDO, const FaBwdParams& p) {
+  constexpr int kTB = kH * kTileBytes;
+  constexpr int kDh = kH * kD;
+  constexpr int kNA = MODE == 0 ? 1 : kH;   // accumulator fragments per thread and output
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sFix = smem;                    // stationary pair: MODE 0: K_j, V_j ; MODE 1: Q_i, dO_i   (2 x 8 KiB)
-  uint8_t* sStr = smem + 2 * kTileBytes;   // streamed pair, 2 stages x (2 x 8 KiB)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sStr + 4 * kTileBytes);
+  uint8_t* sFix = smem;                    // stationary pair: MODE 0: K_j, V_j ; MODE 1: Q_i, dO_i   (2 tiles)
+  uint8_t* sStr = smem + 2 * kTB;          // streamed pair, 2 stages x (2 tiles)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sStr + 4 * kTB);
   uint64_t* fix_full = bars;
   uint64_t* str_full = bars + 1;   // [2]
-  const CUtensorMap* mapF0 = MODE == 0 ? &mapK : &mapQ;
-  const CUtensorMap* mapF1 = MODE == 0 ? &mapV : &mapDO;
-  const CUtensorMap* mapS0 = MODE == 0 ? &mapQ : &mapK;
-  const CUtensorMap* mapS1 = MODE == 0 ? &mapDO : &mapV;
+  const CUtensorMap* mapF0 = MODE == 0 ? mapK : mapQ;
+  const CUtensorMap* mapF1 = MODE == 0 ? mapV : mapDO;
+  const CUtensorMap* mapS0 = MODE == 0 ? mapQ : mapK;
+  const CUtensorMap* mapS1 = MODE == 0 ? mapDO : mapV;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = (tid >> 5) & 3, lane = tid & 31;
+  const int wg = MODE == 0 && kH == 2 ? tid >> 7 : 0;   // MODE 0 at d_head 128: the head-column half this thread owns
   int id = blockIdx.x;
   const int own = id % p.tiles;  // MODE 0: kv tile ; MODE 1: q tile
   id /= p.tiles;
@@ -250,10 +309,10 @@ __global__ void __launch_bounds__(kFaThreads)
   const long long stat0 = ((long long)seq * p.nh + h) * p.S;   // lse / delta row of this (sequence, head)
 
   if (tid == 0) {
-    tma_prefetch_desc(&mapQ);
-    tma_prefetch_desc(&mapK);
-    tma_prefetch_desc(&mapV);
-    tma_prefetch_desc(&mapDO);
+    tma_prefetch_desc(mapQ);
+    tma_prefetch_desc(mapK);
+    tma_prefetch_desc(mapV);
+    tma_prefetch_desc(mapDO);
     mbar_init(fix_full, 1);
     mbar_init(&str_full[0], 1);
     mbar_init(&str_full[1], 1);
@@ -261,13 +320,13 @@ __global__ void __launch_bounds__(kFaThreads)
   }
   __syncthreads();
   if (tid == 0) {
-    mbar_expect_tx(fix_full, 2 * kTileBytes);
-    tma_load_3d(sFix, mapF0, fix_full, h * kD, own * kTile, seq);
-    tma_load_3d(sFix + kTileBytes, mapF1, fix_full, h * kD, own * kTile, seq);
+    mbar_expect_tx(fix_full, 2 * kTB);
+    load_rows<kH>(sFix, mapF0, fix_full, h, own * kTile, seq);
+    load_rows<kH>(sFix + kTB, mapF1, fix_full, h, own * kTile, seq);
     for (int it = 0; it < 2 && it < p.tiles; ++it) {
-      mbar_expect_tx(&str_full[it], 2 * kTileBytes);
-      tma_load_3d(sStr + it * 2 * kTileBytes, mapS0, &str_full[it], h * kD, it * kTile, seq);
-      tma_load_3d(sStr + it * 2 * kTileBytes + kTileBytes, mapS1, &str_full[it], h * kD, it * kTile, seq);
+      mbar_expect_tx(&str_full[it], 2 * kTB);
+      load_rows<kH>(sStr + it * 2 * kTB, mapS0, &str_full[it], h, it * kTile, seq);
+      load_rows<kH>(sStr + it * 2 * kTB + kTB, mapS1, &str_full[it], h, it * kTile, seq);
     }
   }
   const float cl2 = p.scale * 1.4426950408889634f;
@@ -285,21 +344,23 @@ __global__ void __launch_bounds__(kFaThreads)
       }
     }
   }
-  float acc0[32], acc1[32];   // MODE 0: dV, dK ; MODE 1: dQ (acc1 unused)
+  float acc0[kNA][32], acc1[kNA][32];   // MODE 0: dV, dK (head columns of half wg) ; MODE 1: dQ (acc1 unused)
 #pragma unroll
-  for (int i = 0; i < 32; ++i) acc0[i] = acc1[i] = 0.f;
-  const uint32_t f0 = smem_u32(sFix), f1 = f0 + kTileBytes;
+  for (int c = 0; c < kNA; ++c)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc0[c][i] = acc1[c][i] = 0.f;
+  const uint32_t f0 = smem_u32(sFix), f1 = f0 + kTB;
   mbar_wait(fix_full, 0);
   for (int it = 0; it < p.tiles; ++it) {
     const int st = it & 1;
     mbar_wait(&str_full[st], (it >> 1) & 1);
-    const uint32_t s0 = smem_u32(sStr + st * 2 * kTileBytes), s1 = s0 + kTileBytes;
+    const uint32_t s0 = smem_u32(sStr + st * 2 * kTB), s1 = s0 + kTB;
     // MODE 0: s = S^T = K Q^T, dp = dP^T = V dO^T (rows = keys, columns = queries)
     // MODE 1: s = S   = Q K^T, dp = dP   = dO V^T (rows = queries, columns = keys)
     float s[32], dp[32];
     wgmma_fence();
-    gemm_rows(s, f0, s0);
-    gemm_rows(dp, f1, s1);
+    gemm_rows<kH>(s, f0, s0);
+    gemm_rows<kH>(dp, f1, s1);
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(s);
@@ -335,29 +396,50 @@ __global__ void __launch_bounds__(kFaThreads)
     wgmma_fence();
     if (MODE == 0) {
       frag_to_a(s, a_p);
-      gemm_acc(acc0, a_p, s1);    // dV_j += P^T dO_i
-      gemm_acc(acc1, a_ds, s0);   // dK_j += dS^T Q_i
+      gemm_acc(acc0[0], a_p, s1 + wg * kTileBytes);    // dV_j += P^T dO_i
+      gemm_acc(acc1[0], a_ds, s0 + wg * kTileBytes);   // dK_j += dS^T Q_i
     } else {
-      gemm_acc(acc0, a_ds, s0);   // dQ_i += dS K_j
+#pragma unroll
+      for (int c = 0; c < kNA; ++c) gemm_acc(acc0[c], a_ds, s0 + c * kTileBytes);   // dQ_i += dS K_j
     }
     wgmma_commit();
     wgmma_wait<0>();
-    reg_fence(acc0);
-    reg_fence(acc1);
+#pragma unroll
+    for (int c = 0; c < kNA; ++c) {
+      reg_fence(acc0[c]);
+      reg_fence(acc1[c]);
+    }
     __syncthreads();  // every warp is done with stage st
     if (tid == 0 && it + 2 < p.tiles) {
-      mbar_expect_tx(&str_full[st], 2 * kTileBytes);
-      tma_load_3d(sStr + st * 2 * kTileBytes, mapS0, &str_full[st], h * kD, (it + 2) * kTile, seq);
-      tma_load_3d(sStr + st * 2 * kTileBytes + kTileBytes, mapS1, &str_full[st], h * kD, (it + 2) * kTile, seq);
+      mbar_expect_tx(&str_full[st], 2 * kTB);
+      load_rows<kH>(sStr + st * 2 * kTB, mapS0, &str_full[st], h, (it + 2) * kTile, seq);
+      load_rows<kH>(sStr + st * 2 * kTB + kTB, mapS1, &str_full[st], h, (it + 2) * kTile, seq);
     }
   }
   const long long row0 = (long long)seq * p.S + own * kTile;
   if (MODE == 0) {
-    store_frag(acc0, 1.f, p.dv + h * kD, row0, p.S, own * kTile, p.C);
-    store_frag(acc1, p.scale, p.dk + h * kD, row0, p.S, own * kTile, p.C);
+    store_frag(acc0[0], 1.f, p.dv + h * kDh + wg * kD, row0, p.S, own * kTile, p.C);
+    store_frag(acc1[0], p.scale, p.dk + h * kDh + wg * kD, row0, p.S, own * kTile, p.C);
   } else {
-    store_frag(acc0, p.scale, p.dq + h * kD, row0, p.S, own * kTile, p.C);
+#pragma unroll
+    for (int c = 0; c < kNA; ++c) store_frag(acc0[c], p.scale, p.dq + h * kDh + c * kD, row0, p.S, own * kTile, p.C);
   }
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(kFaThreads)
+    og_flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                             const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
+                             const FaBwdParams p) {
+  flash_bwd<MODE, 1>(&mapQ, &mapK, &mapV, &mapDO, p);
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(MODE == 0 ? 2 * kFaThreads : kFaThreads)
+    og_flash_attn_bwd_d128_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                  const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
+                                  const FaBwdParams p) {
+  flash_bwd<MODE, 2>(&mapQ, &mapK, &mapV, &mapDO, p);
 }
 
 // delta[seq][h][s] = sum_d dO * O   (one warp per row, lanes over the head's 64 dims)
@@ -377,6 +459,27 @@ __global__ void og_attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const 
   }
 }
 
+// the same at d_head = 128: four consecutive dims per lane
+__global__ void og_attn_delta_d128_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ d_o,
+                                          float* __restrict__ delta, long long rows, int S, int C, int nh) {
+  const int lane = threadIdx.x & 31;
+  const long long w0 = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+  for (long long t = w0; t < rows * nh; t += nw) {
+    const int h = (int)(t % nh);
+    const long long off = (t / nh) * C + h * 2 * kD + lane * 4;
+    const uint2 ua = *reinterpret_cast<const uint2*>(o + off), ub = *reinterpret_cast<const uint2*>(d_o + off);
+    const float2 a0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&ua.x));
+    const float2 a1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&ua.y));
+    const float2 b0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&ub.x));
+    const float2 b1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&ub.y));
+    float v = a0.x * b0.x + a0.y * b0.y + a1.x * b1.x + a1.y * b1.y;
+    for (int off2 = 16; off2 > 0; off2 >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off2);
+    const long long row = t / nh;
+    if (lane == 0) delta[((row / S) * nh + h) * (long long)S + row % S] = v;
+  }
+}
+
 
 static int make_seq_map(CUtensorMap* m, const void* base, int nseq, int S, int C) {
   uint64_t dims[3] = {(uint64_t)C, (uint64_t)S, (uint64_t)nseq};
@@ -389,11 +492,20 @@ static int make_seq_map(CUtensorMap* m, const void* base, int nseq, int S, int C
 
 using namespace og;
 
+// d_head of C = n_head * d_head, or 0 when the head width has no kernel
+static int flash_d_head(int C, int n_head) {
+  if (n_head < 1) return 0;
+  if (C == n_head * 64) return 64;
+  if (C == n_head * 128) return 128;
+  return 0;
+}
+
 extern "C" int og_flash_attn_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
                                  void* out_res, float* lse, int nseq, int S, int C, int n_head, float scale,
                                  og_stream_t stream) {
   OG_REQUIRE(q && k && v && out, "flash_attn_fwd: null pointer");
-  OG_REQUIRE(n_head >= 1 && C == n_head * kD, "flash_attn_fwd: needs d_head = 64 (C=%d, n_head=%d)", C, n_head);
+  const int dh = flash_d_head(C, n_head);
+  OG_REQUIRE(dh != 0, "flash_attn_fwd: needs d_head = 64 or 128 (C=%d, n_head=%d)", C, n_head);
   OG_REQUIRE(nseq > 0 && S > 0, "flash_attn_fwd: empty problem");
   OG_REQUIRE(scale > 0.f, "flash_attn_fwd: scale must be positive (the row maximum is taken on raw scores)");
   FaParams p;
@@ -411,16 +523,27 @@ extern "C" int og_flash_attn_fwd(const void* q, const void* k, const void* v, vo
   if ((r = make_seq_map(&mq, q, nseq, S, C)) != OG_OK) return r;
   if ((r = make_seq_map(&mk, k, nseq, S, C)) != OG_OK) return r;
   if ((r = make_seq_map(&mv, v, nseq, S, C)) != OG_OK) return r;
-  const size_t smem_bytes = 5 * kTileBytes + 1024 + 64;
-  static bool attr = false;
-  if (!attr) {
-    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)smem_bytes));
-    attr = true;
-  }
   const long long grid = (long long)nseq * n_head * p.q_tiles;
   OG_REQUIRE(grid < (1LL << 31), "flash_attn_fwd: too many tiles");
-  og_flash_attn_fwd_kernel<<<(unsigned)grid, kFaThreads, smem_bytes, (cudaStream_t)stream>>>(mq, mk, mv, p);
+  if (dh == 64) {
+    const size_t smem_bytes = 5 * kTileBytes + 1024 + 64;
+    static bool attr = false;
+    if (!attr) {
+      OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem_bytes));
+      attr = true;
+    }
+    og_flash_attn_fwd_kernel<<<(unsigned)grid, kFaThreads, smem_bytes, (cudaStream_t)stream>>>(mq, mk, mv, p);
+  } else {
+    const size_t smem_bytes = 10 * kTileBytes + 1024 + 64;   // Q, 2 x (K, V) at 16 KiB a tile
+    static bool attr = false;
+    if (!attr) {
+      OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_fwd_d128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem_bytes));
+      attr = true;
+    }
+    og_flash_attn_fwd_d128_kernel<<<(unsigned)grid, kFaThreads, smem_bytes, (cudaStream_t)stream>>>(mq, mk, mv, p);
+  }
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   return OG_OK;
@@ -430,7 +553,8 @@ extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, co
                                  const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq, int S,
                                  int C, int n_head, float scale, og_stream_t stream) {
   OG_REQUIRE(q && k && v && out && dout && lse && delta_ws && dq && dk && dv, "flash_attn_bwd: null pointer");
-  OG_REQUIRE(n_head >= 1 && C == n_head * kD, "flash_attn_bwd: needs d_head = 64 (C=%d, n_head=%d)", C, n_head);
+  const int dh = flash_d_head(C, n_head);
+  OG_REQUIRE(dh != 0, "flash_attn_bwd: needs d_head = 64 or 128 (C=%d, n_head=%d)", C, n_head);
   OG_REQUIRE(nseq > 0 && S > 0, "flash_attn_bwd: empty problem");
   OG_REQUIRE(scale > 0.f, "flash_attn_bwd: scale must be positive (as in the forward pass)");
   cudaStream_t s = (cudaStream_t)stream;
@@ -438,8 +562,12 @@ extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, co
   {
     long long blocks = (rows * n_head + 7) / 8;
     if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
-    og_attn_delta_kernel<<<(unsigned)blocks, 256, 0, s>>>((const __nv_bfloat16*)out, (const __nv_bfloat16*)dout,
-                                                         delta_ws, rows, S, C, n_head);
+    if (dh == 64)
+      og_attn_delta_kernel<<<(unsigned)blocks, 256, 0, s>>>((const __nv_bfloat16*)out, (const __nv_bfloat16*)dout,
+                                                           delta_ws, rows, S, C, n_head);
+    else
+      og_attn_delta_d128_kernel<<<(unsigned)blocks, 256, 0, s>>>(
+          (const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, delta_ws, rows, S, C, n_head);
     OG_CHECK_CUDA(cudaGetLastError());
     g_launches.fetch_add(1);
   }
@@ -456,20 +584,35 @@ extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, co
   if ((r = make_seq_map(&mk, k, nseq, S, C)) != OG_OK) return r;
   if ((r = make_seq_map(&mv, v, nseq, S, C)) != OG_OK) return r;
   if ((r = make_seq_map(&mdo, dout, nseq, S, C)) != OG_OK) return r;
-  const size_t smem_bytes = 6 * kTileBytes + 1024 + 64;
-  static bool attr = false;
-  if (!attr) {
-    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_bwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)smem_bytes));
-    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)smem_bytes));
-    attr = true;
-  }
   const long long grid = (long long)nseq * n_head * p.tiles;
   OG_REQUIRE(grid < (1LL << 31), "flash_attn_bwd: too many tiles");
-  og_flash_attn_bwd_kernel<0><<<(unsigned)grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
-  OG_CHECK_CUDA(cudaGetLastError());
-  og_flash_attn_bwd_kernel<1><<<(unsigned)grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
+  if (dh == 64) {
+    const size_t smem_bytes = 6 * kTileBytes + 1024 + 64;
+    static bool attr = false;
+    if (!attr) {
+      OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_bwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem_bytes));
+      OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem_bytes));
+      attr = true;
+    }
+    og_flash_attn_bwd_kernel<0><<<(unsigned)grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
+    OG_CHECK_CUDA(cudaGetLastError());
+    og_flash_attn_bwd_kernel<1><<<(unsigned)grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
+  } else {
+    const size_t smem_bytes = 12 * kTileBytes + 1024 + 64;   // 2 + 2 x 2 tiles of 16 KiB
+    static bool attr = false;
+    if (!attr) {
+      OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_bwd_d128_kernel<0>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+      OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_bwd_d128_kernel<1>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+      attr = true;
+    }
+    og_flash_attn_bwd_d128_kernel<0><<<(unsigned)grid, 2 * kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
+    OG_CHECK_CUDA(cudaGetLastError());
+    og_flash_attn_bwd_d128_kernel<1><<<(unsigned)grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
+  }
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(2);
   return OG_OK;

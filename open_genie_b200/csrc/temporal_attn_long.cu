@@ -1,5 +1,5 @@
-// temporal_attn_long.cu — temporal (causal, d_head = 64) attention for clips of any length: FlashAttention-2 on
-// mma.sync m16n8k16, tiled over queries and keys, online softmax in fp32.
+// temporal_attn_long.cu — temporal (causal, d_head = 64 or 128) attention for clips of any length: FlashAttention-2
+// on mma.sync m16n8k16, tiled over queries and keys, online softmax in fp32.
 //
 // STATUS: checked by tests/test_gpu_temporal_long.py (kernel level against float64 for T = 1 .. 1024, model level
 // against the CPU oracle); ops._TimeAttnFn uses it for T > 32, the kernels of temporal_attn_mma.cu / attention_rows.cu
@@ -28,6 +28,16 @@
 //                                         with atomics.
 // Both backward kernels recompute P = exp(scale * S - lse); dS = P (dP - delta). No atomics except the kv_bcast flush.
 // Outputs are staged in shared memory and stored as whole 128-byte row segments.
+//
+// Head width D (template argument, 64 or 128; ops._TimeAttnFn sends every T here at D = 128). Staged rows are 2D bytes
+// plus 16 of padding (144 / 272 B, both an odd number of 16-byte units, so ldmatrix stays conflict free); tiles are
+// 9 / 17 KiB, and shared memory at D = 128 is 85 KiB (forward), 119 KiB (dQ) and 103 KiB (dK / dV). The forward and dQ
+// kernels keep their shape, with D / 8 n-tiles of accumulators per lane. The dK / dV kernel cannot hold dK and dV for
+// 128 columns (16 rows x 128 columns x 2 = 128 accumulators per lane on top of S^T and dP^T): at D = 128 it runs 8
+// warps, warps w and w + 4 own the same 16 key rows, both compute the full S^T and dP^T over the 128 dims, and each
+// keeps dK / dV for one 64-column half, as at D = 64.
+// Registers (nvcc 12.9, -O3, sm_90a; no spills): D = 64: fwd 128, dQ 167, dK/dV 230; D = 128: fwd 167, dQ 245,
+// dK/dV 230 (256 threads).
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 #include "temporal_mma_frag.cuh"
@@ -36,8 +46,6 @@ namespace og {
 extern std::atomic<uint64_t> g_launches;
 
 namespace tlong {
-using tmma::kD;
-using tmma::kPitch;
 using tmma::load_a;
 using tmma::load_b_cols;
 using tmma::load_b_rows;
@@ -46,16 +54,23 @@ using tmma::pack_a;
 
 constexpr int kTile = 64;                      // rows per query / key tile (16 per warp)
 constexpr int kThreads = 128;
-constexpr int kTileBytes = kTile * kPitch;     // one staged 64 x 64 bf16 tile: 9216 B
 constexpr int kVecBytes = kTile * 4;           // 64 fp32 values (lse or delta of one query tile)
-constexpr int kFPitch = 288;                   // fp32 output staging: 256 data + 32 pad (float2 stores conflict free)
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 
-constexpr size_t kFwdSmem = 5 * (size_t)kTileBytes;                        // Q, 2 x (K, V)
-constexpr size_t kDqSmem = 7 * (size_t)kTileBytes;                         // Q, dO, O, 2 x (K, V)
-constexpr size_t kDkdvSmem = 6 * (size_t)kTileBytes + 4 * (size_t)kVecBytes;  // K, V, 2 x (Q, dO, lse, delta)
-static_assert(4 * 16 * kFPitch <= 2 * kTileBytes, "fp32 output staging must fit in one ring stage");
+// Shapes at head width D (64 or 128)
+template <int D>
+struct Geo {
+  static constexpr int kPitch = 2 * D + 16;            // staged bf16 row: 144 B at 64, 272 B at 128 (ldmatrix conflict free)
+  static constexpr int kTileBytes = kTile * kPitch;    // one staged 64 x D tile: 9216 B / 17408 B
+  static constexpr int kFPitch = 4 * D + 32;           // fp32 output staging row (float2 stores conflict free)
+  static constexpr int kNT = D / 8;                    // 8-column n-tiles of a full-width fragment
+  static constexpr int kDkdvThreads = D == 64 ? 128 : 256;   // dK / dV: one warp, or a warp pair, per 16 key rows
+  static constexpr size_t kFwdSmem = 5 * (size_t)kTileBytes;                           // Q, 2 x (K, V)
+  static constexpr size_t kDqSmem = 7 * (size_t)kTileBytes;                            // Q, dO, O, 2 x (K, V)
+  static constexpr size_t kDkdvSmem = 6 * (size_t)kTileBytes + 4 * (size_t)kVecBytes;  // K, V, 2 x (Q, dO, lse, delta)
+  static_assert(4 * 16 * kFPitch <= 2 * kTileBytes, "fp32 output staging must fit in one ring stage");
+};
 
 // 16- / 4-byte cp.async with zero fill: `valid` false reads nothing and writes zeros
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
@@ -67,14 +82,18 @@ __device__ __forceinline__ void cp_async4(uint32_t dst, const void* src, bool va
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-// rows t0 .. t0+63 of a sequence (row pitch `pitch` elements) into a staged tile; rows >= T are zero
+// rows t0 .. t0+63 of a sequence (row pitch `pitch` elements) into a staged tile; rows >= T are zero.
+// NTHR threads share the copy.
+template <int D, int NTHR = kThreads>
 __device__ __forceinline__ void load_tile(uint8_t* dst, const __nv_bfloat16* seq, long long pitch, int t0, int T,
                                           int tid) {
+  constexpr int kCh = D / 8;   // 16-byte chunks per row
 #pragma unroll
-  for (int i = 0; i < kTile * 8 / kThreads; ++i) {
-    const int idx = tid + kThreads * i, r = idx >> 3, ch = idx & 7;
+  for (int i = 0; i < kTile * kCh / NTHR; ++i) {
+    const int idx = tid + NTHR * i, r = idx / kCh, ch = idx % kCh;
     const bool ok = t0 + r < T;
-    cp_async16(smem_u32(dst + r * kPitch + ch * 16), seq + (ok ? (long long)(t0 + r) * pitch : 0) + ch * 8, ok);
+    cp_async16(smem_u32(dst + r * Geo<D>::kPitch + ch * 16), seq + (ok ? (long long)(t0 + r) * pitch : 0) + ch * 8,
+               ok);
   }
 }
 // fp32 values t0 .. t0+63 of one sequence's lse / delta row; entries >= T are zero
@@ -85,9 +104,11 @@ __device__ __forceinline__ void load_vec(uint8_t* dst, const float* row, int t0,
   }
 }
 
-// acc = A_w B^T over the 64 head dims: A = 16 staged rows of this warp, B = the 64 rows of a staged tile
+// acc = A_w B^T over the D head dims: A = 16 staged rows of this warp, B = the 64 rows of a staged tile
 // (S = Q K^T, dP = dO V^T, S^T = K Q^T, dP^T = V dO^T); fragment [kc][half][.] covers columns 16 kc + 8 half ..
+template <int D>
 __device__ __forceinline__ void gemm_nt(float (&acc)[4][2][4], const uint8_t* a_rows, const uint8_t* b_rows, int lane) {
+  constexpr int P = Geo<D>::kPitch;
 #pragma unroll
   for (int c = 0; c < 4; ++c)
 #pragma unroll
@@ -95,54 +116,62 @@ __device__ __forceinline__ void gemm_nt(float (&acc)[4][2][4], const uint8_t* a_
 #pragma unroll
       for (int e = 0; e < 4; ++e) acc[c][hf][e] = 0.f;
 #pragma unroll
-  for (int kk = 0; kk < 4; ++kk) {
+  for (int kk = 0; kk < D / 16; ++kk) {
     uint32_t a[4];
-    load_a(a, a_rows, kk * 16, lane);
+    load_a<P>(a, a_rows, kk * 16, lane);
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
       uint32_t b[2];
-      load_b_rows(b, b_rows, nt * 8, kk * 16, lane);
+      load_b_rows<P>(b, b_rows, nt * 8, kk * 16, lane);
       mma16816(acc[nt >> 1][nt & 1], a, b[0], b[1]);
     }
   }
 }
 
-// acc += X B: X = the 16 x 64 fragments `x` (rounded to bf16), B = a staged 64 x 64 tile whose rows are the k index
-// (P V, dS K, P^T dO, dS^T Q)
-__device__ __forceinline__ void gemm_nn_acc(float (&acc)[8][4], const float (&x)[4][2][4], const uint8_t* b_tile,
-                                            int lane) {
+// acc += X B: X = the 16 x 64 fragments `x` (rounded to bf16), B = columns n0 .. n0 + 8 NT - 1 of a staged 64-row
+// tile whose rows are the k index (P V, dS K, P^T dO, dS^T Q)
+template <int D, int NT>
+__device__ __forceinline__ void gemm_nn_acc(float (&acc)[NT][4], const float (&x)[4][2][4], const uint8_t* b_tile,
+                                            int n0, int lane) {
+  constexpr int P = Geo<D>::kPitch;
 #pragma unroll
   for (int kc = 0; kc < 4; ++kc) {
     uint32_t a[4];
     pack_a(a, x[kc]);
 #pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
+    for (int nt = 0; nt < NT; ++nt) {
       uint32_t b[2];
-      load_b_cols(b, b_tile + kc * 16 * kPitch, nt * 8, lane);
+      load_b_cols<P>(b, b_tile + kc * 16 * P, n0 + nt * 8, lane);
       mma16816(acc[nt], a, b[0], b[1]);
     }
   }
 }
 
-// 16 x 64 fp32 fragments (times sc0 / sc1 for rows g / g+8) as bf16 into a warp's 16 staged rows
-__device__ __forceinline__ void frags_to_rows(uint8_t* rows, const float (&o)[8][4], float sc0, float sc1, int lane) {
+// 16 x 8NT fp32 fragments (times sc0 / sc1 for rows g / g+8) as bf16 into columns n0 .. of a warp's 16 staged rows
+template <int D, int NT>
+__device__ __forceinline__ void frags_to_rows(uint8_t* rows, const float (&o)[NT][4], float sc0, float sc1, int n0,
+                                              int lane) {
+  constexpr int P = Geo<D>::kPitch;
   const int g = lane >> 2, q = lane & 3;
 #pragma unroll
-  for (int nt = 0; nt < 8; ++nt) {
-    *reinterpret_cast<uint32_t*>(rows + g * kPitch + (nt * 8 + q * 2) * 2) = pack_bf16x2(o[nt][0] * sc0, o[nt][1] * sc0);
-    *reinterpret_cast<uint32_t*>(rows + (g + 8) * kPitch + (nt * 8 + q * 2) * 2) =
+  for (int nt = 0; nt < NT; ++nt) {
+    *reinterpret_cast<uint32_t*>(rows + g * P + (n0 + nt * 8 + q * 2) * 2) = pack_bf16x2(o[nt][0] * sc0, o[nt][1] * sc0);
+    *reinterpret_cast<uint32_t*>(rows + (g + 8) * P + (n0 + nt * 8 + q * 2) * 2) =
         pack_bf16x2(o[nt][2] * sc1, o[nt][3] * sc1);
   }
 }
-// a warp's 16 staged bf16 rows (sequence rows t0 ..) to global memory, rows >= T dropped
+// 16-byte chunks ch0 .. ch0 + CH - 1 of a warp's 16 staged bf16 rows (sequence rows t0 ..) to global memory, rows >= T
+// dropped
+template <int D, int CH>
 __device__ __forceinline__ void rows_to_global(const uint8_t* rows, __nv_bfloat16* seq, long long pitch, int t0, int T,
-                                               int lane) {
+                                               int ch0, int lane) {
+  constexpr int kRows = 32 / CH;   // rows per pass
 #pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    const int r = (lane >> 3) + 4 * it, ch = lane & 7;
+  for (int it = 0; it < 16 / kRows; ++it) {
+    const int r = lane / CH + kRows * it, ch = ch0 + lane % CH;
     if (t0 + r >= T) continue;
     *(reinterpret_cast<uint4*>(seq + (long long)(t0 + r) * pitch) + ch) =
-        *reinterpret_cast<const uint4*>(rows + r * kPitch + ch * 16);
+        *reinterpret_cast<const uint4*>(rows + r * Geo<D>::kPitch + ch * 16);
   }
 }
 
@@ -151,43 +180,46 @@ struct Seq {
   int b, h;
 };
 // task = (b*nh + h)*P + p: the row of the lse / delta layout
-__device__ __forceinline__ Seq decode(long long task, int T, long long P, int C, int nh, int kv_bcast) {
+__device__ __forceinline__ Seq decode(long long task, int T, long long P, int C, int nh, int D, int kv_bcast) {
   Seq s;
   s.task = task;
   const long long p = task % P, bh = task / P;
   s.h = (int)(bh % nh);
   s.b = (int)(bh / nh);
-  s.q0 = ((long long)s.b * T * P + p) * C + (long long)s.h * kD;
-  s.k0 = kv_bcast ? (long long)s.b * T * C + (long long)s.h * kD : s.q0;
+  s.q0 = ((long long)s.b * T * P + p) * C + (long long)s.h * D;
+  s.k0 = kv_bcast ? (long long)s.b * T * C + (long long)s.h * D : s.q0;
   s.kpitch = kv_bcast ? (long long)C : P * C;
   return s;
 }
 
+template <int D>
 __global__ void __launch_bounds__(kThreads)
     og_temporal_attn_long_fwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                      const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ res,
                                      __nv_bfloat16* __restrict__ out, __nv_bfloat16* __restrict__ out_res,
                                      float* __restrict__ lse, int B, int T, long long P, int C, int nh, float scale,
                                      int kv_bcast, int tiles) {
+  using G = Geo<D>;
+  constexpr int kTileBytes = G::kTileBytes, kPitch = G::kPitch, kFPitch = G::kFPitch, kNT = G::kNT;
   extern __shared__ __align__(16) uint8_t smem_l[];
   uint8_t* qs = smem_l;
   uint8_t* ring = smem_l + kTileBytes;   // stage s: K at ring + 2 s kTileBytes, V right after
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
   const long long ntask = (long long)B * nh * P;
   const int i = tiles - 1 - (int)(blockIdx.x / ntask);   // the longest query tiles are scheduled first
-  const Seq sq = decode(blockIdx.x % ntask, T, P, C, nh, kv_bcast);
+  const Seq sq = decode(blockIdx.x % ntask, T, P, C, nh, D, kv_bcast);
   const long long qpitch = P * C;
-  load_tile(qs, q + sq.q0, qpitch, i * kTile, T, tid);
-  load_tile(ring, k + sq.k0, sq.kpitch, 0, T, tid);
-  load_tile(ring + kTileBytes, v + sq.k0, sq.kpitch, 0, T, tid);
+  load_tile<D>(qs, q + sq.q0, qpitch, i * kTile, T, tid);
+  load_tile<D>(ring, k + sq.k0, sq.kpitch, 0, T, tid);
+  load_tile<D>(ring + kTileBytes, v + sq.k0, sq.kpitch, 0, T, tid);
   cp_async_commit();
   const float cl2 = scale * kLog2e;
   const int row0 = i * kTile + warp * 16 + g;   // this lane's query rows: row0, row0 + 8
   const uint8_t* qw = qs + warp * 16 * kPitch;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-  float o[8][4];
+  float o[kNT][4];
 #pragma unroll
-  for (int nt = 0; nt < 8; ++nt)
+  for (int nt = 0; nt < kNT; ++nt)
 #pragma unroll
     for (int e = 0; e < 4; ++e) o[nt][e] = 0.f;
   for (int j = 0; j <= i; ++j) {
@@ -195,13 +227,13 @@ __global__ void __launch_bounds__(kThreads)
     __syncthreads();   // tile j has landed for every thread; every warp is done with tile j - 1
     if (j < i) {
       uint8_t* nx = ring + ((j + 1) & 1) * 2 * kTileBytes;
-      load_tile(nx, k + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
-      load_tile(nx + kTileBytes, v + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
+      load_tile<D>(nx, k + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
+      load_tile<D>(nx + kTileBytes, v + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
       cp_async_commit();
     }
     const uint8_t* ks = ring + (j & 1) * 2 * kTileBytes;
     float s[4][2][4];
-    gemm_nt(s, qw, ks, lane);
+    gemm_nt<D>(s, qw, ks, lane);
     // scores in the log2 domain; the diagonal tile masks keys after the query. Key 0 is in every row of tile 0, so
     // the row maximum is finite from the first tile on.
     float mx[2] = {m[0], m[1]};
@@ -232,9 +264,12 @@ __global__ void __launch_bounds__(kThreads)
         const float p = ex2_approx(s[nt >> 1][nt & 1][e] - m[rr]);
         s[nt >> 1][nt & 1][e] = p;
         l[rr] += p;
-        o[nt][e] *= alpha[rr];
       }
-    gemm_nn_acc(o, s, ks + kTileBytes, lane);
+#pragma unroll
+    for (int nt = 0; nt < kNT; ++nt)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[nt][e] *= alpha[e >> 1];
+    gemm_nn_acc<D, kNT>(o, s, ks + kTileBytes, 0, lane);
   }
 #pragma unroll
   for (int rr = 0; rr < 2; ++rr) {
@@ -246,16 +281,17 @@ __global__ void __launch_bounds__(kThreads)
   // finished by every warp before the last barrier); each warp writes and reads only its own 16 rows
   uint8_t* st = ring + ((i + 1) & 1) * 2 * kTileBytes + warp * 16 * kFPitch;
 #pragma unroll
-  for (int nt = 0; nt < 8; ++nt)
+  for (int nt = 0; nt < kNT; ++nt)
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr)
       *reinterpret_cast<float2*>(st + (g + 8 * rr) * kFPitch + (nt * 8 + 2 * qd) * 4) =
           make_float2(o[nt][2 * rr] * inv[rr], o[nt][2 * rr + 1] * inv[rr]);
   __syncwarp();
   const int t_w = i * kTile + warp * 16;
+  constexpr int kCh = D / 8, kRows = 32 / kCh;   // 8-column chunks per row, rows per pass
 #pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    const int r = (lane >> 3) + 4 * it, ch = lane & 7;
+  for (int it = 0; it < 16 / kRows; ++it) {
+    const int r = lane / kCh + kRows * it, ch = lane % kCh;
     if (t_w + r >= T) continue;
     const float4 a = *reinterpret_cast<const float4*>(st + r * kFPitch + ch * 32);
     const float4 c = *reinterpret_cast<const float4*>(st + r * kFPitch + ch * 32 + 16);
@@ -279,12 +315,15 @@ __global__ void __launch_bounds__(kThreads)
   }
 }
 
+template <int D>
 __global__ void __launch_bounds__(kThreads)
     og_temporal_attn_long_bwd_dq_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                         const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ o,
                                         const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse,
                                         float* __restrict__ delta, __nv_bfloat16* __restrict__ dq, int B, int T,
                                         long long P, int C, int nh, float scale, int kv_bcast, int tiles) {
+  using G = Geo<D>;
+  constexpr int kTileBytes = G::kTileBytes, kPitch = G::kPitch, kNT = G::kNT;
   extern __shared__ __align__(16) uint8_t smem_l[];
   uint8_t* qs = smem_l;
   uint8_t* dos = qs + kTileBytes;
@@ -293,13 +332,13 @@ __global__ void __launch_bounds__(kThreads)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
   const long long ntask = (long long)B * nh * P;
   const int i = tiles - 1 - (int)(blockIdx.x / ntask);
-  const Seq sq = decode(blockIdx.x % ntask, T, P, C, nh, kv_bcast);
+  const Seq sq = decode(blockIdx.x % ntask, T, P, C, nh, D, kv_bcast);
   const long long qpitch = P * C;
-  load_tile(qs, q + sq.q0, qpitch, i * kTile, T, tid);
-  load_tile(dos, dout + sq.q0, qpitch, i * kTile, T, tid);
-  load_tile(os, o + sq.q0, qpitch, i * kTile, T, tid);
-  load_tile(ring, k + sq.k0, sq.kpitch, 0, T, tid);
-  load_tile(ring + kTileBytes, v + sq.k0, sq.kpitch, 0, T, tid);
+  load_tile<D>(qs, q + sq.q0, qpitch, i * kTile, T, tid);
+  load_tile<D>(dos, dout + sq.q0, qpitch, i * kTile, T, tid);
+  load_tile<D>(os, o + sq.q0, qpitch, i * kTile, T, tid);
+  load_tile<D>(ring, k + sq.k0, sq.kpitch, 0, T, tid);
+  load_tile<D>(ring + kTileBytes, v + sq.k0, sq.kpitch, 0, T, tid);
   cp_async_commit();
   const int t_w = i * kTile + warp * 16, row0 = t_w + g;
   const uint8_t* qw = qs + warp * 16 * kPitch;
@@ -310,15 +349,15 @@ __global__ void __launch_bounds__(kThreads)
   for (int rr = 0; rr < 2; ++rr) lse2[rr] = row0 + 8 * rr < T ? lse[sq.task * T + row0 + 8 * rr] * kLog2e : 0.f;
   cp_async_wait_all();
   __syncthreads();   // the rows of every tile are loaded by all four warps
-  // delta = rowsum(dO * O) of this warp's rows: two lanes per row, 32 columns each
+  // delta = rowsum(dO * O) of this warp's rows: two lanes per row, D / 2 columns each
   float dsum;
   {
-    const int r = lane >> 1, c0 = (lane & 1) * 32;
+    const int r = lane >> 1, c0 = (lane & 1) * (D / 2);
     const uint8_t* dr = dow + r * kPitch + c0 * 2;
     const uint8_t* orow = os + (warp * 16 + r) * kPitch + c0 * 2;
     dsum = 0.f;
 #pragma unroll
-    for (int c = 0; c < 32; c += 2) {
+    for (int c = 0; c < D / 2; c += 2) {
       const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(dr + c * 2));
       const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(orow + c * 2));
       dsum = fmaf(a.x, b.x, dsum);
@@ -329,9 +368,9 @@ __global__ void __launch_bounds__(kThreads)
   }
   const float dl[2] = {__shfl_sync(0xffffffffu, dsum, 2 * g), __shfl_sync(0xffffffffu, dsum, 2 * g + 16)};
   const float cl2 = scale * kLog2e;
-  float acc[8][4];
+  float acc[kNT][4];
 #pragma unroll
-  for (int nt = 0; nt < 8; ++nt)
+  for (int nt = 0; nt < kNT; ++nt)
 #pragma unroll
     for (int e = 0; e < 4; ++e) acc[nt][e] = 0.f;
   for (int j = 0; j <= i; ++j) {
@@ -339,15 +378,15 @@ __global__ void __launch_bounds__(kThreads)
     __syncthreads();
     if (j < i) {
       uint8_t* nx = ring + ((j + 1) & 1) * 2 * kTileBytes;
-      load_tile(nx, k + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
-      load_tile(nx + kTileBytes, v + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
+      load_tile<D>(nx, k + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
+      load_tile<D>(nx + kTileBytes, v + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
       cp_async_commit();
     }
     const uint8_t* ks = ring + (j & 1) * 2 * kTileBytes;
     const uint8_t* vs = ks + kTileBytes;
     float s[4][2][4], dp[4][2][4];
-    gemm_nt(s, qw, ks, lane);
-    gemm_nt(dp, dow, vs, lane);
+    gemm_nt<D>(s, qw, ks, lane);
+    gemm_nt<D>(dp, dow, vs, lane);
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
@@ -357,17 +396,22 @@ __global__ void __launch_bounds__(kThreads)
         if (j == i && col > row0 + 8 * rr) p = 0.f;
         s[nt >> 1][nt & 1][e] = p * (dp[nt >> 1][nt & 1][e] - dl[rr]);   // dS (without the scale)
       }
-    gemm_nn_acc(acc, s, ks, lane);
+    gemm_nn_acc<D, kNT>(acc, s, ks, 0, lane);
   }
   // dQ = scale * sum_j dS K_j; every read of this warp's Q rows is done, so they stage the output
   __syncwarp();
   uint8_t* qw_out = qs + warp * 16 * kPitch;
-  frags_to_rows(qw_out, acc, scale, scale, lane);
+  frags_to_rows<D, kNT>(qw_out, acc, scale, scale, 0, lane);
   __syncwarp();
-  rows_to_global(qw_out, dq + sq.q0, qpitch, t_w, T, lane);
+  rows_to_global<D, D / 8>(qw_out, dq + sq.q0, qpitch, t_w, T, 0, lane);
 }
 
-__global__ void __launch_bounds__(kThreads)
+// D = 64: warp w owns key rows 16 w .. 16 w + 15 and all 64 head columns of dK / dV.
+// D = 128: eight warps; warps w and w + 4 own the same 16 key rows, each computes the full S^T and dP^T (over all 128
+// dims) and keeps dK / dV for head columns [64 (w / 4), 64 (w / 4) + 64) only, so a lane holds 2 x 32 accumulators
+// as at D = 64.
+template <int D>
+__global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
     og_temporal_attn_long_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                           const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ dout,
                                           const float* __restrict__ lse, const float* __restrict__ delta,
@@ -375,38 +419,42 @@ __global__ void __launch_bounds__(kThreads)
                                           float* __restrict__ dk_b, float* __restrict__ dv_b, int B, int T,
                                           long long P, int C, int nh, float scale, int kv_bcast, int tiles,
                                           long long chunk, long long nchunk) {
+  using G = Geo<D>;
+  constexpr int kTileBytes = G::kTileBytes, kPitch = G::kPitch, NTHR = G::kDkdvThreads;
   extern __shared__ __align__(16) uint8_t smem_l[];
   uint8_t* ks = smem_l;
   uint8_t* vs = ks + kTileBytes;
   uint8_t* ring = vs + kTileBytes;   // stage s: Q, dO, lse[64], delta[64]
   constexpr int kStage = 2 * kTileBytes + 2 * kVecBytes;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
+  const int wr = warp & 3, half = warp >> 2;   // key-row group; head-column half (0 at D = 64)
+  const int n0 = half * 64;
   const long long per_j = (long long)B * nh * nchunk;
   const int j = (int)(blockIdx.x / per_j);   // key tile; the longest (j = 0) are scheduled first
   const long long rest = blockIdx.x % per_j, bh = rest / nchunk;
   const long long p0 = (rest % nchunk) * chunk, p1 = p0 + chunk < P ? p0 + chunk : P;
   const int nq = tiles - j;                  // query tiles i = j .. tiles - 1 per pixel
   const long long items = (p1 - p0) * nq;
-  const Seq s0 = decode(bh * P + p0, T, P, C, nh, kv_bcast);
+  const Seq s0 = decode(bh * P + p0, T, P, C, nh, D, kv_bcast);
   const long long qpitch = P * C;
   auto load_item = [&](long long n, int stage) {
     const long long task = bh * P + p0 + n / nq;
     const int i = j + (int)(n % nq);
     const long long q0 = s0.q0 + (task - s0.task) * C;   // the pixels of one (b, h) are C elements apart
     uint8_t* st = ring + stage * kStage;
-    load_tile(st, q + q0, qpitch, i * kTile, T, tid);
-    load_tile(st + kTileBytes, dout + q0, qpitch, i * kTile, T, tid);
+    load_tile<D, NTHR>(st, q + q0, qpitch, i * kTile, T, tid);
+    load_tile<D, NTHR>(st + kTileBytes, dout + q0, qpitch, i * kTile, T, tid);
     load_vec(st + 2 * kTileBytes, lse + task * T, i * kTile, T, tid);
     load_vec(st + 2 * kTileBytes + kVecBytes, delta + task * T, i * kTile, T, tid);
   };
-  load_tile(ks, k + s0.k0, s0.kpitch, j * kTile, T, tid);
-  load_tile(vs, v + s0.k0, s0.kpitch, j * kTile, T, tid);
+  load_tile<D, NTHR>(ks, k + s0.k0, s0.kpitch, j * kTile, T, tid);
+  load_tile<D, NTHR>(vs, v + s0.k0, s0.kpitch, j * kTile, T, tid);
   load_item(0, 0);
   cp_async_commit();
   const float cl2 = scale * kLog2e;
-  const int key0 = j * kTile + warp * 16 + g;   // this lane's key rows: key0, key0 + 8
-  const uint8_t* kw = ks + warp * 16 * kPitch;
-  const uint8_t* vw = vs + warp * 16 * kPitch;
+  const int key0 = j * kTile + wr * 16 + g;   // this lane's key rows: key0, key0 + 8
+  const uint8_t* kw = ks + wr * 16 * kPitch;
+  const uint8_t* vw = vs + wr * 16 * kPitch;
   float dka[8][4], dva[8][4];
 #pragma unroll
   for (int nt = 0; nt < 8; ++nt)
@@ -427,8 +475,8 @@ __global__ void __launch_bounds__(kThreads)
     const int i = j + (int)(n % nq);
     // transposed products: rows = this warp's keys, columns = the 64 queries of tile i
     float s[4][2][4], dp[4][2][4];
-    gemm_nt(s, kw, qsn, lane);
-    gemm_nt(dp, vw, dosn, lane);
+    gemm_nt<D>(s, kw, qsn, lane);
+    gemm_nt<D>(dp, vw, dosn, lane);
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
       const int c = nt * 8 + 2 * qd;
@@ -443,20 +491,21 @@ __global__ void __launch_bounds__(kThreads)
         dp[nt >> 1][nt & 1][e] = p * (dp[nt >> 1][nt & 1][e] - (ce ? dl.y : dl.x));
       }
     }
-    gemm_nn_acc(dva, s, dosn, lane);    // dV += P^T dO
-    gemm_nn_acc(dka, dp, qsn, lane);    // dK += dS^T Q
+    gemm_nn_acc<D, 8>(dva, s, dosn, n0, lane);    // dV += P^T dO
+    gemm_nn_acc<D, 8>(dka, dp, qsn, n0, lane);    // dK += dS^T Q
   }
-  const int t_w = j * kTile + warp * 16;
+  const int t_w = j * kTile + wr * 16;
   if (!kv_bcast) {
-    // every read of this warp's K / V rows is done: they stage the outputs
+    // every read of this warp's K / V rows is done (at D = 128 also by the partner warp, which reads all columns):
+    // they stage the outputs
+    if (D == 64) __syncwarp(); else __syncthreads();
+    uint8_t* kw_out = ks + wr * 16 * kPitch;
+    uint8_t* vw_out = vs + wr * 16 * kPitch;
+    frags_to_rows<D, 8>(kw_out, dka, scale, scale, n0, lane);
+    frags_to_rows<D, 8>(vw_out, dva, 1.f, 1.f, n0, lane);
     __syncwarp();
-    uint8_t* kw_out = ks + warp * 16 * kPitch;
-    uint8_t* vw_out = vs + warp * 16 * kPitch;
-    frags_to_rows(kw_out, dka, scale, scale, lane);
-    frags_to_rows(vw_out, dva, 1.f, 1.f, lane);
-    __syncwarp();
-    rows_to_global(kw_out, dk + s0.q0, qpitch, t_w, T, lane);
-    rows_to_global(vw_out, dv + s0.q0, qpitch, t_w, T, lane);
+    rows_to_global<D, 8>(kw_out, dk + s0.q0, qpitch, t_w, T, half * 8, lane);
+    rows_to_global<D, 8>(vw_out, dv + s0.q0, qpitch, t_w, T, half * 8, lane);
   } else {
     // this chunk's sum over its pixels into the caller's fp32 [B][T][C] (unordered across chunks)
 #pragma unroll
@@ -465,7 +514,7 @@ __global__ void __launch_bounds__(kThreads)
       for (int e = 0; e < 4; ++e) {
         const int t = key0 + 8 * (e >> 1);
         if (t >= T) continue;
-        const long long off = ((long long)s0.b * T + t) * C + (long long)s0.h * kD + nt * 8 + 2 * qd + (e & 1);
+        const long long off = ((long long)s0.b * T + t) * C + (long long)s0.h * D + n0 + nt * 8 + 2 * qd + (e & 1);
         atomicAdd(dk_b + off, dka[nt][e] * scale);
         atomicAdd(dv_b + off, dva[nt][e]);
       }
@@ -480,66 +529,41 @@ using namespace og;
 
 static bool long_aligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-extern "C" int og_temporal_attn_long_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
-                                         void* out_res, float* lse, int B, int T, int64_t P, int C, int n_head,
-                                         float scale, int kv_bcast, og_stream_t stream) {
+namespace {
+template <int D>
+int long_fwd(const void* q, const void* k, const void* v, void* out, const void* residual, void* out_res, float* lse,
+             int B, int T, int64_t P, int C, int n_head, float scale, int kv_bcast, int tiles, long long grid,
+             cudaStream_t stream) {
   using namespace og::tlong;
-  OG_REQUIRE(q && k && v && out && lse, "temporal_attn_long_fwd: null pointer");
-  OG_REQUIRE(!residual == !out_res, "temporal_attn_long_fwd: residual and out_res must be given together");
-  OG_REQUIRE(B >= 1 && T >= 1 && P >= 1, "temporal_attn_long_fwd: empty problem (B=%d, T=%d, P=%lld)", B, T,
-             (long long)P);
-  OG_REQUIRE(n_head >= 1 && C % n_head == 0, "temporal_attn_long_fwd: C=%d not divisible by n_head=%d", C, n_head);
-  OG_REQUIRE(scale > 0.f, "temporal_attn_long_fwd: scale must be positive");
-  if (C / n_head != kD) {
-    set_error("temporal_attn_long_fwd: d_head=%d not supported (64)", C / n_head);
-    return OG_ERR_UNSUPPORTED_SHAPE;
+  static bool attr = false;
+  if (!attr) {   // above the 48 KiB default at D = 128
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_fwd_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)Geo<D>::kFwdSmem));
+    attr = true;
   }
-  OG_REQUIRE(long_aligned(q) && long_aligned(k) && long_aligned(v) && long_aligned(out) && long_aligned(residual) &&
-                 long_aligned(out_res),
-             "temporal_attn_long_fwd: q, k, v, out, residual and out_res must be 16-byte aligned");
-  const int tiles = (T + kTile - 1) / kTile;
-  const long long grid = (long long)B * n_head * P * tiles;
-  OG_REQUIRE(grid < (1LL << 31), "temporal_attn_long_fwd: too many tiles");
-  og_temporal_attn_long_fwd_kernel<<<(unsigned)grid, kThreads, kFwdSmem, (cudaStream_t)stream>>>(
+  og_temporal_attn_long_fwd_kernel<D><<<(unsigned)grid, kThreads, Geo<D>::kFwdSmem, stream>>>(
       (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)residual,
       (__nv_bfloat16*)out, (__nv_bfloat16*)out_res, lse, B, T, P, C, n_head, scale, kv_bcast, tiles);
   OG_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1);
   return OG_OK;
 }
 
-extern "C" int og_temporal_attn_long_bwd(const void* q, const void* k, const void* v, const void* out,
-                                         const void* dout, const float* lse, float* delta_ws, void* dq, void* dk,
-                                         void* dv, float* dk_bcast, float* dv_bcast, int B, int T, int64_t P, int C,
-                                         int n_head, float scale, int kv_bcast, og_stream_t stream) {
+template <int D>
+int long_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout, const float* lse,
+             float* delta_ws, void* dq, void* dk, void* dv, float* dk_bcast, float* dv_bcast, int B, int T, int64_t P,
+             int C, int n_head, float scale, int kv_bcast, int tiles, cudaStream_t s) {
   using namespace og::tlong;
-  OG_REQUIRE(q && k && v && out && dout && lse && delta_ws && dq, "temporal_attn_long_bwd: null pointer");
-  OG_REQUIRE(kv_bcast ? (dk_bcast && dv_bcast) : (dk && dv), "temporal_attn_long_bwd: missing dk/dv buffers");
-  OG_REQUIRE(B >= 1 && T >= 1 && P >= 1, "temporal_attn_long_bwd: empty problem (B=%d, T=%d, P=%lld)", B, T,
-             (long long)P);
-  OG_REQUIRE(n_head >= 1 && C % n_head == 0, "temporal_attn_long_bwd: C=%d not divisible by n_head=%d", C, n_head);
-  OG_REQUIRE(scale > 0.f, "temporal_attn_long_bwd: scale must be positive");
-  if (C / n_head != kD) {
-    set_error("temporal_attn_long_bwd: d_head=%d not supported (64)", C / n_head);
-    return OG_ERR_UNSUPPORTED_SHAPE;
-  }
-  OG_REQUIRE(long_aligned(q) && long_aligned(k) && long_aligned(v) && long_aligned(out) && long_aligned(dout) &&
-                 long_aligned(dq) && (kv_bcast || (long_aligned(dk) && long_aligned(dv))),
-             "temporal_attn_long_bwd: q, k, v, out, dout, dq, dk and dv must be 16-byte aligned");
-  const int tiles = (T + kTile - 1) / kTile;
   const long long ntask = (long long)B * n_head * P;
-  OG_REQUIRE(ntask * tiles < (1LL << 31), "temporal_attn_long_bwd: too many tiles");
-  cudaStream_t s = (cudaStream_t)stream;
   static bool attr = false;
   if (!attr) {
-    OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_bwd_dq_kernel,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDqSmem));
-    OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_bwd_dkdv_kernel,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDkdvSmem));
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_bwd_dq_kernel<D>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Geo<D>::kDqSmem));
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_bwd_dkdv_kernel<D>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Geo<D>::kDkdvSmem));
     attr = true;
   }
   // dQ first: it also writes delta, which the dK / dV kernel reads
-  og_temporal_attn_long_bwd_dq_kernel<<<(unsigned)(ntask * tiles), kThreads, kDqSmem, s>>>(
+  og_temporal_attn_long_bwd_dq_kernel<D><<<(unsigned)(ntask * tiles), kThreads, Geo<D>::kDqSmem, s>>>(
       (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)out,
       (const __nv_bfloat16*)dout, lse, delta_ws, (__nv_bfloat16*)dq, B, T, P, C, n_head, scale, kv_bcast, tiles);
   OG_CHECK_CUDA(cudaGetLastError());
@@ -556,11 +580,70 @@ extern "C" int og_temporal_attn_long_bwd(const void* q, const void* k, const voi
     nchunk = (P + chunk - 1) / chunk;
   }
   const long long grid = (long long)B * n_head * nchunk * tiles;
-  og_temporal_attn_long_bwd_dkdv_kernel<<<(unsigned)grid, kThreads, kDkdvSmem, s>>>(
+  og_temporal_attn_long_bwd_dkdv_kernel<D><<<(unsigned)grid, Geo<D>::kDkdvThreads, Geo<D>::kDkdvSmem, s>>>(
       (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)dout, lse,
       delta_ws, (__nv_bfloat16*)dk, (__nv_bfloat16*)dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale, kv_bcast, tiles,
       chunk, nchunk);
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   return OG_OK;
+}
+}  // namespace
+
+extern "C" int og_temporal_attn_long_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
+                                         void* out_res, float* lse, int B, int T, int64_t P, int C, int n_head,
+                                         float scale, int kv_bcast, og_stream_t stream) {
+  using namespace og::tlong;
+  OG_REQUIRE(q && k && v && out && lse, "temporal_attn_long_fwd: null pointer");
+  OG_REQUIRE(!residual == !out_res, "temporal_attn_long_fwd: residual and out_res must be given together");
+  OG_REQUIRE(B >= 1 && T >= 1 && P >= 1, "temporal_attn_long_fwd: empty problem (B=%d, T=%d, P=%lld)", B, T,
+             (long long)P);
+  OG_REQUIRE(n_head >= 1 && C % n_head == 0, "temporal_attn_long_fwd: C=%d not divisible by n_head=%d", C, n_head);
+  OG_REQUIRE(scale > 0.f, "temporal_attn_long_fwd: scale must be positive");
+  const int dh = C / n_head;
+  if (dh != 64 && dh != 128) {
+    set_error("temporal_attn_long_fwd: d_head=%d not supported (64 or 128)", dh);
+    return OG_ERR_UNSUPPORTED_SHAPE;
+  }
+  OG_REQUIRE(long_aligned(q) && long_aligned(k) && long_aligned(v) && long_aligned(out) && long_aligned(residual) &&
+                 long_aligned(out_res),
+             "temporal_attn_long_fwd: q, k, v, out, residual and out_res must be 16-byte aligned");
+  const int tiles = (T + kTile - 1) / kTile;
+  const long long grid = (long long)B * n_head * P * tiles;
+  OG_REQUIRE(grid < (1LL << 31), "temporal_attn_long_fwd: too many tiles");
+  const int r = dh == 64 ? long_fwd<64>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
+                                        tiles, grid, (cudaStream_t)stream)
+                         : long_fwd<128>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
+                                         tiles, grid, (cudaStream_t)stream);
+  if (r != OG_OK) return r;
+  g_launches.fetch_add(1);
+  return OG_OK;
+}
+
+extern "C" int og_temporal_attn_long_bwd(const void* q, const void* k, const void* v, const void* out,
+                                         const void* dout, const float* lse, float* delta_ws, void* dq, void* dk,
+                                         void* dv, float* dk_bcast, float* dv_bcast, int B, int T, int64_t P, int C,
+                                         int n_head, float scale, int kv_bcast, og_stream_t stream) {
+  using namespace og::tlong;
+  OG_REQUIRE(q && k && v && out && dout && lse && delta_ws && dq, "temporal_attn_long_bwd: null pointer");
+  OG_REQUIRE(kv_bcast ? (dk_bcast && dv_bcast) : (dk && dv), "temporal_attn_long_bwd: missing dk/dv buffers");
+  OG_REQUIRE(B >= 1 && T >= 1 && P >= 1, "temporal_attn_long_bwd: empty problem (B=%d, T=%d, P=%lld)", B, T,
+             (long long)P);
+  OG_REQUIRE(n_head >= 1 && C % n_head == 0, "temporal_attn_long_bwd: C=%d not divisible by n_head=%d", C, n_head);
+  OG_REQUIRE(scale > 0.f, "temporal_attn_long_bwd: scale must be positive");
+  const int dh = C / n_head;
+  if (dh != 64 && dh != 128) {
+    set_error("temporal_attn_long_bwd: d_head=%d not supported (64 or 128)", dh);
+    return OG_ERR_UNSUPPORTED_SHAPE;
+  }
+  OG_REQUIRE(long_aligned(q) && long_aligned(k) && long_aligned(v) && long_aligned(out) && long_aligned(dout) &&
+                 long_aligned(dq) && (kv_bcast || (long_aligned(dk) && long_aligned(dv))),
+             "temporal_attn_long_bwd: q, k, v, out, dout, dq, dk and dv must be 16-byte aligned");
+  const int tiles = (T + kTile - 1) / kTile;
+  const long long ntask = (long long)B * n_head * P;
+  OG_REQUIRE(ntask * tiles < (1LL << 31), "temporal_attn_long_bwd: too many tiles");
+  return dh == 64 ? long_bwd<64>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C,
+                                 n_head, scale, kv_bcast, tiles, (cudaStream_t)stream)
+                  : long_bwd<128>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C,
+                                  n_head, scale, kv_bcast, tiles, (cudaStream_t)stream);
 }

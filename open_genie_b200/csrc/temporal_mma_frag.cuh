@@ -2,7 +2,8 @@
 // (temporal_attn_mma.cu for T <= 16, temporal_attn_long.cu for longer clips).
 //
 // Staged matrices are rows of 64 bf16 in shared memory with a 144-byte pitch (128 data + 16 pad), which makes every
-// ldmatrix below bank-conflict free. Fragment conventions (PTX ISA, mma.m16n8k16 .row.col, bf16):
+// ldmatrix below bank-conflict free. The loaders take the pitch as a template argument (default 144) so the tiled
+// kernels can stage 128-wide rows at 272 bytes (256 data + 16 pad, 17 x 16 B: conflict free as well). Fragment conventions (PTX ISA, mma.m16n8k16 .row.col, bf16):
 //   A (16x16): a0a1 = (g, 2q..), a2a3 = (g+8, 2q..), a4a5 = (g, 8+2q..), a6a7 = (g+8, 8+2q..)   g = lane/4, q = lane%4
 //   B (16x8) : b0b1 = (k = 2q.., n = g), b2b3 = (k = 8+2q.., n = g)
 //   C (16x8) : c0c1 = (g, 2q..), c2c3 = (g+8, 2q..)
@@ -40,16 +41,19 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], 
 }
 
 // A fragment (16 x 16 slice starting at column `col0`) of a staged row-major matrix
+template <int Pitch = kPitch>
 __device__ __forceinline__ void load_a(uint32_t (&a)[4], const uint8_t* m, int col0, int lane) {
-  ldsm_x4(a, smem_u32(m + (lane & 15) * kPitch + (col0 + (lane >> 4) * 8) * 2));
+  ldsm_x4(a, smem_u32(m + (lane & 15) * Pitch + (col0 + (lane >> 4) * 8) * 2));
 }
 // B fragment for  B[k][n] = M[n0 + n][k0 + k]  (rows of the staged matrix are the n index: Q K^T, dO V^T)
+template <int Pitch = kPitch>
 __device__ __forceinline__ void load_b_rows(uint32_t (&b)[2], const uint8_t* m, int n0, int k0, int lane) {
-  ldsm_x2(b, smem_u32(m + (n0 + (lane & 7)) * kPitch + (k0 + ((lane >> 3) & 1) * 8) * 2));
+  ldsm_x2(b, smem_u32(m + (n0 + (lane & 7)) * Pitch + (k0 + ((lane >> 3) & 1) * 8) * 2));
 }
 // B fragment for  B[k][n] = M[k][n0 + n]  (rows of the staged matrix are the k index: P V, dS K, P^T dO, dS^T Q)
+template <int Pitch = kPitch>
 __device__ __forceinline__ void load_b_cols(uint32_t (&b)[2], const uint8_t* m, int n0, int lane) {
-  ldsm_x2_trans(b, smem_u32(m + (lane & 15) * kPitch + n0 * 2));
+  ldsm_x2_trans(b, smem_u32(m + (lane & 15) * Pitch + n0 * 2));
 }
 
 // the C fragments of a 16 x 16 product (two n-tiles) as the bf16 A fragment of the next product

@@ -5,6 +5,9 @@ conv3d_*.cu).
 Only the HEAD-valid configuration is implemented (SURVEY.md §7 H6/H8): d_inp == d_out == n_head*d_head, so
 to_q / to_k / to_v / to_out are Identity, q = k = v = LayerNorm(RoPE(x)); the one live conditioning path is
 the temporal one (latent action -> K, V through `time_attn_kw={'key_dim': k}`). Anything else raises.
+Head widths: d_head = 64 or 128 (flash attention and the temporal kernels have both; temporal attention at 128 runs the
+tiled kernels at every clip length). Space and time attention may use different widths when n_head * d_head matches,
+e.g. SpaceTimeAttention(n_head=(2, 1), d_head=(64, 128)); the FFN GroupNorm takes the temporal head count.
 state_dict keys: {space,temp}_attn.norm.{weight,bias}, {space,temp}_attn.embed.freq,
 temp_attn.to_qkv.to_{k,v}.weight (with key_dim), ffn.1.net.0.{weight,bias}, ffn.1.net.1.0.weight.
 """
@@ -78,9 +81,8 @@ class Attention(nn.Module):
             raise NotImplementedError('attention dropout is not used by any shipped blueprint')
         if not embed:
             raise NotImplementedError('embed=False is not used by any shipped blueprint')
-        if d_head != 64:
-            raise NotImplementedError('the flash attention kernels are specialised for d_head = 64 '
-                                      '(every shipped blueprint uses 64)')
+        if d_head not in (64, 128):
+            raise NotImplementedError(f'the attention kernels take d_head = 64 or 128, not {d_head}')
         self.norm = nn.LayerNorm(hid)
         self.embed = RotaryEmbedding(self.d_inp, kind=self.rope_kind)
         self.to_qkv = Adapter(qry_dim=self.d_inp, n_head=n_head, d_head=d_head, bias=bias, **kwargs)

@@ -964,6 +964,13 @@ class _SpaceAttnFn(torch.autograd.Function):
 _TIME_ATTN_SHORT_T = 32
 
 
+def _time_attn_tiled(T: int, C: int, n_head: int) -> bool:
+    """Whether temporal attention runs on the tiled kernels (og_temporal_attn_long_fwd / bwd): clips longer than
+    _TIME_ATTN_SHORT_T, and every clip at d_head = 128, which the per-pixel kernels do not take (a lane would hold
+    2 x 128 fp32 values)."""
+    return T > _TIME_ATTN_SHORT_T or C == 128 * n_head
+
+
 class _TimeAttnFn(torch.autograd.Function):
     """y = SDPA_causal(q, k, v; scale) + x over t for every pixel; q = LayerNorm(RoPE1d(x)); k = v = q, or the
     projected latent-action conditioning (B, T, C) shared by all pixels (attention.py:347-371, 471)."""
@@ -986,11 +993,11 @@ class _TimeAttnFn(torch.autograd.Function):
         else:
             kc = vc = q
         o = lse = None
-        if T <= _TIME_ATTN_SHORT_T:
+        if not _time_attn_tiled(T, C, n_head):
             _lib.call('og_temporal_attn_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), x.data_ptr(), y.data_ptr(),
                       B, T, P, C, n_head, scale, int(bcast), s)
         else:
-            # longer clips: the tiled kernels, which keep the attention output and log-sum-exp for the backward pass
+            # the tiled kernels, which keep the attention output and log-sum-exp for the backward pass
             o = torch.empty_like(x)
             lse = torch.empty((B, n_head, P, T), dtype=f32, device=x.device)
             _lib.call('og_temporal_attn_long_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), o.data_ptr(),
