@@ -204,6 +204,15 @@ int og_gn_act_bwd(const void* dy, const void* x, const float* A, const float* B,
                   float* dx_colsum, int N, int64_t V, int C, void* workspace, size_t workspace_bytes,
                   og_stream_t stream);
 
+/* GELU of the SpaceTimeAttention feed-forward block's hidden layers: the nn.GELU() that ForwardBlock puts after every
+ * hidden convolution (genie/module/misc.py:92-98, built by genie/module/attention.py:429-438 with hid_dim), exact erf
+ * form, in fp32: a = u Phi(u), Phi(u) = erfc(-u/sqrt 2)/2. u, a: bf16 rows [rows][C]. C % 8 == 0, rows >= 1, pointers
+ * 16-byte aligned; otherwise -1. */
+int og_gelu_fwd(const void* u, void* a, int64_t rows, int C, og_stream_t stream);
+/* Its backward (autograd of the same nn.GELU during loss.backward()): du = da * (Phi(u) + u phi(u)),
+ * phi(u) = exp(-u^2/2)/sqrt(2 pi), in fp32. da, u, du: bf16 [rows][C]; same requirements as og_gelu_fwd. */
+int og_gelu_bwd(const void* da, const void* u, void* du, int64_t rows, int C, og_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * layout / data movement
  * ---------------------------------------------------------------------------------------------- */

@@ -264,6 +264,42 @@ __global__ void __launch_bounds__(256) og_affine_act_fwd_kernel(const uint4* __r
 }
 
 // ------------------------------------------------------------------------------------------------
+// GELU (nn.GELU(), exact erf form) of the SpaceTimeAttention FFN's hidden layers: a = GELU(u), du = da * GELU'(u).
+// Flat grid-stride over 8-element vectors. Phi(u) is taken as erfc(-u/sqrt 2)/2, which keeps its relative accuracy in
+// the negative tail: u * Phi(u) stays exact to a few fp32 ulps until it underflows (to -0 below u ~ -14).
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float gelu_cdf(float u) { return 0.5f * erfcf(-0.70710678118654752f * u); }
+
+__global__ void __launch_bounds__(256) og_gelu_fwd_kernel(const uint4* __restrict__ u, uint4* __restrict__ a,
+                                                          long long nvec) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < nvec;
+       i += (long long)gridDim.x * blockDim.x) {
+    float f[8];
+    unpack8(__ldg(u + i), f);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) f[k] = f[k] * gelu_cdf(f[k]);
+    a[i] = pack8(f);
+  }
+}
+
+// GELU'(u) = Phi(u) + u phi(u), phi(u) = exp(-u^2/2) / sqrt(2 pi)
+__global__ void __launch_bounds__(256) og_gelu_bwd_kernel(const uint4* __restrict__ da, const uint4* __restrict__ u,
+                                                          uint4* __restrict__ du, long long nvec) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < nvec;
+       i += (long long)gridDim.x * blockDim.x) {
+    float g[8], f[8];
+    unpack8(__ldg(da + i), g);
+    unpack8(__ldg(u + i), f);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const float pdf = 0.39894228040143268f * expf(-0.5f * f[k] * f[k]);
+      g[k] *= fmaf(f[k], pdf, gelu_cdf(f[k]));
+    }
+    du[i] = pack8(g);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // backward reduce: S[n][c] = (sum_v dpre, sum_v dpre * x), dpre = dy * act'(x*A+B)
 // grid (chunks, N), block 256; same thread mapping as the stats kernel.
 // ------------------------------------------------------------------------------------------------
@@ -971,6 +1007,34 @@ extern "C" int og_gn_act_bwd(const void* dy, const void* x, const float* A, cons
   if (partials) rc = sum_partials(partials, 1, (int)(grid.x * grid.y), C, C, C, dx_colsum, (cudaStream_t)stream);
   if (rc != OG_OK) return rc;
   if (S) return launch_param_grads(S, mean_rstd, cond_scale, N, C, G, dgamma, dbeta, (cudaStream_t)stream);
+  return OG_OK;
+}
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+extern "C" int og_gelu_fwd(const void* u, void* a, int64_t rows, int C, og_stream_t stream) {
+  OG_REQUIRE(u && a, "gelu_fwd: null pointer");
+  OG_REQUIRE(C > 0 && C % 8 == 0, "gelu_fwd: C=%d must be a positive multiple of 8", C);
+  OG_REQUIRE(rows > 0, "gelu_fwd: empty problem (rows=%lld)", (long long)rows);
+  OG_REQUIRE(aligned16(u) && aligned16(a), "gelu_fwd: u and a must be 16-byte aligned");
+  const long long nvec = rows * (C / 8);
+  og_gelu_fwd_kernel<<<ew_grid(nvec, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const uint4*>(u),
+                                                                          reinterpret_cast<uint4*>(a), nvec);
+  OG_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1);
+  return OG_OK;
+}
+
+extern "C" int og_gelu_bwd(const void* da, const void* u, void* du, int64_t rows, int C, og_stream_t stream) {
+  OG_REQUIRE(da && u && du, "gelu_bwd: null pointer");
+  OG_REQUIRE(C > 0 && C % 8 == 0, "gelu_bwd: C=%d must be a positive multiple of 8", C);
+  OG_REQUIRE(rows > 0, "gelu_bwd: empty problem (rows=%lld)", (long long)rows);
+  OG_REQUIRE(aligned16(da) && aligned16(u) && aligned16(du), "gelu_bwd: da, u and du must be 16-byte aligned");
+  const long long nvec = rows * (C / 8);
+  og_gelu_bwd_kernel<<<ew_grid(nvec, 256), 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const uint4*>(da), reinterpret_cast<const uint4*>(u), reinterpret_cast<uint4*>(du), nvec);
+  OG_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1);
   return OG_OK;
 }
 

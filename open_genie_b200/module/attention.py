@@ -2,14 +2,18 @@
 genie/module/attention.py, executed by the fused CUDA kernels (csrc/attention_rows.cu, flash_attn.cu,
 conv3d_*.cu).
 
-Only the HEAD-valid configuration is implemented (SURVEY.md §7 H6/H8): d_inp == d_out == n_head*d_head, so
-to_q / to_k / to_v / to_out are Identity, q = k = v = LayerNorm(RoPE(x)); the one live conditioning path is
-the temporal one (latent action -> K, V through `time_attn_kw={'key_dim': k}`). Anything else raises.
+Attention runs in the HEAD-valid configuration (SURVEY.md §7 H6/H8): d_inp == n_head*d_head, so to_q / to_k / to_v /
+to_out are Identity, q = k = v = LayerNorm(RoPE(x)); the one live conditioning path is the temporal one (latent action
+-> K, V through `time_attn_kw={'key_dim': k}`). Anything else raises.
 Head widths: d_head = 64 or 128 (flash attention and the temporal kernels have both; temporal attention at 128 runs the
 tiled kernels at every clip length). Space and time attention may use different widths when n_head * d_head matches,
 e.g. SpaceTimeAttention(n_head=(2, 1), d_head=(64, 128)); the FFN GroupNorm takes the temporal head count.
+The FFN is the reference's ForwardBlock: GroupNorm -> conv (-> GELU -> conv)* with `hid_dim` hidden widths, ending at
+`d_out` channels (with transpose=True, where the skip becomes the 1x1x1 ffn_skip conv); `bias` gives every FFN conv a
+bias. Hidden widths and d_out are multiples of 64.
 state_dict keys: {space,temp}_attn.norm.{weight,bias}, {space,temp}_attn.embed.freq,
-temp_attn.to_qkv.to_{k,v}.weight (with key_dim), ffn.1.net.0.{weight,bias}, ffn.1.net.1.0.weight.
+temp_attn.to_qkv.to_{k,v}.{weight[,bias]} (with key_dim), ffn.1.net.0.{weight,bias}, ffn.1.net.{i}.0.{weight[,bias]}
+(i = 1 .. len(hid_dim) + 1), ffn_skip.{weight,bias} (d_out != n_head*d_head).
 """
 from __future__ import annotations
 
@@ -22,7 +26,7 @@ from torch import Tensor
 
 from .. import ops
 from ..utils import default, exists
-from .video import Conv3dParams
+from .video import Conv3dParams, _Slot
 
 
 class RotaryEmbedding(nn.Module):
@@ -142,16 +146,20 @@ class TemporalAttention(Attention):
 
 
 class _FfnNet(nn.Module):
-    """Mirror of ForwardBlock(in_dim, block=nn.Conv3d, hid_dim=None) -> net = Sequential(GroupNorm,
-    Sequential(Conv3d, Identity)) (genie/module/misc.py:71-104) for state_dict keys net.0.*, net.1.0.weight."""
+    """Mirror of ForwardBlock(in_dim, out_dim, hid_dim, block=nn.Conv3d, num_groups, bias, kernel_size, padding)
+    (genie/module/misc.py:71-104): net = Sequential(GroupNorm, Sequential(Conv3d, GELU), ..., Sequential(Conv3d,
+    Identity)) for state_dict keys net.0.*, net.{i}.0.{weight[,bias]}. The GELU slots hold no parameters: ops.ffn_res
+    applies GELU with og_gelu_fwd / og_gelu_bwd."""
 
-    def __init__(self, dim: int, num_groups: int, kernel_size: int, bias: bool) -> None:
+    def __init__(self, dim: int, out_dim: int, hid_dim: Tuple[int, ...], num_groups: int, kernel_size: int,
+                 bias: bool) -> None:
         super().__init__()
-        if bias:
-            raise NotImplementedError('SpaceTimeAttention(bias=True) is not used by any shipped blueprint')
+        dims = (dim,) + hid_dim + (out_dim,)
         self.net = nn.Sequential(
             nn.GroupNorm(num_groups, dim),
-            nn.Sequential(Conv3dParams(dim, dim, kernel_size, causal=False, bias=False), nn.Identity()),
+            *[nn.Sequential(Conv3dParams(ci, co, kernel_size, causal=False, bias=bias),
+                            _Slot() if i < len(dims) - 2 else nn.Identity())
+              for i, (ci, co) in enumerate(zip(dims[:-1], dims[1:]))],
         )
 
 
@@ -168,22 +176,43 @@ class SpaceTimeAttention(nn.Module):
             d_head = (d_head, d_head)
         if isinstance(embed, bool):
             embed = (embed, embed)
-        if exists(hid_dim) or exists(d_inp) or exists(d_out):
-            raise NotImplementedError('d_inp / d_out / hid_dim variants do not run at the reference HEAD')
         if n_head[0] * d_head[0] != n_head[1] * d_head[1]:
             raise NotImplementedError('space and time widths must match')
+        dim = n_head[1] * d_head[1]
+        if exists(d_inp) and d_inp != dim:
+            raise NotImplementedError('SpaceTimeAttention(d_inp != n_head*d_head) fails in the reference too: its '
+                                      'spatial LayerNorm is built for n_head*d_head channels (attention.py:179,220)')
+        d_out = default(d_out, dim)
+        if d_out != dim and not transpose:
+            raise NotImplementedError('SpaceTimeAttention(d_out != n_head*d_head) needs transpose=True: with '
+                                      'transpose=False the reference applies its 1x1x1 ffn_skip conv to the '
+                                      'channels-last tensor (attention.py:472) and fails')
+        hid_dim = (hid_dim,) if isinstance(hid_dim, int) else tuple(default(hid_dim, ()))
+        if any(w <= 0 or w % 64 for w in hid_dim + (d_out,)):
+            raise NotImplementedError(f'SpaceTimeAttention: hid_dim {hid_dim} and d_out {d_out} must be positive '
+                                      f'multiples of 64 (the channel blocks of the convolution GEMMs)')
         self.space_attn = SpatialAttention(n_head=n_head[0], d_head=d_head[0], bias=bias, scale=scale, embed=embed[0],
                                            causal=False, dropout=dropout, transpose=transpose, **space_attn_kw)
         self.temp_attn = TemporalAttention(n_head=n_head[1], d_head=d_head[1], bias=bias, scale=scale, embed=embed[1],
                                            causal=True, dropout=dropout, transpose=transpose, **time_attn_kw)
-        dim = n_head[1] * d_head[1]
         # nn.Sequential(Rearrange, ForwardBlock, Rearrange): ForwardBlock sits at index 1 -> keys 'ffn.1.net...'
-        self.ffn = nn.Sequential(nn.Identity(), _FfnNet(dim, n_head[1], kernel_size, bias), nn.Identity())
-        self.in_channels = self.out_channels = dim
+        self.ffn = nn.Sequential(nn.Identity(), _FfnNet(dim, d_out, hid_dim, n_head[1], kernel_size, bias),
+                                 nn.Identity())
+        self.in_channels, self.out_channels = dim, d_out
         self.transpose = transpose
         self.time_skip = nn.Identity()
         self.space_skip = nn.Identity()
-        self.ffn_skip = nn.Identity()
+        # nn.Conv3d(dim, d_out, 1) (bias on) in the reference; runs as extra K columns of the last FFN conv
+        self.ffn_skip = Conv3dParams(dim, d_out, 1, causal=False) if d_out != dim else nn.Identity()
+        self._fuse_skip()
+
+    def _fuse_skip(self):
+        if isinstance(self.ffn_skip, Conv3dParams):
+            self.ffn[1].net[-1][0].fuse_shortcut(self.ffn_skip)
+
+    def __setstate__(self, state):
+        super().__setstate__(state)
+        self._fuse_skip()     # re-link inside the copy (see Conv3dParams.__setstate__)
 
     def forward(self, video: Tensor, cond=None, mask: Tensor | None = None) -> Tensor:
         if not isinstance(cond, tuple):
@@ -199,6 +228,7 @@ class SpaceTimeAttention(nn.Module):
         tc = time_cond if isinstance(self.temp_attn.to_qkv.to_k, nn.Linear) else None
         x = self.temp_attn(x, cond=tc, transpose=False, _residual=True)
         gn = self.ffn[1].net[0]
-        conv = self.ffn[1].net[1][0]
-        x = ops.ffn_res(x, gn.weight, gn.bias, conv.weight, conv.packed(), conv.geom, gn.num_groups, gn.eps)
+        convs = [(c.weight, c.bias, c.packed(), c.geom) for c in (layer[0] for layer in self.ffn[1].net[1:])]
+        skip = self.ffn_skip if isinstance(self.ffn_skip, Conv3dParams) else None
+        x = ops.ffn_res(x, gn.weight, gn.bias, convs, gn.num_groups, gn.eps, *((skip.weight, skip.bias) if skip else ()))
         return x.permute(0, 4, 1, 2, 3) if self.transpose else x

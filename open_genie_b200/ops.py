@@ -1048,11 +1048,14 @@ class _TimeAttnFn(torch.autograd.Function):
 
 
 class _FfnFn(torch.autograd.Function):
-    """y = Conv3d_k3(GroupNorm_G(x)) + x  — the ST block's "FFN" and its skip (attention.py:429-444, 472;
-    misc.py:92-98). The skip is added inside the conv epilogue, its gradient inside the GN backward pass."""
+    """out = FFN(x) + skip(x) — the ST block's ForwardBlock and its skip (attention.py:429-454, 472; misc.py:71-104):
+        h = GroupNorm_G(x);  h = GELU(conv_i(h)) for every hidden layer;  y = conv_last(h)
+    skip(x) = x (added inside the last conv's epilogue, its gradient inside the GN backward pass) or, when the block
+    changes the width, the 1x1x1 ffn_skip conv as the second K segment of the last conv (x1 of og_conv3d_fwd).
+    Inputs after `skip_b`: (weight, bias or None, packed operand) per conv, in order; `geoms` holds their ConvGeoms."""
 
     @staticmethod
-    def forward(ctx, x, gn_w, gn_b, conv_w, packed, geom: ConvGeom, G: int, eps: float):
+    def forward(ctx, x, gn_w, gn_b, geoms, G: int, eps: float, skip_w, skip_b, *convs):
         _require_cuda(x, 'ffn input')
         x = _rows_bf16(x)
         B, T, H, W, C = x.shape
@@ -1067,45 +1070,106 @@ class _FfnFn(torch.autograd.Function):
         hn = torch.empty_like(x)
         _lib.call('og_gn_act_fwd', x.data_ptr(), sums.data_ptr(), gn_w.data_ptr(), gn_b.data_ptr(), None, None, eps, G, 0,
                   hn.data_ptr(), A.data_ptr(), Bc.data_ptr(), mr.data_ptr(), B, V, C, s)
-        y = torch.empty_like(x)
-        ws = _workspace(dev, B * V * C * 4)
-        _conv_call('fwd', 2.0 * B * V * C * geom.k_main, 'og_conv3d_fwd', hn.data_ptr(), C, geom.kt, geom.kh, geom.kw,
-                   geom.pt, geom.ph, geom.pw, None, 0, packed.data_ptr(), packed.shape[1], None, None, x.data_ptr(),
-                   y.data_ptr(), 0, B, T, H, W, C, ws.data_ptr(), ws.numel(), None, s)
-        ctx.cfg = (geom, G)
-        ctx.save_for_backward(x, hn, A, Bc, mr, gn_w, gn_b, packed)
+        ws = _workspace(dev, B * V * max(C, *(g.cout for g in geoms)) * 4)
+        h, pre = hn, []                   # pre: the bf16 pre-activations u of the hidden layers (GELU backward)
+        for i, geom in enumerate(geoms[:-1]):
+            _, bias, packed = convs[3 * i:3 * i + 3]
+            u = torch.empty((B, T, H, W, geom.cout), dtype=bf16, device=dev)
+            _conv_call('fwd', 2.0 * B * V * geom.cout * geom.k_main, 'og_conv3d_fwd', h.data_ptr(), geom.cin, geom.kt,
+                       geom.kh, geom.kw, geom.pt, geom.ph, geom.pw, None, 0, packed.data_ptr(), packed.shape[1],
+                       _ptr(bias), None, None, u.data_ptr(), 0, B, T, H, W, geom.cout, ws.data_ptr(), ws.numel(), None, s)
+            h = torch.empty_like(u)
+            _lib.call('og_gelu_fwd', u.data_ptr(), h.data_ptr(), B * V, geom.cout, s)
+            pre.append(u)
+            pre.append(h)
+        geom = geoms[-1]
+        _, bias, packed = convs[-3:]
+        y = torch.empty((B, T, H, W, geom.cout), dtype=bf16, device=dev)
+        c1 = C if skip_w is not None else 0
+        _conv_call('fwd', 2.0 * B * V * geom.cout * (geom.k_main + c1), 'og_conv3d_fwd', h.data_ptr(), geom.cin, geom.kt,
+                   geom.kh, geom.kw, geom.pt, geom.ph, geom.pw, x.data_ptr() if c1 else None, c1, packed.data_ptr(),
+                   packed.shape[1], _ptr(bias), _ptr(skip_b), None if c1 else x.data_ptr(), y.data_ptr(), 0, B, T, H, W,
+                   geom.cout, ws.data_ptr(), ws.numel(), None, s)
+        ctx.cfg = (geoms, G, tuple(convs[3 * i + 1] is not None for i in range(len(geoms))), skip_w is not None)
+        ctx.save_for_backward(x, hn, A, Bc, mr, gn_w, gn_b, *convs[2::3], *pre)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, hn, A, Bc, mr, gn_w, gn_b, packed = ctx.saved_tensors
-        geom, G = ctx.cfg
+        geoms, G, has_bias, has_skip = ctx.cfg
+        n = len(geoms)
+        x, hn, A, Bc, mr, gn_w, gn_b, *rest = ctx.saved_tensors
+        packs, pre = rest[:n], rest[n:]
         B, T, H, W, C = x.shape
         V = T * H * W
         s = _stream()
         dev = x.device
         dy = _rows_bf16(dy)
-        ws = _workspace(dev, B * V * C * 4)
+        ws = _workspace(dev, B * V * max(C, *(g.cout for g in geoms)) * 4)
         dh = torch.empty_like(x)
         S = _zeros((B, C, 2), f32, dev)
-        # data gradient, then the GroupNorm backward reduction over it
-        _conv_call('dgrad', 2.0 * B * V * C * geom.k_main, 'og_conv3d_dgrad', dy.data_ptr(), C, C, packed.data_ptr(),
-                   packed.shape[1], 0, geom.kt, geom.kh, geom.kw, geom.pt, geom.ph, geom.pw, dh.data_ptr(), 0, B, T, H,
-                   W, C, ws.data_ptr(), ws.numel(), s)
-        _lib.call('og_affine_act_bwd_reduce', dh.data_ptr(), x.data_ptr(), A.data_ptr(), Bc.data_ptr(), 0, S.data_ptr(),
-                  B, V, C, *_scratch(dh), s)
-        g = _zeros((C, geom.ntaps * C), f32, dev)
-        _conv_call('wgrad', 2.0 * B * V * C * geom.k_main, 'og_conv3d_wgrad', dy.data_ptr(), C, hn.data_ptr(), C,
-                   g.data_ptr(), g.shape[1], geom.kt, geom.kh, geom.kw, geom.pt, geom.ph, geom.pw, B, T, H, W,
-                   *_scratch(dy), s)
-        dw = g.view(C, geom.kt, geom.kh, geom.kw, C).permute(0, 4, 1, 2, 3)
+        grads = [None] * (3 * n)
+        # per conv, last to first: data gradient -> GELU backward of the layer below it (or, below the first conv, the
+        # GroupNorm backward reduction) -> weight (+ bias) gradient
+        d_out = dy
+        for i in reversed(range(n)):
+            geom, packed = geoms[i], packs[i]
+            cin, cout = geom.cin, geom.cout
+            d_in = dh if i == 0 else torch.empty((B, T, H, W, cin), dtype=bf16, device=dev)
+            _conv_call('dgrad', 2.0 * B * V * cout * geom.k_main, 'og_conv3d_dgrad', d_out.data_ptr(), cout, cout,
+                       packed.data_ptr(), packed.shape[1], 0, geom.kt, geom.kh, geom.kw, geom.pt, geom.ph, geom.pw,
+                       d_in.data_ptr(), 0, B, T, H, W, cin, ws.data_ptr(), ws.numel(), s)
+            if i == 0:
+                _lib.call('og_affine_act_bwd_reduce', dh.data_ptr(), x.data_ptr(), A.data_ptr(), Bc.data_ptr(), 0,
+                          S.data_ptr(), B, V, C, *_scratch(dh), s)
+                inp = hn
+            else:
+                u, inp = pre[2 * i - 2], pre[2 * i - 1]
+                d_u = torch.empty_like(u)
+                _lib.call('og_gelu_bwd', d_in.data_ptr(), u.data_ptr(), d_u.data_ptr(), B * V, cin, s)
+            g = _zeros((cout, geom.ntaps * cin), f32, dev)
+            fl = 2.0 * B * V * cout * geom.k_main
+            if has_bias[i]:
+                db = _zeros(cout, f32, dev)
+                _conv_call('wgrad', fl, 'og_conv3d_wgrad_bias', d_out.data_ptr(), cout, inp.data_ptr(), cin, g.data_ptr(),
+                           g.shape[1], geom.kt, geom.kh, geom.kw, geom.pt, geom.ph, geom.pw, B, T, H, W, db.data_ptr(),
+                           cout, *_scratch(d_out), s)
+                grads[3 * i + 1] = db
+            else:
+                _conv_call('wgrad', fl, 'og_conv3d_wgrad', d_out.data_ptr(), cout, inp.data_ptr(), cin, g.data_ptr(),
+                           g.shape[1], geom.kt, geom.kh, geom.kw, geom.pt, geom.ph, geom.pw, B, T, H, W,
+                           *_scratch(d_out), s)
+            grads[3 * i] = g.view(cout, geom.kt, geom.kh, geom.kw, cin).permute(0, 4, 1, 2, 3)
+            if i > 0:
+                d_out = d_u
+        add = dy
+        dskip_w = dskip_b = None
+        if has_skip:
+            # the 1x1x1 shortcut: its data gradient is the `add` of the GN backward pass; its weight gradient reads x;
+            # its bias gradient is the column sum of dy, as is that of the last conv's bias
+            geom, packed = geoms[-1], packs[-1]
+            cout = geom.cout
+            add = torch.empty_like(x)
+            _conv_call('dgrad', 2.0 * B * V * cout * C, 'og_conv3d_dgrad', dy.data_ptr(), cout, cout, packed.data_ptr(),
+                       packed.shape[1], geom.kpad, 1, 1, 1, 0, 0, 0, add.data_ptr(), 0, B, T, H, W, C, ws.data_ptr(),
+                       ws.numel(), s)
+            g = _zeros((cout, C), f32, dev)
+            if has_bias[-1]:
+                dskip_b = grads[-2].clone()
+                _conv_call('wgrad', 2.0 * B * V * cout * C, 'og_conv3d_wgrad', dy.data_ptr(), cout, x.data_ptr(), C,
+                           g.data_ptr(), C, 1, 1, 1, 0, 0, 0, B, T, H, W, *_scratch(dy), s)
+            else:
+                dskip_b = _zeros(cout, f32, dev)
+                _conv_call('wgrad', 2.0 * B * V * cout * C, 'og_conv3d_wgrad_bias', dy.data_ptr(), cout, x.data_ptr(), C,
+                           g.data_ptr(), C, 1, 1, 1, 0, 0, 0, B, T, H, W, dskip_b.data_ptr(), cout, *_scratch(dy), s)
+            dskip_w = g.view(cout, 1, 1, 1, C).permute(0, 4, 1, 2, 3)
         dgw = _zeros(C, f32, dev)
         dgb = _zeros(C, f32, dev)
         dx = torch.empty_like(x)
         _lib.call('og_gn_act_bwd', dh.data_ptr(), x.data_ptr(), A.data_ptr(), Bc.data_ptr(), S.data_ptr(), mr.data_ptr(),
-                  gn_w.data_ptr(), gn_b.data_ptr(), None, G, 0, dy.data_ptr(), dx.data_ptr(), dgw.data_ptr(),
+                  gn_w.data_ptr(), gn_b.data_ptr(), None, G, 0, add.data_ptr(), dx.data_ptr(), dgw.data_ptr(),
                   dgb.data_ptr(), None, None, None, B, V, C, *_scratch(dy), s)
-        return dx, dgw, dgb, dw, None, None, None, None
+        return (dx, dgw, dgb, None, None, None, dskip_w, dskip_b, *grads)
 
 
 def space_attention_res(x, freq, gamma, beta, n_head, scale, eps=1e-5):
@@ -1116,8 +1180,13 @@ def time_attention_res(x, freq, gamma, beta, n_head, scale, k_cond=None, v_cond=
     return _TimeAttnFn.apply(x, freq, gamma, beta, k_cond, v_cond, n_head, float(scale), float(eps))
 
 
-def ffn_res(x, gn_w, gn_b, conv_w, packed, geom, num_groups, eps=1e-5):
-    return _FfnFn.apply(x, gn_w, gn_b, conv_w, packed, geom, num_groups, float(eps))
+def ffn_res(x, gn_w, gn_b, convs, num_groups, eps=1e-5, skip_w=None, skip_b=None):
+    """convs: (weight, bias or None, packed operand, ConvGeom) per conv of the FFN, first to last, a GELU after every
+    conv but the last. skip_w / skip_b: the 1x1x1 ffn_skip conv, already fused into the last conv's packed operand
+    (Conv3dParams.fuse_shortcut); without it the skip is x itself."""
+    geoms = tuple(c[3] for c in convs)
+    return _FfnFn.apply(x, gn_w, gn_b, geoms, num_groups, float(eps), skip_w, skip_b,
+                        *(t for w, b, p, _ in convs for t in (w, b, p)))
 
 
 # ------------------------------------------------------------------------------------------------
