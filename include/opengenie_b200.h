@@ -321,8 +321,8 @@ int og_rope_ln_bwd(const void* x, const float* freq, const float* gamma, float e
                    int64_t pos_div, int pos_mod, const float* cos_sin, og_stream_t stream);
 
 /* Spatial attention: F.scaled_dot_product_attention(q,k,v, scale) non-causal (attention.py:229-234) on
- * wgmma tensor cores. q,k,v,out: [nseq][S][C], C = n_head*64 or n_head*128 (d_head 64 or 128; any other width returns
- * -1). lse: fp32 [nseq][n_head][S] (saved for backward).
+ * wgmma tensor cores. q,k,v,out: [nseq][S][C], C = n_head*64, n_head*128 or n_head*16 (d_head 64, 128 or 16; any
+ * other width returns -1). lse: fp32 [nseq][n_head][S] (saved for backward).
  * residual / out_res (optional, bf16 like out): out_res = out + residual, i.e. `attn(x) + skip(x)`
  * (attention.py:470-471), added in fp32; `out` itself is still written (the backward pass needs it). */
 int og_flash_attn_fwd(const void* q, const void* k, const void* v, void* out, const void* residual, void* out_res,
@@ -333,8 +333,8 @@ int og_flash_attn_bwd(const void* q, const void* k, const void* v, const void* o
                       int n_head, float scale, og_stream_t stream);
 
 /* Temporal attention, is_causal=True (attention.py:347-371, 423): one sequence per (batch, pixel), T <= 32
- * (longer clips, and d_head = 128 at any T: og_temporal_attn_long_fwd / bwd below). d_head 32 or 64; other widths
- * return -2.
+ * (longer clips, and d_head = 16 or 128 at any T: og_temporal_attn_long_fwd / bwd below). d_head 32 or 64; other
+ * widths return -2.
  * q/out rows ((b*T + t)*P + p); k,v either the same layout (kv_bcast=0) or [B][T][C] shared by all pixels
  * (kv_bcast=1: latent-action conditioning through to_k/to_v, attention.py:127-129,362-363). */
 int og_temporal_attn_fwd(const void* q, const void* k, const void* v, const void* residual, void* out, int B, int T,
@@ -345,7 +345,7 @@ int og_temporal_attn_bwd(const void* q, const void* k, const void* v, const void
                          int kv_bcast, og_stream_t stream);
 
 /* Temporal attention for clips of any length (T >= 1; the modules call it for T > 32 at d_head = 64 and for every T
- * at d_head = 128), d_head = 64 or 128 (C = n_head*64 or n_head*128; other widths return -2): the same
+ * at d_head = 16 and 128), d_head = 16, 64 or 128 (C = n_head * d_head; other widths return -2): the same
  * causal attention and layouts as og_temporal_attn_fwd / bwd, FlashAttention-2 style on mma.sync tensor cores (64-row
  * query and key tiles, online softmax), with the forward / backward contract of og_flash_attn_fwd / bwd.
  * out: bf16 like q (always written: the backward pass needs it). residual / out_res (optional, both or neither):

@@ -3,7 +3,7 @@
 // Reference: F.scaled_dot_product_attention(q, k, v, scale = n_head * d_head**-0.5) reached from
 // SpatialAttention.forward -> Attention.forward (genie/module/attention.py:279-307, 199-239), with
 // q = k = v = LayerNorm(RoPE(x)) in the HEAD-valid configuration. Layout: [nseq][S][C] bf16 rows
-// (one sequence = the H*W tokens of one frame, contiguous in NDHWC), head h = columns [h*d, h*d+d), d = 64 or 128.
+// (one sequence = the H*W tokens of one frame, contiguous in NDHWC), head h = columns [h*d, h*d+d), d = 16, 64 or 128.
 //
 // Every kernel is one warpgroup (128 threads) owning a 64-row tile; thread 0 streams the other operand's 64-row tiles
 // through a two-stage TMA ring (rows beyond S are zero-filled by TMA and masked). Accumulators live in registers in the
@@ -34,8 +34,16 @@
 //           dims: the score GEMMs run twice), warpgroup w keeps dV and dK for head columns [64w, 64w + 64), so a
 //           thread holds 2 x 32 accumulators as at d = 64. smem 2 + 2 x 2 tiles = 96 KiB.
 //   MODE 1: one warpgroup, dQ as two m64n64 fragments.
+//
+// d_head = 16 (og_flash_attn_fwd_d16_kernel, og_flash_attn_bwd_d16_kernel<MODE>, og_attn_delta_d16_kernel): the same
+// bodies at kDh = 16. A 64 x 16 tile is one 32-byte-wide TMA box with the 32-byte swizzle (2 KiB), read through
+// gmma_desc_sw32: K-major for the score GEMMs (one k16 slice, 8-row groups 256 B apart), MN-major for the products
+// with a register A operand, which issue m64n16k16 (wgmma_rs_n16; 8-row k groups 256 B apart, 512 B per k16 slice).
+// The score tile is still m64n64, so the softmax is that of d = 64; O, dV, dK and dQ are one m64n16 fragment
+// (8 registers). smem: forward 11 KiB, backward 13 KiB. The exponentials, not the MMAs, bound these kernels (one ex2
+// per 64 MMA FLOP forward).
 // Registers (nvcc 12.9, -O3, sm_90a; no spills): d = 64: fwd 98, MODE 0 168, MODE 1 122; d = 128: fwd 130,
-// MODE 0 175 (256 threads), MODE 1 154.
+// MODE 0 175 (256 threads), MODE 1 154; d = 16: fwd 66, MODE 0 128, MODE 1 98, delta 32.
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 
@@ -79,27 +87,50 @@ __device__ __forceinline__ void frag_to_a(const float (&x)[32], uint32_t (&a)[4]
   }
 }
 
-// D = X Y^T over the 64 kH head dims: both tiles K-major, kH half-tiles [64 rows][64 d] with the 128-byte swizzle,
-// kTileBytes apart (k16 slices 4c .. 4c + 3 come from half c)
-template <int kH>
+// Geometry at head width kDh. d = 64, 128: kH 64-column halves with the 128-byte swizzle, outputs as kH m64n64
+// fragments. d = 16: one 64 x 16 tile with the 32-byte swizzle (2 KiB), outputs as one m64n16 fragment.
+template <int kDh>
+struct FaGeo {
+  static constexpr int kH = kDh >= kD ? kDh / kD : 1;   // accumulator fragments per output
+  static constexpr int kN = kDh >= kD ? kD : kDh;       // fragment width (N of the MN-major products)
+  static constexpr int kR = kN / 2;                     // fp32 registers per fragment and thread
+  static constexpr int kTB = kTile * kDh * 2;           // one 64-row tile
+};
+
+// D = X Y^T over the kDh head dims, both tiles K-major. d = 64, 128: kH half-tiles [64 rows][64 d] with the 128-byte
+// swizzle, kTileBytes apart (k16 slices 4c .. 4c + 3 come from half c). d = 16: one k16 slice of 32-byte rows.
+template <int kDh>
 __device__ __forceinline__ void gemm_rows(float (&d)[32], uint32_t x_addr, uint32_t y_addr) {
+  if constexpr (kDh == 16) {
+    wgmma_ss<64, 0, 0>(d, gmma_desc_sw32(x_addr, 16, 256), gmma_desc_sw32(y_addr, 16, 256), 0);
+  } else {
+    constexpr int kH = kDh / kD;
 #pragma unroll
-  for (int c = 0; c < kH; ++c)
+    for (int c = 0; c < kH; ++c)
 #pragma unroll
-    for (int k = 0; k < kD / 16; ++k)
-      wgmma_ss<64, 0, 0>(d, gmma_desc_sw128(x_addr + c * kTileBytes + k * 32, 16, 1024),
-                         gmma_desc_sw128(y_addr + c * kTileBytes + k * 32, 16, 1024), c > 0 || k > 0);
+      for (int k = 0; k < kD / 16; ++k)
+        wgmma_ss<64, 0, 0>(d, gmma_desc_sw128(x_addr + c * kTileBytes + k * 32, 16, 1024),
+                           gmma_desc_sw128(y_addr + c * kTileBytes + k * 32, 16, 1024), c > 0 || k > 0);
+  }
 }
 
-// D += A Y: A from registers (64 rows x 64 k), Y a [64 k rows][64 d] half-tile read MN-major
-__device__ __forceinline__ void gemm_acc(float (&d)[32], const uint32_t (&a)[4][4], uint32_t y_addr) {
+// D += A Y: A from registers (64 rows x 64 k), Y a [64 k rows][kN d] tile read MN-major: a 64-wide half-tile with the
+// 128-byte swizzle (m64n64k16), or a 16-wide tile with the 32-byte swizzle (m64n16k16, 512 B per k16 slice)
+template <int kN>
+__device__ __forceinline__ void gemm_acc(float (&d)[kN / 2], const uint32_t (&a)[4][4], uint32_t y_addr) {
 #pragma unroll
-  for (int kk = 0; kk < 4; ++kk) wgmma_rs_n64<1>(d, a[kk], gmma_desc_sw128(y_addr + kk * 2048, 8192, 1024), 1);
+  for (int kk = 0; kk < 4; ++kk) {
+    if constexpr (kN == 16)
+      wgmma_rs_n16<1>(d, a[kk], gmma_desc_sw32(y_addr + kk * 512, 2048, 256), 1);
+    else
+      wgmma_rs_n64<1>(d, a[kk], gmma_desc_sw128(y_addr + kk * 2048, 8192, 1024), 1);
+  }
 }
 
-// 64 x 64 fragment (times `sc`) -> bf16 rows of [nseq][S][C] (rows >= S dropped)
-__device__ __forceinline__ void store_frag(const float (&d)[32], float sc, __nv_bfloat16* base, long long row0, int S,
-                                           int row_in_seq0, int C) {
+// 64 x kN fragment (times `sc`) -> bf16 rows of [nseq][S][C] (rows >= S dropped)
+template <int kN>
+__device__ __forceinline__ void store_frag(const float (&d)[kN / 2], float sc, __nv_bfloat16* base, long long row0,
+                                           int S, int row_in_seq0, int C) {
   const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
 #pragma unroll
   for (int rr = 0; rr < 2; ++rr) {
@@ -107,24 +138,29 @@ __device__ __forceinline__ void store_frag(const float (&d)[32], float sc, __nv_
     if (row_in_seq0 + r >= S) continue;
     __nv_bfloat16* dst = base + (row0 + r) * C + 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
+    for (int j = 0; j < kN / 8; ++j)
       *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16x2(d[4 * j + 2 * rr] * sc, d[4 * j + 2 * rr + 1] * sc);
   }
 }
 
-// rows row0 .. row0 + 63, head columns [h 64 kH, h 64 kH + 64 kH) of one sequence -> kH half-tiles
-template <int kH>
+// rows row0 .. row0 + 63, head columns [h kDh, h kDh + kDh) of one sequence -> kH half-tiles, or one 16-wide tile
+template <int kDh>
 __device__ __forceinline__ void load_rows(uint8_t* dst, const CUtensorMap* map, uint64_t* bar, int h, int row0, int seq) {
+  if constexpr (kDh == 16) {
+    tma_load_3d(dst, map, bar, h * kDh, row0, seq);
+  } else {
+    constexpr int kH = kDh / kD;
 #pragma unroll
-  for (int c = 0; c < kH; ++c) tma_load_3d(dst + c * kTileBytes, map, bar, (h * kH + c) * kD, row0, seq);
+    for (int c = 0; c < kH; ++c) tma_load_3d(dst + c * kTileBytes, map, bar, (h * kH + c) * kD, row0, seq);
+  }
 }
 
-// Forward of one (sequence, head, 64-query tile); kH = d_head / 64 half-tiles per row tile, O as kH m64n64 fragments.
-template <int kH>
+// Forward of one (sequence, head, 64-query tile) at head width kDh; O as kH fragments of 64 x kN.
+template <int kDh>
 __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtensorMap* mapK, const CUtensorMap* mapV,
                                           const FaParams& p) {
-  constexpr int kTB = kH * kTileBytes;   // one 64-row tile
-  constexpr int kDh = kH * kD;           // d_head
+  using G = FaGeo<kDh>;
+  constexpr int kTB = G::kTB, kH = G::kH, kN = G::kN, kR = G::kR;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;                   // 1 tile
@@ -153,21 +189,21 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
   __syncthreads();
   if (tid == 0) {
     mbar_expect_tx(q_full, kTB);
-    load_rows<kH>(sQ, mapQ, q_full, h, q0, seq);
+    load_rows<kDh>(sQ, mapQ, q_full, h, q0, seq);
     for (int j = 0; j < 2 && j < p.kv_tiles; ++j) {
       mbar_expect_tx(&kv_full[j], 2 * kTB);
-      load_rows<kH>(sKV + j * 2 * kTB, mapK, &kv_full[j], h, j * kTile, seq);
-      load_rows<kH>(sKV + j * 2 * kTB + kTB, mapV, &kv_full[j], h, j * kTile, seq);
+      load_rows<kDh>(sKV + j * 2 * kTB, mapK, &kv_full[j], h, j * kTile, seq);
+      load_rows<kDh>(sKV + j * 2 * kTB + kTB, mapV, &kv_full[j], h, j * kTile, seq);
     }
   }
   // Online softmax in base 2 with the scale folded in: p = 2^(s*c - m), c = scale*log2(e). l is a per-thread partial
   // row sum (the quad's four partial sums are added once at the end).
   const float cl2 = p.scale * 1.4426950408889634f;
-  float o[kH][32];
+  float o[kH][kR];
 #pragma unroll
   for (int c = 0; c < kH; ++c)
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
+    for (int i = 0; i < kR; ++i) o[c][i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   const uint32_t q_addr = smem_u32(sQ);
   mbar_wait(q_full, 0);
@@ -177,7 +213,7 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
     const uint32_t k_addr = smem_u32(sKV + st * 2 * kTB), v_addr = k_addr + kTB;
     float s[32];
     wgmma_fence();
-    gemm_rows<kH>(s, q_addr, k_addr);
+    gemm_rows<kDh>(s, q_addr, k_addr);
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(s);
@@ -213,12 +249,12 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
 #pragma unroll
     for (int c = 0; c < kH; ++c)
 #pragma unroll
-      for (int i = 0; i < 32; ++i) o[c][i] *= alpha[(i >> 1) & 1];
+      for (int i = 0; i < kR; ++i) o[c][i] *= alpha[(i >> 1) & 1];
     uint32_t a[4][4];
     frag_to_a(s, a);
     wgmma_fence();
 #pragma unroll
-    for (int c = 0; c < kH; ++c) gemm_acc(o[c], a, v_addr + c * kTileBytes);
+    for (int c = 0; c < kH; ++c) gemm_acc<kN>(o[c], a, v_addr + c * kTileBytes);
     wgmma_commit();
     wgmma_wait<0>();
 #pragma unroll
@@ -226,8 +262,8 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
     __syncthreads();  // every warp is done with stage st
     if (tid == 0 && j + 2 < p.kv_tiles) {
       mbar_expect_tx(&kv_full[st], 2 * kTB);
-      load_rows<kH>(sKV + st * 2 * kTB, mapK, &kv_full[st], h, (j + 2) * kTile, seq);
-      load_rows<kH>(sKV + st * 2 * kTB + kTB, mapV, &kv_full[st], h, (j + 2) * kTile, seq);
+      load_rows<kDh>(sKV + st * 2 * kTB, mapK, &kv_full[st], h, (j + 2) * kTile, seq);
+      load_rows<kDh>(sKV + st * 2 * kTB + kTB, mapV, &kv_full[st], h, (j + 2) * kTile, seq);
     }
   }
 #pragma unroll
@@ -239,10 +275,10 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
 #pragma unroll
   for (int c = 0; c < kH; ++c)
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[c][i] *= inv[(i >> 1) & 1];
+    for (int i = 0; i < kR; ++i) o[c][i] *= inv[(i >> 1) & 1];
   const long long row0 = (long long)seq * p.S + q0;
 #pragma unroll
-  for (int c = 0; c < kH; ++c) store_frag(o[c], 1.f, p.out + h * kDh + c * kD, row0, p.S, q0, p.C);
+  for (int c = 0; c < kH; ++c) store_frag<kN>(o[c], 1.f, p.out + h * kDh + c * kD, row0, p.S, q0, p.C);
 #pragma unroll
   for (int rr = 0; rr < 2; ++rr) {
     const int r = warp * 16 + (lane >> 2) + rr * 8;
@@ -252,7 +288,7 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
       for (int c = 0; c < kH; ++c) {
         const long long off = (row0 + r) * p.C + h * kDh + c * kD + 2 * (lane & 3);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
+        for (int j = 0; j < kN / 8; ++j) {
           const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.res + off + 8 * j));
           *reinterpret_cast<uint32_t*>(p.out_res + off + 8 * j) =
               pack_bf16x2(o[c][4 * j + 2 * rr] + t.x, o[c][4 * j + 2 * rr + 1] + t.y);
@@ -267,25 +303,32 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
 __global__ void __launch_bounds__(kFaThreads)
     og_flash_attn_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                              const __grid_constant__ CUtensorMap mapV, const FaParams p) {
-  flash_fwd<1>(&mapQ, &mapK, &mapV, p);
+  flash_fwd<64>(&mapQ, &mapK, &mapV, p);
 }
 
 __global__ void __launch_bounds__(kFaThreads)
     og_flash_attn_fwd_d128_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                                   const __grid_constant__ CUtensorMap mapV, const FaParams p) {
-  flash_fwd<2>(&mapQ, &mapK, &mapV, p);
+  flash_fwd<128>(&mapQ, &mapK, &mapV, p);
+}
+
+__global__ void __launch_bounds__(kFaThreads)
+    og_flash_attn_fwd_d16_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                 const __grid_constant__ CUtensorMap mapV, const FaParams p) {
+  flash_fwd<16>(&mapQ, &mapK, &mapV, p);
 }
 
 // ------------------------------------------------------------------------------------------------
 // backward (see the file header). The softmax scale is applied once per output element of dK / dQ, not per score.
-// kH = d_head / 64. MODE 0 at kH = 2 runs two warpgroups: both compute the full S^T and dP^T (contracting over all
-// 128 head dims), warpgroup w keeps dV and dK for head columns [64 w, 64 w + 64). MODE 1 keeps dQ as kH fragments.
+// kH = d_head / 64 at d = 64, 128 (1 at d = 16). MODE 0 at kH = 2 runs two warpgroups: both compute the full S^T and
+// dP^T (contracting over all 128 head dims), warpgroup w keeps dV and dK for head columns [64 w, 64 w + 64). MODE 1
+// keeps dQ as kH fragments.
 // ------------------------------------------------------------------------------------------------
-template <int MODE, int kH>
+template <int MODE, int kDh>
 __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtensorMap* mapK, const CUtensorMap* mapV,
                                           const CUtensorMap* mapDO, const FaBwdParams& p) {
-  constexpr int kTB = kH * kTileBytes;
-  constexpr int kDh = kH * kD;
+  using G = FaGeo<kDh>;
+  constexpr int kTB = G::kTB, kH = G::kH, kN = G::kN, kR = G::kR;
   constexpr int kNA = MODE == 0 ? 1 : kH;   // accumulator fragments per thread and output
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -321,12 +364,12 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
   __syncthreads();
   if (tid == 0) {
     mbar_expect_tx(fix_full, 2 * kTB);
-    load_rows<kH>(sFix, mapF0, fix_full, h, own * kTile, seq);
-    load_rows<kH>(sFix + kTB, mapF1, fix_full, h, own * kTile, seq);
+    load_rows<kDh>(sFix, mapF0, fix_full, h, own * kTile, seq);
+    load_rows<kDh>(sFix + kTB, mapF1, fix_full, h, own * kTile, seq);
     for (int it = 0; it < 2 && it < p.tiles; ++it) {
       mbar_expect_tx(&str_full[it], 2 * kTB);
-      load_rows<kH>(sStr + it * 2 * kTB, mapS0, &str_full[it], h, it * kTile, seq);
-      load_rows<kH>(sStr + it * 2 * kTB + kTB, mapS1, &str_full[it], h, it * kTile, seq);
+      load_rows<kDh>(sStr + it * 2 * kTB, mapS0, &str_full[it], h, it * kTile, seq);
+      load_rows<kDh>(sStr + it * 2 * kTB + kTB, mapS1, &str_full[it], h, it * kTile, seq);
     }
   }
   const float cl2 = p.scale * 1.4426950408889634f;
@@ -344,11 +387,11 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
       }
     }
   }
-  float acc0[kNA][32], acc1[kNA][32];   // MODE 0: dV, dK (head columns of half wg) ; MODE 1: dQ (acc1 unused)
+  float acc0[kNA][kR], acc1[kNA][kR];   // MODE 0: dV, dK (head columns of half wg) ; MODE 1: dQ (acc1 unused)
 #pragma unroll
   for (int c = 0; c < kNA; ++c)
 #pragma unroll
-    for (int i = 0; i < 32; ++i) acc0[c][i] = acc1[c][i] = 0.f;
+    for (int i = 0; i < kR; ++i) acc0[c][i] = acc1[c][i] = 0.f;
   const uint32_t f0 = smem_u32(sFix), f1 = f0 + kTB;
   mbar_wait(fix_full, 0);
   for (int it = 0; it < p.tiles; ++it) {
@@ -359,8 +402,8 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
     // MODE 1: s = S   = Q K^T, dp = dP   = dO V^T (rows = queries, columns = keys)
     float s[32], dp[32];
     wgmma_fence();
-    gemm_rows<kH>(s, f0, s0);
-    gemm_rows<kH>(dp, f1, s1);
+    gemm_rows<kDh>(s, f0, s0);
+    gemm_rows<kDh>(dp, f1, s1);
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(s);
@@ -396,11 +439,11 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
     wgmma_fence();
     if (MODE == 0) {
       frag_to_a(s, a_p);
-      gemm_acc(acc0[0], a_p, s1 + wg * kTileBytes);    // dV_j += P^T dO_i
-      gemm_acc(acc1[0], a_ds, s0 + wg * kTileBytes);   // dK_j += dS^T Q_i
+      gemm_acc<kN>(acc0[0], a_p, s1 + wg * kTileBytes);    // dV_j += P^T dO_i
+      gemm_acc<kN>(acc1[0], a_ds, s0 + wg * kTileBytes);   // dK_j += dS^T Q_i
     } else {
 #pragma unroll
-      for (int c = 0; c < kNA; ++c) gemm_acc(acc0[c], a_ds, s0 + c * kTileBytes);   // dQ_i += dS K_j
+      for (int c = 0; c < kNA; ++c) gemm_acc<kN>(acc0[c], a_ds, s0 + c * kTileBytes);   // dQ_i += dS K_j
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -412,17 +455,18 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
     __syncthreads();  // every warp is done with stage st
     if (tid == 0 && it + 2 < p.tiles) {
       mbar_expect_tx(&str_full[st], 2 * kTB);
-      load_rows<kH>(sStr + st * 2 * kTB, mapS0, &str_full[st], h, (it + 2) * kTile, seq);
-      load_rows<kH>(sStr + st * 2 * kTB + kTB, mapS1, &str_full[st], h, (it + 2) * kTile, seq);
+      load_rows<kDh>(sStr + st * 2 * kTB, mapS0, &str_full[st], h, (it + 2) * kTile, seq);
+      load_rows<kDh>(sStr + st * 2 * kTB + kTB, mapS1, &str_full[st], h, (it + 2) * kTile, seq);
     }
   }
   const long long row0 = (long long)seq * p.S + own * kTile;
   if (MODE == 0) {
-    store_frag(acc0[0], 1.f, p.dv + h * kDh + wg * kD, row0, p.S, own * kTile, p.C);
-    store_frag(acc1[0], p.scale, p.dk + h * kDh + wg * kD, row0, p.S, own * kTile, p.C);
+    store_frag<kN>(acc0[0], 1.f, p.dv + h * kDh + wg * kD, row0, p.S, own * kTile, p.C);
+    store_frag<kN>(acc1[0], p.scale, p.dk + h * kDh + wg * kD, row0, p.S, own * kTile, p.C);
   } else {
 #pragma unroll
-    for (int c = 0; c < kNA; ++c) store_frag(acc0[c], p.scale, p.dq + h * kDh + c * kD, row0, p.S, own * kTile, p.C);
+    for (int c = 0; c < kNA; ++c)
+      store_frag<kN>(acc0[c], p.scale, p.dq + h * kDh + c * kD, row0, p.S, own * kTile, p.C);
   }
 }
 
@@ -431,7 +475,7 @@ __global__ void __launch_bounds__(kFaThreads)
     og_flash_attn_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                              const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
                              const FaBwdParams p) {
-  flash_bwd<MODE, 1>(&mapQ, &mapK, &mapV, &mapDO, p);
+  flash_bwd<MODE, 64>(&mapQ, &mapK, &mapV, &mapDO, p);
 }
 
 template <int MODE>
@@ -439,7 +483,15 @@ __global__ void __launch_bounds__(MODE == 0 ? 2 * kFaThreads : kFaThreads)
     og_flash_attn_bwd_d128_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                                   const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
                                   const FaBwdParams p) {
-  flash_bwd<MODE, 2>(&mapQ, &mapK, &mapV, &mapDO, p);
+  flash_bwd<MODE, 128>(&mapQ, &mapK, &mapV, &mapDO, p);
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(kFaThreads)
+    og_flash_attn_bwd_d16_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                 const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
+                                 const FaBwdParams p) {
+  flash_bwd<MODE, 16>(&mapQ, &mapK, &mapV, &mapDO, p);
 }
 
 // delta[seq][h][s] = sum_d dO * O   (one warp per row, lanes over the head's 64 dims)
@@ -480,12 +532,42 @@ __global__ void og_attn_delta_d128_kernel(const __nv_bfloat16* __restrict__ o, c
   }
 }
 
+// the same at d_head = 16: one thread per (row, head), its 16 dims as two 16-byte loads of each operand, summed in
+// column order
+__global__ void og_attn_delta_d16_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ d_o,
+                                         float* __restrict__ delta, long long rows, int S, int C, int nh) {
+  const long long n0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long nt = (long long)gridDim.x * blockDim.x;
+  for (long long t = n0; t < rows * nh; t += nt) {
+    const int h = (int)(t % nh);
+    const long long row = t / nh;
+    const uint4* pa = reinterpret_cast<const uint4*>(o + row * C + h * 16);
+    const uint4* pb = reinterpret_cast<const uint4*>(d_o + row * C + h * 16);
+    float v = 0.f;
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      const uint4 ua = pa[c], ub = pb[c];
+      const __nv_bfloat162* a2 = reinterpret_cast<const __nv_bfloat162*>(&ua);
+      const __nv_bfloat162* b2 = reinterpret_cast<const __nv_bfloat162*>(&ub);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 a = __bfloat1622float2(a2[e]), b = __bfloat1622float2(b2[e]);
+        v = fmaf(a.x, b.x, v);
+        v = fmaf(a.y, b.y, v);
+      }
+    }
+    delta[((row / S) * nh + h) * (long long)S + row % S] = v;
+  }
+}
 
-static int make_seq_map(CUtensorMap* m, const void* base, int nseq, int S, int C) {
+// [nseq][S][C] rows; boxes of 64 rows by one 64-column half (128-byte swizzle) or, at d_head = 16, by one 16-column
+// head (32-byte swizzle)
+static int make_seq_map(CUtensorMap* m, const void* base, int nseq, int S, int C, int dh) {
   uint64_t dims[3] = {(uint64_t)C, (uint64_t)S, (uint64_t)nseq};
   uint64_t str[2] = {(uint64_t)C * 2, (uint64_t)S * C * 2};
-  uint32_t box[3] = {kD, kTile, 1};
-  return make_tmap_bf16(m, base, 3, dims, str, box);
+  uint32_t box[3] = {dh == 16 ? 16u : (uint32_t)kD, kTile, 1};
+  return make_tmap_bf16(m, base, 3, dims, str, box, nullptr,
+                        dh == 16 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 }  // namespace og
@@ -497,6 +579,7 @@ static int flash_d_head(int C, int n_head) {
   if (n_head < 1) return 0;
   if (C == n_head * 64) return 64;
   if (C == n_head * 128) return 128;
+  if (C == n_head * 16) return 16;
   return 0;
 }
 
@@ -505,7 +588,7 @@ extern "C" int og_flash_attn_fwd(const void* q, const void* k, const void* v, vo
                                  og_stream_t stream) {
   OG_REQUIRE(q && k && v && out, "flash_attn_fwd: null pointer");
   const int dh = flash_d_head(C, n_head);
-  OG_REQUIRE(dh != 0, "flash_attn_fwd: needs d_head = 64 or 128 (C=%d, n_head=%d)", C, n_head);
+  OG_REQUIRE(dh != 0, "flash_attn_fwd: needs d_head = 64, 128 or 16 (C=%d, n_head=%d)", C, n_head);
   OG_REQUIRE(nseq > 0 && S > 0, "flash_attn_fwd: empty problem");
   OG_REQUIRE(scale > 0.f, "flash_attn_fwd: scale must be positive (the row maximum is taken on raw scores)");
   FaParams p;
@@ -520,9 +603,9 @@ extern "C" int og_flash_attn_fwd(const void* q, const void* k, const void* v, vo
   OG_REQUIRE(!residual || out_res, "flash_attn_fwd: residual given without out_res");
   CUtensorMap mq, mk, mv;
   int r;
-  if ((r = make_seq_map(&mq, q, nseq, S, C)) != OG_OK) return r;
-  if ((r = make_seq_map(&mk, k, nseq, S, C)) != OG_OK) return r;
-  if ((r = make_seq_map(&mv, v, nseq, S, C)) != OG_OK) return r;
+  if ((r = make_seq_map(&mq, q, nseq, S, C, dh)) != OG_OK) return r;
+  if ((r = make_seq_map(&mk, k, nseq, S, C, dh)) != OG_OK) return r;
+  if ((r = make_seq_map(&mv, v, nseq, S, C, dh)) != OG_OK) return r;
   const long long grid = (long long)nseq * n_head * p.q_tiles;
   OG_REQUIRE(grid < (1LL << 31), "flash_attn_fwd: too many tiles");
   if (dh == 64) {
@@ -534,6 +617,9 @@ extern "C" int og_flash_attn_fwd(const void* q, const void* k, const void* v, vo
       attr = true;
     }
     og_flash_attn_fwd_kernel<<<(unsigned)grid, kFaThreads, smem_bytes, (cudaStream_t)stream>>>(mq, mk, mv, p);
+  } else if (dh == 16) {
+    const size_t smem_bytes = 5 * FaGeo<16>::kTB + 1024 + 64;   // Q, 2 x (K, V) at 2 KiB a tile
+    og_flash_attn_fwd_d16_kernel<<<(unsigned)grid, kFaThreads, smem_bytes, (cudaStream_t)stream>>>(mq, mk, mv, p);
   } else {
     const size_t smem_bytes = 10 * kTileBytes + 1024 + 64;   // Q, 2 x (K, V) at 16 KiB a tile
     static bool attr = false;
@@ -554,7 +640,7 @@ extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, co
                                  int C, int n_head, float scale, og_stream_t stream) {
   OG_REQUIRE(q && k && v && out && dout && lse && delta_ws && dq && dk && dv, "flash_attn_bwd: null pointer");
   const int dh = flash_d_head(C, n_head);
-  OG_REQUIRE(dh != 0, "flash_attn_bwd: needs d_head = 64 or 128 (C=%d, n_head=%d)", C, n_head);
+  OG_REQUIRE(dh != 0, "flash_attn_bwd: needs d_head = 64, 128 or 16 (C=%d, n_head=%d)", C, n_head);
   OG_REQUIRE(nseq > 0 && S > 0, "flash_attn_bwd: empty problem");
   OG_REQUIRE(scale > 0.f, "flash_attn_bwd: scale must be positive (as in the forward pass)");
   cudaStream_t s = (cudaStream_t)stream;
@@ -565,6 +651,10 @@ extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, co
     if (dh == 64)
       og_attn_delta_kernel<<<(unsigned)blocks, 256, 0, s>>>((const __nv_bfloat16*)out, (const __nv_bfloat16*)dout,
                                                            delta_ws, rows, S, C, n_head);
+    else if (dh == 16)
+      og_attn_delta_d16_kernel<<<(unsigned)std::min((rows * n_head + 255) / 256, (long long)num_sms() * 16), 256, 0,
+                                 s>>>(
+          (const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, delta_ws, rows, S, C, n_head);
     else
       og_attn_delta_d128_kernel<<<(unsigned)blocks, 256, 0, s>>>(
           (const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, delta_ws, rows, S, C, n_head);
@@ -580,10 +670,10 @@ extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, co
   p.dq = (__nv_bfloat16*)dq; p.dk = (__nv_bfloat16*)dk; p.dv = (__nv_bfloat16*)dv;
   CUtensorMap mq, mk, mv, mdo;
   int r;
-  if ((r = make_seq_map(&mq, q, nseq, S, C)) != OG_OK) return r;
-  if ((r = make_seq_map(&mk, k, nseq, S, C)) != OG_OK) return r;
-  if ((r = make_seq_map(&mv, v, nseq, S, C)) != OG_OK) return r;
-  if ((r = make_seq_map(&mdo, dout, nseq, S, C)) != OG_OK) return r;
+  if ((r = make_seq_map(&mq, q, nseq, S, C, dh)) != OG_OK) return r;
+  if ((r = make_seq_map(&mk, k, nseq, S, C, dh)) != OG_OK) return r;
+  if ((r = make_seq_map(&mv, v, nseq, S, C, dh)) != OG_OK) return r;
+  if ((r = make_seq_map(&mdo, dout, nseq, S, C, dh)) != OG_OK) return r;
   const long long grid = (long long)nseq * n_head * p.tiles;
   OG_REQUIRE(grid < (1LL << 31), "flash_attn_bwd: too many tiles");
   if (dh == 64) {
@@ -599,6 +689,11 @@ extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, co
     og_flash_attn_bwd_kernel<0><<<(unsigned)grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
     OG_CHECK_CUDA(cudaGetLastError());
     og_flash_attn_bwd_kernel<1><<<(unsigned)grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
+  } else if (dh == 16) {
+    const size_t smem_bytes = 6 * FaGeo<16>::kTB + 1024 + 64;   // 2 + 2 x 2 tiles of 2 KiB
+    og_flash_attn_bwd_d16_kernel<0><<<(unsigned)grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
+    OG_CHECK_CUDA(cudaGetLastError());
+    og_flash_attn_bwd_d16_kernel<1><<<(unsigned)grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p);
   } else {
     const size_t smem_bytes = 12 * kTileBytes + 1024 + 64;   // 2 + 2 x 2 tiles of 16 KiB
     static bool attr = false;

@@ -32,7 +32,7 @@ PFN_encodeTiled get_encode_tiled() {
 }
 
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box, const uint32_t* elem_strides) {
+                   const uint32_t* box, const uint32_t* elem_strides, CUtensorMapSwizzle swizzle) {
   PFN_encodeTiled enc = get_encode_tiled();
   if (!enc) {
     set_error("cuTensorMapEncodeTiled is unavailable (no CUDA driver / GPU?)");
@@ -48,7 +48,7 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
   }
   for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
   CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed (CUresult %d): rank %d dims [%llu %llu %llu %llu %llu] box [%u %u %u %u %u]",

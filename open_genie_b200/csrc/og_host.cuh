@@ -39,12 +39,13 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
 
 PFN_encodeTiled get_encode_tiled();
 
-// Encode a bf16 tensor map with 128-byte swizzle and zero OOB fill.
+// Encode a bf16 tensor map with zero OOB fill and the given swizzle (128-byte by default).
 // dims[0] is the contiguous dimension; strides_bytes[i] is the stride of dims[i+1].
 // elem_strides (optional): TMA traversal stride per dimension — box[i] then counts the SOURCE span, and
 // ceil(box[i] / elem_strides[i]) elements land in shared memory (strided convolution input boxes).
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box, const uint32_t* elem_strides = nullptr);
+                   const uint32_t* box, const uint32_t* elem_strides = nullptr,
+                   CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
 
 int num_sms();
 

@@ -150,6 +150,18 @@ __host__ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr,
   return d;
 }
 
+// The same with the 32-byte swizzle (layout type 3): rows of 16 bf16 (32 B), the pattern repeating every 256 B.
+// K-major operand: 8-row groups `sbo` = 256 B apart, one k16 slice per row. MN-major operand: 16-element MN panels
+// `lbo` bytes apart, 8 k-rows of 32 B per 256 B group (`sbo`); a k16 step is 512 B.
+__host__ __device__ __forceinline__ uint64_t gmma_desc_sw32(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
+  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
+  d |= static_cast<uint64_t>(3) << 62;
+  return d;
+}
+
 // TA / TB: 1 = the operand is MN-major in shared memory (transposed), 0 = K-major.
 template <int TA, int TB>
 __device__ __forceinline__ void wgmma_ss_n16(float (&d)[8], uint64_t adesc, uint64_t bdesc, int scale_d) {
@@ -176,6 +188,16 @@ __device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t adesc, uin
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+// A from registers (the m64k16 A fragment: a[0..3] = rows r0 / r0 + 8, k 2q.. / 8 + 2q..), B from shared memory
+template <int TB>
+__device__ __forceinline__ void wgmma_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, %14;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d), "n"(TB));
 }
 
 template <int TB>

@@ -1,4 +1,4 @@
-// temporal_attn_long.cu — temporal (causal, d_head = 64 or 128) attention for clips of any length: FlashAttention-2
+// temporal_attn_long.cu — temporal (causal, d_head = 16, 64 or 128) attention for clips of any length: FlashAttention-2
 // on mma.sync m16n8k16, tiled over queries and keys, online softmax in fp32.
 //
 // STATUS: checked by tests/test_gpu_temporal_long.py (kernel level against float64 for T = 1 .. 1024, model level
@@ -27,17 +27,20 @@
 //                                         (b, h), accumulates in registers and adds the chunk into the fp32 outputs
 //                                         with atomics.
 // Both backward kernels recompute P = exp(scale * S - lse); dS = P (dP - delta). No atomics except the kv_bcast flush.
-// Outputs are staged in shared memory and stored as whole 128-byte row segments.
+// Outputs are staged in shared memory and stored as whole row segments (128 bytes at D = 64).
 //
-// Head width D (template argument, 64 or 128; ops._TimeAttnFn sends every T here at D = 128). Staged rows are 2D bytes
-// plus 16 of padding (144 / 272 B, both an odd number of 16-byte units, so ldmatrix stays conflict free); tiles are
-// 9 / 17 KiB, and shared memory at D = 128 is 85 KiB (forward), 119 KiB (dQ) and 103 KiB (dK / dV). The forward and dQ
-// kernels keep their shape, with D / 8 n-tiles of accumulators per lane. The dK / dV kernel cannot hold dK and dV for
-// 128 columns (16 rows x 128 columns x 2 = 128 accumulators per lane on top of S^T and dP^T): at D = 128 it runs 8
+// Head width D (template argument, 16, 64 or 128; ops._TimeAttnFn sends every T here at D = 16 and 128). Staged rows
+// are 2D bytes plus 16 of padding (144 / 272 B, both an odd number of 16-byte units, so ldmatrix stays conflict free);
+// tiles are 9 / 17 KiB, and shared memory at D = 128 is 85 KiB (forward), 119 KiB (dQ) and 103 KiB (dK / dV). The
+// forward and dQ kernels keep their shape, with D / 8 n-tiles of accumulators per lane. The dK / dV kernel cannot hold
+// dK and dV for 128 columns (16 rows x 128 columns x 2 = 128 accumulators per lane on top of S^T and dP^T): at D = 128 it runs 8
 // warps, warps w and w + 4 own the same 16 key rows, both compute the full S^T and dP^T over the 128 dims, and each
 // keeps dK / dV for one 64-column half, as at D = 64.
+// At D = 16 rows are staged at a 48-byte pitch (3 x 16 B, conflict free as well) in 3 KiB tiles, a row leaves as two
+// 16-byte chunks, the fp32 output staging exactly fills one ring stage, and the dK / dV kernel (4 warps) keeps two n8
+// tiles of dK and dV per lane. Shared memory: 15 KiB (forward), 21 KiB (dQ), 19 KiB (dK / dV).
 // Registers (nvcc 12.9, -O3, sm_90a; no spills): D = 64: fwd 128, dQ 167, dK/dV 230; D = 128: fwd 167, dQ 245,
-// dK/dV 230 (256 threads).
+// dK/dV 230 (256 threads); D = 16: fwd 72, dQ 94, dK/dV 135.
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 #include "temporal_mma_frag.cuh"
@@ -58,14 +61,15 @@ constexpr int kVecBytes = kTile * 4;           // 64 fp32 values (lse or delta o
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 
-// Shapes at head width D (64 or 128)
+// Shapes at head width D (16, 64 or 128)
 template <int D>
 struct Geo {
-  static constexpr int kPitch = 2 * D + 16;            // staged bf16 row: 144 B at 64, 272 B at 128 (ldmatrix conflict free)
-  static constexpr int kTileBytes = kTile * kPitch;    // one staged 64 x D tile: 9216 B / 17408 B
+  static constexpr int kPitch = 2 * D + 16;            // staged bf16 row: 48 / 144 / 272 B (ldmatrix conflict free)
+  static constexpr int kTileBytes = kTile * kPitch;    // one staged 64 x D tile: 3072 / 9216 / 17408 B
   static constexpr int kFPitch = 4 * D + 32;           // fp32 output staging row (float2 stores conflict free)
   static constexpr int kNT = D / 8;                    // 8-column n-tiles of a full-width fragment
-  static constexpr int kDkdvThreads = D == 64 ? 128 : 256;   // dK / dV: one warp, or a warp pair, per 16 key rows
+  static constexpr int kDkdvThreads = D == 128 ? 256 : 128;  // dK / dV: one warp, or a warp pair, per 16 key rows
+  static constexpr int kDkdvNT = D == 16 ? 2 : 8;      // dK / dV n-tiles a warp keeps (64 columns at D = 64, 128)
   static constexpr size_t kFwdSmem = 5 * (size_t)kTileBytes;                           // Q, 2 x (K, V)
   static constexpr size_t kDqSmem = 7 * (size_t)kTileBytes;                            // Q, dO, O, 2 x (K, V)
   static constexpr size_t kDkdvSmem = 6 * (size_t)kTileBytes + 4 * (size_t)kVecBytes;  // K, V, 2 x (Q, dO, lse, delta)
@@ -455,9 +459,10 @@ __global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
   const int key0 = j * kTile + wr * 16 + g;   // this lane's key rows: key0, key0 + 8
   const uint8_t* kw = ks + wr * 16 * kPitch;
   const uint8_t* vw = vs + wr * 16 * kPitch;
-  float dka[8][4], dva[8][4];
+  constexpr int kAN = G::kDkdvNT;
+  float dka[kAN][4], dva[kAN][4];
 #pragma unroll
-  for (int nt = 0; nt < 8; ++nt)
+  for (int nt = 0; nt < kAN; ++nt)
 #pragma unroll
     for (int e = 0; e < 4; ++e) dka[nt][e] = dva[nt][e] = 0.f;
   for (long long n = 0; n < items; ++n) {
@@ -491,25 +496,25 @@ __global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
         dp[nt >> 1][nt & 1][e] = p * (dp[nt >> 1][nt & 1][e] - (ce ? dl.y : dl.x));
       }
     }
-    gemm_nn_acc<D, 8>(dva, s, dosn, n0, lane);    // dV += P^T dO
-    gemm_nn_acc<D, 8>(dka, dp, qsn, n0, lane);    // dK += dS^T Q
+    gemm_nn_acc<D, kAN>(dva, s, dosn, n0, lane);    // dV += P^T dO
+    gemm_nn_acc<D, kAN>(dka, dp, qsn, n0, lane);    // dK += dS^T Q
   }
   const int t_w = j * kTile + wr * 16;
   if (!kv_bcast) {
     // every read of this warp's K / V rows is done (at D = 128 also by the partner warp, which reads all columns):
     // they stage the outputs
-    if (D == 64) __syncwarp(); else __syncthreads();
+    if (D == 128) __syncthreads(); else __syncwarp();
     uint8_t* kw_out = ks + wr * 16 * kPitch;
     uint8_t* vw_out = vs + wr * 16 * kPitch;
-    frags_to_rows<D, 8>(kw_out, dka, scale, scale, n0, lane);
-    frags_to_rows<D, 8>(vw_out, dva, 1.f, 1.f, n0, lane);
+    frags_to_rows<D, kAN>(kw_out, dka, scale, scale, n0, lane);
+    frags_to_rows<D, kAN>(vw_out, dva, 1.f, 1.f, n0, lane);
     __syncwarp();
-    rows_to_global<D, 8>(kw_out, dk + s0.q0, qpitch, t_w, T, half * 8, lane);
-    rows_to_global<D, 8>(vw_out, dv + s0.q0, qpitch, t_w, T, half * 8, lane);
+    rows_to_global<D, kAN>(kw_out, dk + s0.q0, qpitch, t_w, T, half * 8, lane);
+    rows_to_global<D, kAN>(vw_out, dv + s0.q0, qpitch, t_w, T, half * 8, lane);
   } else {
     // this chunk's sum over its pixels into the caller's fp32 [B][T][C] (unordered across chunks)
 #pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
+    for (int nt = 0; nt < kAN; ++nt)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int t = key0 + 8 * (e >> 1);
@@ -601,8 +606,8 @@ extern "C" int og_temporal_attn_long_fwd(const void* q, const void* k, const voi
   OG_REQUIRE(n_head >= 1 && C % n_head == 0, "temporal_attn_long_fwd: C=%d not divisible by n_head=%d", C, n_head);
   OG_REQUIRE(scale > 0.f, "temporal_attn_long_fwd: scale must be positive");
   const int dh = C / n_head;
-  if (dh != 64 && dh != 128) {
-    set_error("temporal_attn_long_fwd: d_head=%d not supported (64 or 128)", dh);
+  if (dh != 64 && dh != 128 && dh != 16) {
+    set_error("temporal_attn_long_fwd: d_head=%d not supported (16, 64 or 128)", dh);
     return OG_ERR_UNSUPPORTED_SHAPE;
   }
   OG_REQUIRE(long_aligned(q) && long_aligned(k) && long_aligned(v) && long_aligned(out) && long_aligned(residual) &&
@@ -611,10 +616,12 @@ extern "C" int og_temporal_attn_long_fwd(const void* q, const void* k, const voi
   const int tiles = (T + kTile - 1) / kTile;
   const long long grid = (long long)B * n_head * P * tiles;
   OG_REQUIRE(grid < (1LL << 31), "temporal_attn_long_fwd: too many tiles");
-  const int r = dh == 64 ? long_fwd<64>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
-                                        tiles, grid, (cudaStream_t)stream)
-                         : long_fwd<128>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
-                                         tiles, grid, (cudaStream_t)stream);
+  const int r = dh == 64    ? long_fwd<64>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
+                                           tiles, grid, (cudaStream_t)stream)
+                 : dh == 128 ? long_fwd<128>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
+                                             tiles, grid, (cudaStream_t)stream)
+                             : long_fwd<16>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
+                                            tiles, grid, (cudaStream_t)stream);
   if (r != OG_OK) return r;
   g_launches.fetch_add(1);
   return OG_OK;
@@ -632,8 +639,8 @@ extern "C" int og_temporal_attn_long_bwd(const void* q, const void* k, const voi
   OG_REQUIRE(n_head >= 1 && C % n_head == 0, "temporal_attn_long_bwd: C=%d not divisible by n_head=%d", C, n_head);
   OG_REQUIRE(scale > 0.f, "temporal_attn_long_bwd: scale must be positive");
   const int dh = C / n_head;
-  if (dh != 64 && dh != 128) {
-    set_error("temporal_attn_long_bwd: d_head=%d not supported (64 or 128)", dh);
+  if (dh != 64 && dh != 128 && dh != 16) {
+    set_error("temporal_attn_long_bwd: d_head=%d not supported (16, 64 or 128)", dh);
     return OG_ERR_UNSUPPORTED_SHAPE;
   }
   OG_REQUIRE(long_aligned(q) && long_aligned(k) && long_aligned(v) && long_aligned(out) && long_aligned(dout) &&
@@ -642,6 +649,9 @@ extern "C" int og_temporal_attn_long_bwd(const void* q, const void* k, const voi
   const int tiles = (T + kTile - 1) / kTile;
   const long long ntask = (long long)B * n_head * P;
   OG_REQUIRE(ntask * tiles < (1LL << 31), "temporal_attn_long_bwd: too many tiles");
+  if (dh == 16)
+    return long_bwd<16>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale,
+                        kv_bcast, tiles, (cudaStream_t)stream);
   return dh == 64 ? long_bwd<64>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C,
                                  n_head, scale, kv_bcast, tiles, (cudaStream_t)stream)
                   : long_bwd<128>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C,

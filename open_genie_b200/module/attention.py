@@ -5,9 +5,10 @@ conv3d_*.cu).
 Attention runs in the HEAD-valid configuration (SURVEY.md §7 H6/H8): d_inp == n_head*d_head, so to_q / to_k / to_v /
 to_out are Identity, q = k = v = LayerNorm(RoPE(x)); the one live conditioning path is the temporal one (latent action
 -> K, V through `time_attn_kw={'key_dim': k}`). Anything else raises.
-Head widths: d_head = 64 or 128 (flash attention and the temporal kernels have both; temporal attention at 128 runs the
-tiled kernels at every clip length). Space and time attention may use different widths when n_head * d_head matches,
-e.g. SpaceTimeAttention(n_head=(2, 1), d_head=(64, 128)); the FFN GroupNorm takes the temporal head count.
+Head widths: d_head = 16, 64 or 128 (flash attention and the temporal kernels have all three; temporal attention at 16
+and 128 runs the tiled kernels at every clip length). Space and time attention may use different widths when n_head * d_head
+matches, e.g. SpaceTimeAttention(n_head=(2, 1), d_head=(64, 128)) or (n_head=(4, 1), d_head=(16, 64)); the FFN
+GroupNorm takes the temporal head count.
 The FFN is the reference's ForwardBlock: GroupNorm -> conv (-> GELU -> conv)* with `hid_dim` hidden widths, ending at
 `d_out` channels (with transpose=True, where the skip becomes the 1x1x1 ffn_skip conv); `bias` gives every FFN conv a
 bias. Hidden widths and d_out are multiples of 64.
@@ -85,8 +86,8 @@ class Attention(nn.Module):
             raise NotImplementedError('attention dropout is not used by any shipped blueprint')
         if not embed:
             raise NotImplementedError('embed=False is not used by any shipped blueprint')
-        if d_head not in (64, 128):
-            raise NotImplementedError(f'the attention kernels take d_head = 64 or 128, not {d_head}')
+        if d_head not in (16, 64, 128):
+            raise NotImplementedError(f'the attention kernels take d_head = 16, 64 or 128, not {d_head}')
         self.norm = nn.LayerNorm(hid)
         self.embed = RotaryEmbedding(self.d_inp, kind=self.rope_kind)
         self.to_qkv = Adapter(qry_dim=self.d_inp, n_head=n_head, d_head=d_head, bias=bias, **kwargs)

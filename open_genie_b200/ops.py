@@ -966,9 +966,11 @@ _TIME_ATTN_SHORT_T = 32
 
 def _time_attn_tiled(T: int, C: int, n_head: int) -> bool:
     """Whether temporal attention runs on the tiled kernels (og_temporal_attn_long_fwd / bwd): clips longer than
-    _TIME_ATTN_SHORT_T, and every clip at d_head = 128, which the per-pixel kernels do not take (a lane would hold
-    2 x 128 fp32 values)."""
-    return T > _TIME_ATTN_SHORT_T or C == 128 * n_head
+    _TIME_ATTN_SHORT_T, and every clip at d_head = 128 or 16. The per-pixel kernels do not take 128 (a lane would hold
+    2 x 128 fp32 values). At 16 they would not be faster: timed at T = 16, B = 8, 256 pixels, 16 heads of 16 (H100
+    80GB HBM3, 700 W), the per-pixel kernels instantiated at 16 took 0.124 + 0.333 ms (fwd + bwd) against the tiled
+    kernels' 0.123 + 0.334 ms, and 0.111 + 0.287 ms against 0.123 + 0.252 ms with broadcast K / V."""
+    return T > _TIME_ATTN_SHORT_T or C == 128 * n_head or C == 16 * n_head
 
 
 class _TimeAttnFn(torch.autograd.Function):
