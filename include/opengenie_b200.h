@@ -237,6 +237,16 @@ int og_pixel_shuffle3d(const void* x, void* y, int inverse, int N, int T, int H,
 int og_blurpool3d(const void* x, void* y, float* scratch, int backward, int N, int T, int H, int W, int cin, int cout,
                   int k, int st, int sh, int sw, og_stream_t stream);
 
+/* BlurPooling3d with num_groups = groups (genie/module/video.py:487-537): output channel o belongs to group
+ * g = o / (cout/groups), and y[o] = blur_k(sum of input channels g*cin/groups .. (g+1)*cin/groups - 1); the backward
+ * is dx[c] = blur_k^T(sum of dy over the output channels of c's group). Same layouts, stride and padding as
+ * og_blurpool3d, and groups == 1 gives bit-identical results to it.
+ * scratch >= N*T*H*W*groups floats forward, N*To*Ho*Wo*groups backward (the per-voxel group sums).
+ * cin % groups == cout % groups == 0, (cin/groups) % 8 == (cout/groups) % 8 == 0 (a 16-byte vector stays in one
+ * group); x and y 16-byte aligned, scratch 4-byte aligned; odd k <= 7. */
+int og_blurpool3d_grouped(const void* x, void* y, float* scratch, int backward, int N, int T, int H, int W, int cin,
+                          int cout, int groups, int k, int st, int sh, int sw, og_stream_t stream);
+
 /* BlurPooling2d with num_groups == 1 (genie/module/image.py:43-85; registry name 'blur_pool'): x [N,H,W,cin] ->
  * y [N,Ho,Wo,cout], Pascal kernel k x k, stride (sh, sw), symmetric padding `pad` (the reference uses (k-1)//stride). */
 int og_blurpool2d(const void* x, void* y, float* scratch, int backward, int N, int H, int W, int cin, int cout, int k,

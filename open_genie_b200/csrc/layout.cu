@@ -511,12 +511,16 @@ extern "C" int og_pad_channels(const void* x, int x_f32, void* y, int64_t rows, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// BlurPooling3d (genie/module/video.py:487-537) with num_groups == 1: the reference repeats ONE Pascal kernel
-// over a dense (C_out x C_in) conv, so every output channel equals blur(sum_c x[:, c]) (SURVEY.md §8 a6).
-//   pass 1: s[v] = sum_c x[v][c]                       (fp32 [N*T*H*W])
-//   pass 2: y[vo][o] = sum_taps blur[tap] * s[vo*stride + tap - pad]   broadcast over o (bf16 NDHWC)
-// The adjoint (backward) is the same pair with the stencil transposed: g[vo] = sum_o dy[vo][o], then
-//   dx[v][c] = sum over (tap, vo) hitting v of blur[tap] * g[vo], broadcast over c.
+// BlurPooling3d (genie/module/video.py:487-537): the reference repeats ONE Pascal kernel over a conv with
+// `num_groups` = G groups, so output channel o of group g = o / (C_out/G) equals blur(sum of the C_in/G input
+// channels of group g) (SURVEY.md §8 a6). G = 1 is a dense conv: every output channel is blur(sum_c x[:, c]).
+//   pass 1: s[v][g] = sum_{c in group g} x[v][c]       (fp32 [N*T*H*W][G])
+//   pass 2: y[vo][o] = sum_taps blur[tap] * s[vo*stride + tap - pad][g(o)]   (bf16 NDHWC, 16-byte vectors)
+// The adjoint (backward) is the same pair with the stencil transposed: g[vo][g] = sum_{o in group g} dy[vo][o], then
+//   dx[v][c] = sum over (tap, vo) hitting v of blur[tap] * g[vo][g(c)].
+// Each 16-byte vector of 8 channels lies inside one group ((C/G) % 8 == 0), so pass 2 writes whole vectors.
+// ptxas -v (sm_90a, -O3): og_channel_sum_kernel 30 registers, og_group_sum_kernel 40, og_blur3d_fwd_kernel 48,
+// og_blur3d_bwd_kernel 46; no spills, 0-byte stack frames.
 // ------------------------------------------------------------------------------------------------
 namespace og {
 
@@ -532,20 +536,43 @@ __global__ void og_channel_sum_kernel(const __nv_bfloat16* __restrict__ x, float
   }
 }
 
+// num_groups > 1: one thread per (row, group). A group is cg = C / G contiguous channels (cg % 8 == 0), so the sum of
+// entry i = row * G + g reads cg / 8 whole 16-byte vectors starting at x + i * cg, and adds them in channel order.
+__global__ void og_group_sum_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ s, long long n_sums, int cg) {
+  const int nv = cg >> 3;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n_sums;
+       i += (long long)gridDim.x * blockDim.x) {
+    const uint4* p = reinterpret_cast<const uint4*>(x) + i * nv;
+    float a = 0.f;
+    for (int v = 0; v < nv; ++v) {
+      const uint4 u = __ldg(p + v);
+      const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[j]));
+        a += f.x;
+        a += f.y;
+      }
+    }
+    s[i] = a;
+  }
+}
+
 __device__ __forceinline__ float pascal(int k, int i) {  // binomial(k-1, i)
   float v = 1.f;
   for (int j = 0; j < i; ++j) v = v * (float)(k - 1 - j) / (float)(j + 1);
   return v;
 }
 
-// forward stencil + broadcast: one thread per (output voxel, 8-channel vector)
+// forward stencil + broadcast over the group: one thread per (output voxel, 8-channel vector)
 __global__ void og_blur3d_fwd_kernel(const float* __restrict__ s, __nv_bfloat16* __restrict__ y, int T, int H, int W,
                                      int To, int Ho, int Wo, int k, int st, int sh, int sw, int Cout, float norm,
-                                     long long total_vec, int kt, int pad_t, int pad) {
-  const int cv = Cout >> 3;
+                                     long long total_vec, int kt, int pad_t, int pad, int G) {
+  const int cv = Cout >> 3, gv = cv / G;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total_vec;
        i += (long long)gridDim.x * blockDim.x) {
     long long vo = i / cv;
+    const int g = (int)(i - vo * cv) / gv;
     const int wo = (int)(vo % Wo);
     long long r = vo / Wo;
     const int ho = (int)(r % Ho);
@@ -562,7 +589,7 @@ __global__ void og_blur3d_fwd_kernel(const float* __restrict__ s, __nv_bfloat16*
         for (int iw = 0; iw < k; ++iw) {
           const int w = wo * sw + iw - pad;
           if (w < 0 || w >= W) continue;
-          acc += pascal(kt, it) * pascal(k, ih) * pascal(k, iw) * s[(((long long)n * T + t) * H + h) * W + w];
+          acc += pascal(kt, it) * pascal(k, ih) * pascal(k, iw) * s[((((long long)n * T + t) * H + h) * W + w) * G + g];
         }
       }
     }
@@ -572,14 +599,15 @@ __global__ void og_blur3d_fwd_kernel(const float* __restrict__ s, __nv_bfloat16*
   }
 }
 
-// adjoint stencil + broadcast: one thread per (input voxel, 8-channel vector)
+// adjoint stencil + broadcast over the group: one thread per (input voxel, 8-channel vector)
 __global__ void og_blur3d_bwd_kernel(const float* __restrict__ g, __nv_bfloat16* __restrict__ dx, int T, int H, int W,
                                      int To, int Ho, int Wo, int k, int st, int sh, int sw, int Cin, float norm,
-                                     long long total_vec, int kt, int pad_t, int pad) {
-  const int cv = Cin >> 3;
+                                     long long total_vec, int kt, int pad_t, int pad, int G) {
+  const int cv = Cin >> 3, gv = cv / G;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total_vec;
        i += (long long)gridDim.x * blockDim.x) {
     long long v = i / cv;
+    const int grp = (int)(i - v * cv) / gv;
     const int w = (int)(v % W);
     long long r = v / W;
     const int h = (int)(r % H);
@@ -597,7 +625,7 @@ __global__ void og_blur3d_bwd_kernel(const float* __restrict__ g, __nv_bfloat16*
           const int wn = w + pad - iw;
           if (wn < 0 || wn % sw || wn / sw >= Wo) continue;
           acc += pascal(kt, it) * pascal(k, ih) * pascal(k, iw) *
-                 g[(((long long)n * To + tn / st) * Ho + hn / sh) * Wo + wn / sw];
+                 g[((((long long)n * To + tn / st) * Ho + hn / sh) * Wo + wn / sw) * G + grp];
         }
       }
     }
@@ -610,7 +638,8 @@ __global__ void og_blur3d_bwd_kernel(const float* __restrict__ g, __nv_bfloat16*
 }  // namespace og
 
 static int blurpool_launch(const void* x, void* y, float* scratch, int backward, int N, int T, int H, int W, int cin,
-                           int cout, int kt, int k, int st, int sh, int sw, int pad_t, int pad, og_stream_t stream) {
+                           int cout, int kt, int k, int st, int sh, int sw, int pad_t, int pad, og_stream_t stream,
+                           int G = 1) {
   using namespace og;
   OG_REQUIRE(x && y && scratch, "blurpool: null pointer");
   OG_REQUIRE(cin % 8 == 0 && cout % 8 == 0 && k >= 1 && k <= 7 && kt >= 1 && kt <= 7, "blurpool: need C %% 8 == 0 and k <= 7");
@@ -635,21 +664,27 @@ static int blurpool_launch(const void* x, void* y, float* scratch, int backward,
   const float norm = 1.f / (row_sum(kt) * row_sum(k) * row_sum(k));
   cudaStream_t s = (cudaStream_t)stream;
   if (!backward) {
-    // x: [N,T,H,W,cin] -> y: [N,To,Ho,Wo,cout]; scratch: N*T*H*W floats
+    // x: [N,T,H,W,cin] -> y: [N,To,Ho,Wo,cout]; scratch: N*T*H*W*G floats
     const long long rows = (long long)N * T * H * W;
-    og_channel_sum_kernel<<<ew_blocks(rows, 8), 256, 0, s>>>((const __nv_bfloat16*)x, scratch, rows, cin);
+    if (G == 1)
+      og_channel_sum_kernel<<<ew_blocks(rows, 8), 256, 0, s>>>((const __nv_bfloat16*)x, scratch, rows, cin);
+    else
+      og_group_sum_kernel<<<ew_blocks(rows * G, 256), 256, 0, s>>>((const __nv_bfloat16*)x, scratch, rows * G, cin / G);
     OG_CHECK_CUDA(cudaGetLastError());
     const long long total = (long long)N * To * Ho * Wo * (cout / 8);
     og_blur3d_fwd_kernel<<<ew_blocks(total, 256), 256, 0, s>>>(scratch, (__nv_bfloat16*)y, T, H, W, To, Ho, Wo, k, st, sh,
-                                                              sw, cout, norm, total, kt, pad_t, pad);
+                                                              sw, cout, norm, total, kt, pad_t, pad, G);
   } else {
-    // x: dy [N,To,Ho,Wo,cout] -> y: dx [N,T,H,W,cin]; scratch: N*To*Ho*Wo floats
+    // x: dy [N,To,Ho,Wo,cout] -> y: dx [N,T,H,W,cin]; scratch: N*To*Ho*Wo*G floats
     const long long rows = (long long)N * To * Ho * Wo;
-    og_channel_sum_kernel<<<ew_blocks(rows, 8), 256, 0, s>>>((const __nv_bfloat16*)x, scratch, rows, cout);
+    if (G == 1)
+      og_channel_sum_kernel<<<ew_blocks(rows, 8), 256, 0, s>>>((const __nv_bfloat16*)x, scratch, rows, cout);
+    else
+      og_group_sum_kernel<<<ew_blocks(rows * G, 256), 256, 0, s>>>((const __nv_bfloat16*)x, scratch, rows * G, cout / G);
     OG_CHECK_CUDA(cudaGetLastError());
     const long long total = (long long)N * T * H * W * (cin / 8);
     og_blur3d_bwd_kernel<<<ew_blocks(total, 256), 256, 0, s>>>(scratch, (__nv_bfloat16*)y, T, H, W, To, Ho, Wo, k, st, sh,
-                                                              sw, cin, norm, total, kt, pad_t, pad);
+                                                              sw, cin, norm, total, kt, pad_t, pad, G);
   }
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(2);
@@ -660,6 +695,23 @@ extern "C" int og_blurpool3d(const void* x, void* y, float* scratch, int backwar
                              int cout, int k, int st, int sh, int sw, og_stream_t stream) {
   OG_REQUIRE((k & 1) == 1, "blurpool3d: odd kernel sizes only (k=%d)", k);
   return blurpool_launch(x, y, scratch, backward, N, T, H, W, cin, cout, k, k, st, sh, sw, (k - 1) / 2, (k - 1) / 2, stream);
+}
+
+extern "C" int og_blurpool3d_grouped(const void* x, void* y, float* scratch, int backward, int N, int T, int H, int W,
+                                     int cin, int cout, int groups, int k, int st, int sh, int sw, og_stream_t stream) {
+  using namespace og;
+  OG_REQUIRE((k & 1) == 1, "blurpool3d_grouped: odd kernel sizes only (k=%d)", k);
+  OG_REQUIRE(groups >= 1 && cin % groups == 0 && cout % groups == 0,
+             "blurpool3d_grouped: groups=%d must divide cin=%d and cout=%d", groups, cin, cout);
+  OG_REQUIRE((cin / groups) % 8 == 0 && (cout / groups) % 8 == 0,
+             "blurpool3d_grouped: need (cin/groups) %% 8 == 0 and (cout/groups) %% 8 == 0 (cin=%d cout=%d groups=%d)",
+             cin, cout, groups);
+  OG_REQUIRE(x && y && scratch, "blurpool3d_grouped: null pointer");
+  // the group sums read x in 16-byte vectors
+  OG_REQUIRE(aligned16(x), "blurpool3d_grouped: x must be 16-byte aligned");
+  OG_REQUIRE((reinterpret_cast<uintptr_t>(scratch) & 3) == 0, "blurpool3d_grouped: scratch must be 4-byte aligned");
+  return blurpool_launch(x, y, scratch, backward, N, T, H, W, cin, cout, k, k, st, sh, sw, (k - 1) / 2, (k - 1) / 2,
+                         stream, groups);
 }
 
 extern "C" int og_blurpool2d(const void* x, void* y, float* scratch, int backward, int N, int H, int W, int cin, int cout,

@@ -108,17 +108,33 @@ class Conv3dParams(nn.Module):
         return ops.conv3d(x, self.weight, self.bias, self.packed(), self.geom, out_f32)
 
 
+def _causal_space_pads(padding, kernel_size):
+    """The (height, width) pads CausalConv3d derives from `padding` (genie/module/video.py:144-157): an int or None is
+    used for both, otherwise entries 0 and 1 are the height and width pads and further entries are ignored; None means
+    (k - 1) // 2. Returns None for a `padding` the reference would not accept."""
+    if padding is None or isinstance(padding, int):
+        padding = (padding, padding)
+    if not isinstance(padding, (tuple, list)) or len(padding) < 2:
+        return None
+    _, kh, kw = kernel_size
+    return (default(padding[0], (kh - 1) // 2), default(padding[1], (kw - 1) // 2))
+
+
 class CausalConv3d(nn.Module):
     """3-D causal convolution: time padded on the left only. Mirrors genie/module/video.py:106-200
-    (state_dict keys 'conv3d.weight', 'conv3d.bias'). pad_mode='constant' and dilation 1 only."""
+    (state_dict keys 'conv3d.weight', 'conv3d.bias'). pad_mode='constant' and dilation 1 only. `padding` is accepted
+    when it resolves to the default spatial pads, (kh - 1) // 2 and (kw - 1) // 2, which are the pads the kernels
+    implement."""
 
     def __init__(self, in_channels: int, out_channels: int, kernel_size, stride=(1, 1, 1), dilation=(1, 1, 1),
                  padding=None, pad_mode: str = 'constant', **kwargs):
         super().__init__()
         if _triple(dilation) != (1, 1, 1):
             raise NotImplementedError('CausalConv3d: dilation != 1 is outside the hot-path scope')
-        if pad_mode != 'constant' or padding not in (None, (None, None)):
-            raise NotImplementedError('CausalConv3d: only default constant padding is implemented')
+        k = _triple(kernel_size)
+        if pad_mode != 'constant' or _causal_space_pads(padding, k) != ((k[1] - 1) // 2, (k[2] - 1) // 2):
+            raise NotImplementedError('CausalConv3d: only constant padding with the default spatial pads '
+                                      '((k - 1) // 2) is implemented')
         self.conv3d = Conv3dParams(in_channels, out_channels, kernel_size, stride, causal=True,
                                    bias=kwargs.get('bias', True))
         self.in_channels, self.out_channels = in_channels, out_channels
@@ -215,16 +231,20 @@ class DepthToSpaceTimeUpsample(Upsample):
 
 
 class BlurPooling3d(nn.Module):
-    """Anti-aliased strided pooling — genie/module/video.py:487-537. With num_groups == 1 (the only value the
-    reference's VideoResidualBlock passes through its default) the repeated Pascal kernel makes every output
-    channel blur(sum_c x_c); that is what the kernel computes. Buffer 'blur' is kept for state_dict parity."""
+    """Anti-aliased strided pooling — genie/module/video.py:487-537. The reference repeats one normalised Pascal kernel
+    over a conv with `num_groups` groups, so output channel o of group g = o // (out_channels / num_groups) is
+    blur(sum of input group g); with num_groups == 1 every output channel is blur(sum_c x_c). That is what the kernels
+    compute. Time is padded symmetrically by (k - 1) // 2 like space, also inside a causal VideoResidualBlock, as in
+    the reference: the pooling is not causal. Buffer 'blur' is kept for state_dict parity."""
 
     def __init__(self, in_channels: int, kernel_size, out_channels: int | None = None, time_factor: int = 2,
                  space_factor=2, num_groups: int = 1, **kwargs) -> None:
         super().__init__()
         kernel_size = _triple(kernel_size)
-        if len(set(kernel_size)) != 1 or num_groups != 1 or kwargs:
-            raise NotImplementedError('BlurPooling3d: cubic kernels and num_groups == 1 only')
+        if len(set(kernel_size)) != 1 or kwargs:
+            raise NotImplementedError('BlurPooling3d: cubic kernels only')
+        if num_groups < 1 or (out_channels is not None and out_channels % num_groups):
+            raise ValueError(f'BlurPooling3d: out_channels={out_channels} must be divisible by num_groups={num_groups}')
         if isinstance(space_factor, int):
             space_factor = (space_factor, space_factor)
         k = kernel_size[0]
@@ -237,7 +257,11 @@ class BlurPooling3d(nn.Module):
         self.out_channels = out_channels
 
     def forward(self, inp: Tensor) -> Tensor:
-        return ops.blurpool3d(inp, self.k, self.stride, default(self.out_channels, inp.shape[1]))
+        cout = default(self.out_channels, inp.shape[1])
+        if inp.shape[1] % self.num_groups or cout % self.num_groups:
+            raise ValueError(f'BlurPooling3d: {inp.shape[1]} input and {cout} output channels must be divisible by '
+                             f'num_groups={self.num_groups}')
+        return ops.blurpool3d(inp, self.k, self.stride, cout, self.num_groups)
 
 
 class _GNParams(nn.GroupNorm):
@@ -252,12 +276,21 @@ class _Slot(nn.Identity):
     """Keeps nn.Sequential indices aligned with the reference (activation / Identity positions)."""
 
 
+def _conv_params(m: nn.Module) -> Conv3dParams:
+    return m.conv3d if isinstance(m, CausalConv3d) else m
+
+
 class VideoResidualBlock(nn.Module):
     """GN -> act -> conv -> GN -> act -> conv, plus an (always present) 1x1x1 conv shortcut —
     genie/module/video.py:539-656. state_dict keys: main.{0,4}.{weight,bias}, main.{2,6}.{weight,bias},
-    res.1.{weight,bias}.
+    res.1.{weight,bias}; with use_causal=True every conv is a CausalConv3d (main.{2,6}.conv3d.*, res.1.conv3d.*).
 
-    GPU execution: each GN+SiLU is one statistics pass + one fused apply pass, and the second conv, the
+    use_causal=True pads time by kt - 1 frames in front and none behind. The block is still not strictly causal, in the
+    reference too: GroupNorm statistics span all frames, and the blur pooling of `downsample` pads time symmetrically.
+    The reference passes padding=((kt-1)//2, (kh-1)//2, (kw-1)//2) to its CausalConv3d, which reads entries 0 and 1 as
+    the height and width pads; kernels where that differs from the default pads change H and W there, and raise here.
+
+    GPU execution: each GN+act is one statistics pass + one fused apply pass, and the second conv, the
     shortcut conv and the residual add are a single implicit GEMM (the shortcut's K columns are appended
     to the main conv's operand matrix)."""
 
@@ -268,15 +301,23 @@ class VideoResidualBlock(nn.Module):
         if isinstance(downsample, int):
             downsample = (downsample, downsample)
         if exists(downsample) and not use_blur:
-            raise NotImplementedError('VideoResidualBlock(downsample=..., use_blur=False) is not used by any blueprint')
-        if use_causal:
-            raise NotImplementedError('VideoResidualBlock(use_causal=True) is not used by any shipped blueprint')
+            raise NotImplementedError('VideoResidualBlock(downsample=..., use_blur=False) does not construct in the '
+                                      'reference (it passes num_groups to nn.Conv3d)')
         if act_fn not in ('swish', 'silu', 'leaky', 'relu') or not use_norm or pad_mode != 'constant':
             raise NotImplementedError('VideoResidualBlock: GroupNorm + SiLU / LeakyReLU / ReLU blocks are implemented')
         self.act_fn = 'silu' if act_fn == 'swish' else act_fn
         kernel_size = _triple(kernel_size)
+        if use_causal and len({(k - 1) // 2 for k in kernel_size}) != 1:
+            raise NotImplementedError(
+                f'VideoResidualBlock(use_causal=True, kernel_size={kernel_size}): the reference pads height by '
+                f'(kt - 1) // 2 and width by (kh - 1) // 2 (its CausalConv3d reads the padding tuple from the time '
+                f'entry), which changes H and W and breaks its residual add; only kernels with equal (k - 1) // 2 in '
+                f'all three dimensions are implemented')
         out_channels = default(out_channels, in_channels)
-        conv = lambda ci, co, k: Conv3dParams(ci, co, k, causal=use_causal)
+        if use_causal:
+            conv = lambda ci, co, k: CausalConv3d(ci, co, k)
+        else:
+            conv = lambda ci, co, k: Conv3dParams(ci, co, k, causal=False)
         tf, sf = downsample if exists(downsample) else (None, None)
         down = (lambda c: BlurPooling3d(c, kernel_size, time_factor=tf, space_factor=sf, num_groups=num_groups)) \
             if exists(downsample) else (lambda c: _Slot())
@@ -286,22 +327,25 @@ class VideoResidualBlock(nn.Module):
             _GNParams(num_groups, out_channels), _Slot(), conv(out_channels, out_channels, kernel_size),
         )
         self.has_down = exists(downsample)
+        self.use_causal = use_causal
         self.main[0].act = self.main[4].act = self.act_fn
-        self.main[6].fuse_shortcut(self.res[1])
+        _conv_params(self.main[6]).fuse_shortcut(_conv_params(self.res[1]))
         self.inp_channels, self.out_channels = in_channels, out_channels
         self.in_channels = in_channels
 
     def __setstate__(self, state):
         super().__setstate__(state)
-        self.main[6].fuse_shortcut(self.res[1])     # re-link inside the copy (see Conv3dParams.__setstate__)
+        # re-link inside the copy (see Conv3dParams.__setstate__)
+        _conv_params(self.main[6]).fuse_shortcut(_conv_params(self.res[1]))
 
     def forward(self, inp: Tensor) -> Tensor:
         fusable = all((c // self.main[0].num_groups) % 8 == 0 for c in (self.inp_channels, self.out_channels))
+        c1, c2, cr = _conv_params(self.main[2]), _conv_params(self.main[6]), _conv_params(self.res[1])
         if not self.has_down and inp.is_cuda and fusable:
             # whole block as one autograd node: GroupNorm statistics / backward reductions come out of the GEMM
             # epilogues, the shortcut gradient is added inside the last apply pass. The statistics of the output
             # ride along on the tensor so that the next block's first GroupNorm needs no pass of its own.
-            g1, c1, g2, c2, cr = self.main[0], self.main[2], self.main[4], self.main[6], self.res[1]
+            g1, g2 = self.main[0], self.main[4]
             ops._require_cuda(c1.weight, 'module parameters')
             sums = getattr(inp, '_og_gn_sums', None) if g1.num_groups == 1 else None
             y, y_sums = ops.residual_block(inp, sums, g1.weight, g1.bias, c1.weight, c1.bias, g2.weight, g2.bias,
@@ -309,14 +353,14 @@ class VideoResidualBlock(nn.Module):
                                            c2.geom, g1.num_groups, g1.eps, act=self.act_fn)
             y._og_gn_sums = y_sums
             return y
-        h = self.main[0](inp)                # GN + SiLU (fused)
-        h = self.main[2](h)                  # conv k3
+        h = self.main[0](inp)                # GN + act (fused)
+        h = c1(h)                            # conv k3
         skip = inp
         if self.has_down:                    # anti-aliased down-sampling of both branches (video.py:589-621)
             h = self.main[3](h)
             skip = self.res[0](inp)
-        h = self.main[4](h)                  # GN + SiLU (fused)
-        return self.main[6](h, x2=skip)      # conv k3 (+) 1x1x1 shortcut (+) add : one kernel
+        h = self.main[4](h)                  # GN + act (fused)
+        return c2(h, x2=skip)                # conv k3 (+) 1x1x1 shortcut (+) add : one kernel
 
     @property
     def inp_dim(self):

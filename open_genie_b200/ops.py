@@ -769,36 +769,46 @@ def space_to_depth3d(x, p, q, r):
 
 
 # ------------------------------------------------------------------------------------------------
-# blur pooling (num_groups == 1)
+# blur pooling
 # ------------------------------------------------------------------------------------------------
 class _BlurPoolFn(torch.autograd.Function):
+    """BlurPooling3d with `groups` groups: og_blurpool3d at groups == 1, og_blurpool3d_grouped otherwise."""
+
     @staticmethod
-    def forward(ctx, x, k: int, stride, cout: int):
+    def forward(ctx, x, k: int, stride, cout: int, groups: int = 1):
         xi = to_internal(x, bf16)
         B, C, T, H, W = xi.shape
         st, sh, sw = stride
         pad = (k - 1) // 2
         To, Ho, Wo = (T + 2 * pad - k) // st + 1, (H + 2 * pad - k) // sh + 1, (W + 2 * pad - k) // sw + 1
         y = empty_internal(B, cout, To, Ho, Wo, bf16, xi.device)
-        scratch = torch.empty(B * T * H * W, dtype=f32, device=xi.device)
-        _lib.call('og_blurpool3d', xi.data_ptr(), y.data_ptr(), scratch.data_ptr(), 0, B, T, H, W, C, cout, k, st, sh, sw,
-                  _stream())
-        ctx.cfg = (B, C, T, H, W, cout, k, st, sh, sw, To, Ho, Wo)
+        scratch = torch.empty(B * T * H * W * groups, dtype=f32, device=xi.device)
+        if groups == 1:
+            _lib.call('og_blurpool3d', xi.data_ptr(), y.data_ptr(), scratch.data_ptr(), 0, B, T, H, W, C, cout, k, st, sh,
+                      sw, _stream())
+        else:
+            _lib.call('og_blurpool3d_grouped', xi.data_ptr(), y.data_ptr(), scratch.data_ptr(), 0, B, T, H, W, C, cout,
+                      groups, k, st, sh, sw, _stream())
+        ctx.cfg = (B, C, T, H, W, cout, k, st, sh, sw, To, Ho, Wo, groups)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        B, C, T, H, W, cout, k, st, sh, sw, To, Ho, Wo = ctx.cfg
+        B, C, T, H, W, cout, k, st, sh, sw, To, Ho, Wo, groups = ctx.cfg
         dyb = _as_bf16_rows(dy, cout, cout)
         dx = empty_internal(B, C, T, H, W, bf16, dy.device)
-        scratch = torch.empty(B * To * Ho * Wo, dtype=f32, device=dy.device)
-        _lib.call('og_blurpool3d', dyb.data_ptr(), dx.data_ptr(), scratch.data_ptr(), 1, B, T, H, W, C, cout, k, st, sh,
-                  sw, _stream())
-        return dx, None, None, None
+        scratch = torch.empty(B * To * Ho * Wo * groups, dtype=f32, device=dy.device)
+        if groups == 1:
+            _lib.call('og_blurpool3d', dyb.data_ptr(), dx.data_ptr(), scratch.data_ptr(), 1, B, T, H, W, C, cout, k, st,
+                      sh, sw, _stream())
+        else:
+            _lib.call('og_blurpool3d_grouped', dyb.data_ptr(), dx.data_ptr(), scratch.data_ptr(), 1, B, T, H, W, C, cout,
+                      groups, k, st, sh, sw, _stream())
+        return dx, None, None, None, None
 
 
-def blurpool3d(x, k, stride, cout):
-    return _BlurPoolFn.apply(x, k, tuple(stride), cout)
+def blurpool3d(x, k, stride, cout, groups=1):
+    return _BlurPoolFn.apply(x, k, tuple(stride), cout, groups)
 
 
 # ------------------------------------------------------------------------------------------------
