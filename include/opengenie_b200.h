@@ -342,6 +342,24 @@ int og_flash_attn_bwd(const void* q, const void* k, const void* v, const void* o
                       const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq, int S, int C,
                       int n_head, float scale, og_stream_t stream);
 
+/* Attention dropout (SDPA's dropout_p, attention.py:229-234): the softmax probabilities P, after the causal mask, are
+ * multiplied by Z = M / (1 - p) with M a keep mask, O = (P Z) V. The backward pass is FlashAttention-2's: dV = (P Z)^T dO,
+ * dS = P ((dO V^T) Z - delta), delta = rowsum(dO O) of the dropped O. lse stays the log-sum-exp of the undropped scores.
+ * The mask is a pure function of (seed, sequence, head, query i, key j), regenerated by every pass:
+ *   z = sequence * n_head + head (64-bit; sequence = frame for flash attention, b * P + p for temporal attention)
+ *   c = ((j >> 4) * 8 + (j & 7), (i >> 4) * 8 + (i & 7), lo32(z), hi32(z))
+ *   r = Philox4x32-10(counter c, key (lo32(seed), hi32(seed)));  w = r[2 * ((i >> 3) & 1) + ((j >> 3) & 1)]
+ *   keep(i, j) iff w >= t, t = min(round(p * 2^32), 2^32 - 1)
+ * seed: device pointer to a uint64_t read by the kernels (a captured CUDA graph then reads the value of each replay).
+ * The arguments of og_flash_attn_fwd / bwd plus p and seed; -1 for a null seed or p outside [0, 1), otherwise the
+ * status codes and messages of og_flash_attn_fwd / bwd. */
+int og_flash_attn_dropout_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
+                              void* out_res, float* lse, int nseq, int S, int C, int n_head, float scale, float p,
+                              const uint64_t* seed, og_stream_t stream);
+int og_flash_attn_dropout_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout,
+                              const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq, int S, int C,
+                              int n_head, float scale, float p, const uint64_t* seed, og_stream_t stream);
+
 /* Temporal attention, is_causal=True (attention.py:347-371, 423): one sequence per (batch, pixel), T <= 32
  * (longer clips, and d_head = 16 or 128 at any T: og_temporal_attn_long_fwd / bwd below). d_head 32 or 64; other
  * widths return -2.
@@ -371,6 +389,15 @@ int og_temporal_attn_long_bwd(const void* q, const void* k, const void* v, const
                               const float* lse, float* delta_ws, void* dq, void* dk, void* dv, float* dk_bcast,
                               float* dv_bcast, int B, int T, int64_t P, int C, int n_head, float scale, int kv_bcast,
                               og_stream_t stream);
+/* Temporal attention with dropout: the arguments of og_temporal_attn_long_fwd / bwd plus p and seed, with the mask and
+ * the contract of og_flash_attn_dropout_fwd / bwd (sequence = b * P + p, also with kv_bcast). */
+int og_temporal_attn_long_dropout_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
+                                      void* out_res, float* lse, int B, int T, int64_t P, int C, int n_head,
+                                      float scale, int kv_bcast, float p, const uint64_t* seed, og_stream_t stream);
+int og_temporal_attn_long_dropout_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout,
+                                      const float* lse, float* delta_ws, void* dq, void* dk, void* dv,
+                                      float* dk_bcast, float* dv_bcast, int B, int T, int64_t P, int C, int n_head,
+                                      float scale, int kv_bcast, float p, const uint64_t* seed, og_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * DynamicsModel rows (genie/dynamics.py)

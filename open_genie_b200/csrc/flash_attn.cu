@@ -44,8 +44,16 @@
 // per 64 MMA FLOP forward).
 // Registers (nvcc 12.9, -O3, sm_90a; no spills): d = 64: fwd 98, MODE 0 168, MODE 1 122; d = 128: fwd 130,
 // MODE 0 175 (256 threads), MODE 1 154; d = 16: fwd 66, MODE 0 128, MODE 1 98, delta 32.
+//
+// Dropout (og_flash_attn_dropout_fwd_kernel<d>, og_flash_attn_dropout_bwd_kernel<MODE, d>): the same bodies with kDrop
+// set; the mask is attn_dropout.cuh's. The forward keeps the row max and sum of the undropped P (the lse it writes is
+// the undropped one), zeroes the dropped P before P V and applies 1 / (1 - p) with 1 / l. MODE 0 feeds P Z^T to dV
+// (1 / (1 - p) at the store) and masks dP^T; MODE 1 masks dP; the delta kernels are unchanged (O is the dropped output).
+// With kDrop off the kernels are instruction-identical to those before dropout. Registers (no spills): d = 16: fwd 72,
+// MODE 0 126, MODE 1 117; d = 64: fwd 130, MODE 0 182, MODE 1 154; d = 128: fwd 128, MODE 0 195, MODE 1 198.
 #include "og_host.cuh"
 #include "og_ptx.cuh"
+#include "attn_dropout.cuh"
 
 namespace og {
 extern std::atomic<uint64_t> g_launches;
@@ -156,9 +164,9 @@ __device__ __forceinline__ void load_rows(uint8_t* dst, const CUtensorMap* map, 
 }
 
 // Forward of one (sequence, head, 64-query tile) at head width kDh; O as kH fragments of 64 x kN.
-template <int kDh>
+template <int kDh, bool kDrop = false>
 __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtensorMap* mapK, const CUtensorMap* mapV,
-                                          const FaParams& p) {
+                                          const FaParams& p, const DropParams* dr = nullptr) {
   using G = FaGeo<kDh>;
   constexpr int kTB = G::kTB, kH = G::kH, kN = G::kN, kR = G::kR;
   extern __shared__ uint8_t smem_raw[];
@@ -206,6 +214,8 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
     for (int i = 0; i < kR; ++i) o[c][i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   const uint32_t q_addr = smem_u32(sQ);
+  uint2 dkey;
+  if constexpr (kDrop) dkey = drop_key(dr->seed);
   mbar_wait(q_full, 0);
   for (int j = 0; j < p.kv_tiles; ++j) {
     const int st = j & 1;
@@ -246,6 +256,13 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
       }
       l[rr] = l[rr] * alpha[rr] + ls;
     }
+    if constexpr (kDrop) {   // l keeps the undropped sum; P V takes the kept probabilities (1 / (1 - p) at the end)
+      const uint32_t keep = drop_keep_tile<false>(q0 + warp * 16 + (lane >> 2), j * kTile + 2 * (lane & 3),
+                                                  (uint64_t)seq * p.nh + h, dkey, dr->thresh);
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (!((keep >> i) & 1u)) s[i] = 0.f;
+    }
 #pragma unroll
     for (int c = 0; c < kH; ++c)
 #pragma unroll
@@ -271,7 +288,11 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
     l[rr] += __shfl_xor_sync(0xffffffffu, l[rr], 1);
     l[rr] += __shfl_xor_sync(0xffffffffu, l[rr], 2);
   }
-  const float inv[2] = {1.f / l[0], 1.f / l[1]};
+  float inv[2] = {1.f / l[0], 1.f / l[1]};
+  if constexpr (kDrop) {
+    inv[0] *= dr->rscale;
+    inv[1] *= dr->rscale;
+  }
 #pragma unroll
   for (int c = 0; c < kH; ++c)
 #pragma unroll
@@ -318,15 +339,24 @@ __global__ void __launch_bounds__(kFaThreads)
   flash_fwd<16>(&mapQ, &mapK, &mapV, p);
 }
 
+// with attention dropout (attn_dropout.cuh), d_head = kDh
+template <int kDh>
+__global__ void __launch_bounds__(kFaThreads)
+    og_flash_attn_dropout_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                     const __grid_constant__ CUtensorMap mapV, const FaParams p, const DropParams d) {
+  flash_fwd<kDh, true>(&mapQ, &mapK, &mapV, p, &d);
+}
+
 // ------------------------------------------------------------------------------------------------
 // backward (see the file header). The softmax scale is applied once per output element of dK / dQ, not per score.
 // kH = d_head / 64 at d = 64, 128 (1 at d = 16). MODE 0 at kH = 2 runs two warpgroups: both compute the full S^T and
 // dP^T (contracting over all 128 head dims), warpgroup w keeps dV and dK for head columns [64 w, 64 w + 64). MODE 1
 // keeps dQ as kH fragments.
 // ------------------------------------------------------------------------------------------------
-template <int MODE, int kDh>
+template <int MODE, int kDh, bool kDrop = false>
 __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtensorMap* mapK, const CUtensorMap* mapV,
-                                          const CUtensorMap* mapDO, const FaBwdParams& p) {
+                                          const CUtensorMap* mapDO, const FaBwdParams& p,
+                                          const DropParams* dr = nullptr) {
   using G = FaGeo<kDh>;
   constexpr int kTB = G::kTB, kH = G::kH, kN = G::kN, kR = G::kR;
   constexpr int kNA = MODE == 0 ? 1 : kH;   // accumulator fragments per thread and output
@@ -393,6 +423,8 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
 #pragma unroll
     for (int i = 0; i < kR; ++i) acc0[c][i] = acc1[c][i] = 0.f;
   const uint32_t f0 = smem_u32(sFix), f1 = f0 + kTB;
+  uint2 dkey;
+  if constexpr (kDrop) dkey = drop_key(dr->seed);
   mbar_wait(fix_full, 0);
   for (int it = 0; it < p.tiles; ++it) {
     const int st = it & 1;
@@ -410,6 +442,10 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
     reg_fence(dp);
     const int row_tile = own, col_tile = it;
     const bool rows_full = (row_tile + 1) * kTile <= p.S, cols_full = (col_tile + 1) * kTile <= p.S;
+    uint32_t keep = 0;   // dropout: MODE 0 holds S^T (rows are keys), MODE 1 holds S
+    if constexpr (kDrop)
+      keep = drop_keep_tile<MODE == 0>(row_tile * kTile + r_base, col_tile * kTile + c_base, (uint64_t)seq * p.nh + h,
+                                       dkey, dr->thresh);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
@@ -429,8 +465,14 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
             const int row = row_tile * kTile + r_base + rr * 8;
             if (row >= p.S || col >= p.S) pv = 0.f;
           }
-          s[i] = pv;
-          dp[i] = pv * (dp[i] - dl);
+          if constexpr (kDrop) {   // dV takes P~ = P Z (1 / (1 - p) at the store); dS = P (dP Z - delta)
+            const bool kp = (keep >> i) & 1u;
+            s[i] = kp ? pv : 0.f;
+            dp[i] = pv * ((kp ? dp[i] * dr->rscale : 0.f) - dl);
+          } else {
+            s[i] = pv;
+            dp[i] = pv * (dp[i] - dl);
+          }
         }
       }
     }
@@ -461,7 +503,10 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
   }
   const long long row0 = (long long)seq * p.S + own * kTile;
   if (MODE == 0) {
-    store_frag<kN>(acc0[0], 1.f, p.dv + h * kDh + wg * kD, row0, p.S, own * kTile, p.C);
+    if constexpr (kDrop)
+      store_frag<kN>(acc0[0], dr->rscale, p.dv + h * kDh + wg * kD, row0, p.S, own * kTile, p.C);
+    else
+      store_frag<kN>(acc0[0], 1.f, p.dv + h * kDh + wg * kD, row0, p.S, own * kTile, p.C);
     store_frag<kN>(acc1[0], p.scale, p.dk + h * kDh + wg * kD, row0, p.S, own * kTile, p.C);
   } else {
 #pragma unroll
@@ -492,6 +537,14 @@ __global__ void __launch_bounds__(kFaThreads)
                                  const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
                                  const FaBwdParams p) {
   flash_bwd<MODE, 16>(&mapQ, &mapK, &mapV, &mapDO, p);
+}
+
+template <int MODE, int kDh>
+__global__ void __launch_bounds__(MODE == 0 && kDh == 128 ? 2 * kFaThreads : kFaThreads)
+    og_flash_attn_dropout_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                     const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
+                                     const FaBwdParams p, const DropParams d) {
+  flash_bwd<MODE, kDh, true>(&mapQ, &mapK, &mapV, &mapDO, p, &d);
 }
 
 // delta[seq][h][s] = sum_d dO * O   (one warp per row, lanes over the head's 64 dims)
@@ -583,9 +636,45 @@ static int flash_d_head(int C, int n_head) {
   return 0;
 }
 
-extern "C" int og_flash_attn_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
-                                 void* out_res, float* lse, int nseq, int S, int C, int n_head, float scale,
-                                 og_stream_t stream) {
+// the dropout kernels at d_head = kDh (shared memory as for the kernels without dropout)
+template <int kDh>
+static int flash_dropout_fwd_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv,
+                                    const FaParams& p, const DropParams& d, unsigned grid, cudaStream_t s) {
+  const size_t smem_bytes = 5 * FaGeo<kDh>::kTB + 1024 + 64;
+  static bool attr = false;
+  if (!attr) {
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_dropout_fwd_kernel<kDh>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    attr = true;
+  }
+  og_flash_attn_dropout_fwd_kernel<kDh><<<grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, p, d);
+  return OG_OK;
+}
+
+template <int kDh>
+static int flash_dropout_bwd_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv,
+                                    const CUtensorMap& mdo, const FaBwdParams& p, const DropParams& d, unsigned grid,
+                                    cudaStream_t s) {
+  const size_t smem_bytes = 6 * FaGeo<kDh>::kTB + 1024 + 64;
+  static bool attr = false;
+  if (!attr) {
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_dropout_bwd_kernel<0, kDh>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_dropout_bwd_kernel<1, kDh>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    attr = true;
+  }
+  og_flash_attn_dropout_bwd_kernel<0, kDh><<<grid, kDh == 128 ? 2 * kFaThreads : kFaThreads, smem_bytes, s>>>(
+      mq, mk, mv, mdo, p, d);
+  OG_CHECK_CUDA(cudaGetLastError());
+  og_flash_attn_dropout_bwd_kernel<1, kDh><<<grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p, d);
+  return OG_OK;
+}
+
+// og_flash_attn_fwd, and og_flash_attn_dropout_fwd when `drop` is given
+static int flash_fwd_call(const void* q, const void* k, const void* v, void* out, const void* residual, void* out_res,
+                          float* lse, int nseq, int S, int C, int n_head, float scale, const DropParams* drop,
+                          og_stream_t stream) {
   OG_REQUIRE(q && k && v && out, "flash_attn_fwd: null pointer");
   const int dh = flash_d_head(C, n_head);
   OG_REQUIRE(dh != 0, "flash_attn_fwd: needs d_head = 64, 128 or 16 (C=%d, n_head=%d)", C, n_head);
@@ -608,7 +697,12 @@ extern "C" int og_flash_attn_fwd(const void* q, const void* k, const void* v, vo
   if ((r = make_seq_map(&mv, v, nseq, S, C, dh)) != OG_OK) return r;
   const long long grid = (long long)nseq * n_head * p.q_tiles;
   OG_REQUIRE(grid < (1LL << 31), "flash_attn_fwd: too many tiles");
-  if (dh == 64) {
+  if (drop) {
+    const int r2 = dh == 64    ? flash_dropout_fwd_launch<64>(mq, mk, mv, p, *drop, (unsigned)grid, (cudaStream_t)stream)
+                   : dh == 128 ? flash_dropout_fwd_launch<128>(mq, mk, mv, p, *drop, (unsigned)grid, (cudaStream_t)stream)
+                               : flash_dropout_fwd_launch<16>(mq, mk, mv, p, *drop, (unsigned)grid, (cudaStream_t)stream);
+    if (r2 != OG_OK) return r2;
+  } else if (dh == 64) {
     const size_t smem_bytes = 5 * kTileBytes + 1024 + 64;
     static bool attr = false;
     if (!attr) {
@@ -635,9 +729,24 @@ extern "C" int og_flash_attn_fwd(const void* q, const void* k, const void* v, vo
   return OG_OK;
 }
 
-extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout,
-                                 const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq, int S,
-                                 int C, int n_head, float scale, og_stream_t stream) {
+extern "C" int og_flash_attn_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
+                                 void* out_res, float* lse, int nseq, int S, int C, int n_head, float scale,
+                                 og_stream_t stream) {
+  return flash_fwd_call(q, k, v, out, residual, out_res, lse, nseq, S, C, n_head, scale, nullptr, stream);
+}
+
+extern "C" int og_flash_attn_dropout_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
+                                         void* out_res, float* lse, int nseq, int S, int C, int n_head, float scale,
+                                         float p, const uint64_t* seed, og_stream_t stream) {
+  DropParams d;
+  if (const int r = drop_params(p, seed, "flash_attn_dropout_fwd", &d)) return r;
+  return flash_fwd_call(q, k, v, out, residual, out_res, lse, nseq, S, C, n_head, scale, &d, stream);
+}
+
+// og_flash_attn_bwd, and og_flash_attn_dropout_bwd when `drop` is given
+static int flash_bwd_call(const void* q, const void* k, const void* v, const void* out, const void* dout,
+                          const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq, int S, int C,
+                          int n_head, float scale, const DropParams* drop, og_stream_t stream) {
   OG_REQUIRE(q && k && v && out && dout && lse && delta_ws && dq && dk && dv, "flash_attn_bwd: null pointer");
   const int dh = flash_d_head(C, n_head);
   OG_REQUIRE(dh != 0, "flash_attn_bwd: needs d_head = 64, 128 or 16 (C=%d, n_head=%d)", C, n_head);
@@ -676,7 +785,12 @@ extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, co
   if ((r = make_seq_map(&mdo, dout, nseq, S, C, dh)) != OG_OK) return r;
   const long long grid = (long long)nseq * n_head * p.tiles;
   OG_REQUIRE(grid < (1LL << 31), "flash_attn_bwd: too many tiles");
-  if (dh == 64) {
+  if (drop) {
+    const int r2 = dh == 64    ? flash_dropout_bwd_launch<64>(mq, mk, mv, mdo, p, *drop, (unsigned)grid, s)
+                   : dh == 128 ? flash_dropout_bwd_launch<128>(mq, mk, mv, mdo, p, *drop, (unsigned)grid, s)
+                               : flash_dropout_bwd_launch<16>(mq, mk, mv, mdo, p, *drop, (unsigned)grid, s);
+    if (r2 != OG_OK) return r2;
+  } else if (dh == 64) {
     const size_t smem_bytes = 6 * kTileBytes + 1024 + 64;
     static bool attr = false;
     if (!attr) {
@@ -711,4 +825,19 @@ extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, co
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(2);
   return OG_OK;
+}
+
+extern "C" int og_flash_attn_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout,
+                                 const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq, int S,
+                                 int C, int n_head, float scale, og_stream_t stream) {
+  return flash_bwd_call(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, nseq, S, C, n_head, scale, nullptr, stream);
+}
+
+extern "C" int og_flash_attn_dropout_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout,
+                                         const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq,
+                                         int S, int C, int n_head, float scale, float p, const uint64_t* seed,
+                                         og_stream_t stream) {
+  DropParams d;
+  if (const int r = drop_params(p, seed, "flash_attn_dropout_bwd", &d)) return r;
+  return flash_bwd_call(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, nseq, S, C, n_head, scale, &d, stream);
 }

@@ -41,9 +41,15 @@
 // tiles of dK and dV per lane. Shared memory: 15 KiB (forward), 21 KiB (dQ), 19 KiB (dK / dV).
 // Registers (nvcc 12.9, -O3, sm_90a; no spills): D = 64: fwd 128, dQ 167, dK/dV 230; D = 128: fwd 167, dQ 245,
 // dK/dV 230 (256 threads); D = 16: fwd 72, dQ 94, dK/dV 135.
+// Dropout (og_temporal_attn_long_dropout_{fwd,bwd_dq,bwd_dkdv}_kernel<D>): the same bodies with kDrop set, the mask of
+// attn_dropout.cuh with sequence b * P + p (with kv_bcast too). The forward keeps the undropped row sum and lse; dQ
+// masks dP; dK / dV takes P Z for dV (1 / (1 - p) at the store or the atomic flush) and masks dP^T. With kDrop off the
+// kernels are instruction-identical to those before dropout. Registers (no spills): D = 16: fwd 78, dQ 127, dK/dV 168;
+// D = 64: fwd 128, dQ 168, dK/dV 237; D = 128: fwd 168, dQ 240, dK/dV 238 (256 threads).
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 #include "temporal_mma_frag.cuh"
+#include "attn_dropout.cuh"
 
 namespace og {
 extern std::atomic<uint64_t> g_launches;
@@ -196,13 +202,14 @@ __device__ __forceinline__ Seq decode(long long task, int T, long long P, int C,
   return s;
 }
 
-template <int D>
-__global__ void __launch_bounds__(kThreads)
-    og_temporal_attn_long_fwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+// Kernel bodies, templated on the head width and on dropout (attn_dropout.cuh; without it they are the kernels as they
+// were before dropout). The __global__ wrappers follow each body.
+template <int D, bool kDrop>
+__device__ __forceinline__ void long_fwd_body(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                      const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ res,
                                      __nv_bfloat16* __restrict__ out, __nv_bfloat16* __restrict__ out_res,
                                      float* __restrict__ lse, int B, int T, long long P, int C, int nh, float scale,
-                                     int kv_bcast, int tiles) {
+                                     int kv_bcast, int tiles, const DropParams* dr) {
   using G = Geo<D>;
   constexpr int kTileBytes = G::kTileBytes, kPitch = G::kPitch, kFPitch = G::kFPitch, kNT = G::kNT;
   extern __shared__ __align__(16) uint8_t smem_l[];
@@ -221,6 +228,12 @@ __global__ void __launch_bounds__(kThreads)
   const int row0 = i * kTile + warp * 16 + g;   // this lane's query rows: row0, row0 + 8
   const uint8_t* qw = qs + warp * 16 * kPitch;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  uint2 dkey;
+  uint64_t dz;
+  if constexpr (kDrop) {
+    dkey = drop_key(dr->seed);
+    dz = ((uint64_t)sq.b * P + sq.task % P) * nh + sq.h;
+  }
   float o[kNT][4];
 #pragma unroll
   for (int nt = 0; nt < kNT; ++nt)
@@ -269,6 +282,14 @@ __global__ void __launch_bounds__(kThreads)
         s[nt >> 1][nt & 1][e] = p;
         l[rr] += p;
       }
+    if constexpr (kDrop) {   // l keeps the undropped sum; P V takes the kept probabilities (1 / (1 - p) at the end)
+      const uint32_t keep = drop_keep_tile<false>(row0, j * kTile + 2 * qd, dz, dkey, dr->thresh);
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (!((keep >> (4 * nt + e)) & 1u)) s[nt >> 1][nt & 1][e] = 0.f;
+    }
 #pragma unroll
     for (int nt = 0; nt < kNT; ++nt)
 #pragma unroll
@@ -280,7 +301,11 @@ __global__ void __launch_bounds__(kThreads)
     l[rr] += __shfl_xor_sync(0xffffffffu, l[rr], 1);
     l[rr] += __shfl_xor_sync(0xffffffffu, l[rr], 2);
   }
-  const float inv[2] = {1.f / l[0], 1.f / l[1]};
+  float inv[2] = {1.f / l[0], 1.f / l[1]};
+  if constexpr (kDrop) {
+    inv[0] *= dr->rscale;
+    inv[1] *= dr->rscale;
+  }
   // fp32 staging of the normalised output in the ring stage the loop no longer reads (its last tile, i - 1, was
   // finished by every warp before the last barrier); each warp writes and reads only its own 16 rows
   uint8_t* st = ring + ((i + 1) & 1) * 2 * kTileBytes + warp * 16 * kFPitch;
@@ -321,11 +346,30 @@ __global__ void __launch_bounds__(kThreads)
 
 template <int D>
 __global__ void __launch_bounds__(kThreads)
-    og_temporal_attn_long_bwd_dq_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+    og_temporal_attn_long_fwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                     const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ res,
+                                     __nv_bfloat16* __restrict__ out, __nv_bfloat16* __restrict__ out_res,
+                                     float* __restrict__ lse, int B, int T, long long P, int C, int nh, float scale,
+                                     int kv_bcast, int tiles) {
+  long_fwd_body<D, false>(q, k, v, res, out, out_res, lse, B, T, P, C, nh, scale, kv_bcast, tiles, nullptr);
+}
+
+template <int D>
+__global__ void __launch_bounds__(kThreads)
+    og_temporal_attn_long_dropout_fwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                     const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ res,
+                                     __nv_bfloat16* __restrict__ out, __nv_bfloat16* __restrict__ out_res,
+                                     float* __restrict__ lse, int B, int T, long long P, int C, int nh, float scale,
+                                     int kv_bcast, int tiles, const DropParams d) {
+  long_fwd_body<D, true>(q, k, v, res, out, out_res, lse, B, T, P, C, nh, scale, kv_bcast, tiles, &d);
+}
+
+template <int D, bool kDrop>
+__device__ __forceinline__ void long_dq_body(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                         const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ o,
                                         const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse,
                                         float* __restrict__ delta, __nv_bfloat16* __restrict__ dq, int B, int T,
-                                        long long P, int C, int nh, float scale, int kv_bcast, int tiles) {
+                                        long long P, int C, int nh, float scale, int kv_bcast, int tiles, const DropParams* dr) {
   using G = Geo<D>;
   constexpr int kTileBytes = G::kTileBytes, kPitch = G::kPitch, kNT = G::kNT;
   extern __shared__ __align__(16) uint8_t smem_l[];
@@ -372,6 +416,12 @@ __global__ void __launch_bounds__(kThreads)
   }
   const float dl[2] = {__shfl_sync(0xffffffffu, dsum, 2 * g), __shfl_sync(0xffffffffu, dsum, 2 * g + 16)};
   const float cl2 = scale * kLog2e;
+  uint2 dkey;
+  uint64_t dz;
+  if constexpr (kDrop) {
+    dkey = drop_key(dr->seed);
+    dz = ((uint64_t)sq.b * P + sq.task % P) * nh + sq.h;
+  }
   float acc[kNT][4];
 #pragma unroll
   for (int nt = 0; nt < kNT; ++nt)
@@ -391,6 +441,8 @@ __global__ void __launch_bounds__(kThreads)
     float s[4][2][4], dp[4][2][4];
     gemm_nt<D>(s, qw, ks, lane);
     gemm_nt<D>(dp, dow, vs, lane);
+    uint32_t keep = 0;
+    if constexpr (kDrop) keep = drop_keep_tile<false>(row0, j * kTile + 2 * qd, dz, dkey, dr->thresh);
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
@@ -398,7 +450,12 @@ __global__ void __launch_bounds__(kThreads)
         const int rr = e >> 1, col = j * kTile + nt * 8 + 2 * qd + (e & 1);
         float p = ex2_approx(fmaf(s[nt >> 1][nt & 1][e], cl2, -lse2[rr]));
         if (j == i && col > row0 + 8 * rr) p = 0.f;
-        s[nt >> 1][nt & 1][e] = p * (dp[nt >> 1][nt & 1][e] - dl[rr]);   // dS (without the scale)
+        if constexpr (kDrop) {   // dS = P (dP Z - delta)
+          const float d = (keep >> (4 * nt + e)) & 1u ? dp[nt >> 1][nt & 1][e] * dr->rscale : 0.f;
+          s[nt >> 1][nt & 1][e] = p * (d - dl[rr]);
+        } else {
+          s[nt >> 1][nt & 1][e] = p * (dp[nt >> 1][nt & 1][e] - dl[rr]);   // dS (without the scale)
+        }
       }
     gemm_nn_acc<D, kNT>(acc, s, ks, 0, lane);
   }
@@ -410,19 +467,38 @@ __global__ void __launch_bounds__(kThreads)
   rows_to_global<D, D / 8>(qw_out, dq + sq.q0, qpitch, t_w, T, 0, lane);
 }
 
+template <int D>
+__global__ void __launch_bounds__(kThreads)
+    og_temporal_attn_long_bwd_dq_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                        const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ o,
+                                        const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse,
+                                        float* __restrict__ delta, __nv_bfloat16* __restrict__ dq, int B, int T,
+                                        long long P, int C, int nh, float scale, int kv_bcast, int tiles) {
+  long_dq_body<D, false>(q, k, v, o, dout, lse, delta, dq, B, T, P, C, nh, scale, kv_bcast, tiles, nullptr);
+}
+
+template <int D>
+__global__ void __launch_bounds__(kThreads)
+    og_temporal_attn_long_dropout_bwd_dq_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                        const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ o,
+                                        const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse,
+                                        float* __restrict__ delta, __nv_bfloat16* __restrict__ dq, int B, int T,
+                                        long long P, int C, int nh, float scale, int kv_bcast, int tiles, const DropParams d) {
+  long_dq_body<D, true>(q, k, v, o, dout, lse, delta, dq, B, T, P, C, nh, scale, kv_bcast, tiles, &d);
+}
+
 // D = 64: warp w owns key rows 16 w .. 16 w + 15 and all 64 head columns of dK / dV.
 // D = 128: eight warps; warps w and w + 4 own the same 16 key rows, each computes the full S^T and dP^T (over all 128
 // dims) and keeps dK / dV for head columns [64 (w / 4), 64 (w / 4) + 64) only, so a lane holds 2 x 32 accumulators
 // as at D = 64.
-template <int D>
-__global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
-    og_temporal_attn_long_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+template <int D, bool kDrop>
+__device__ __forceinline__ void long_dkdv_body(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                           const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ dout,
                                           const float* __restrict__ lse, const float* __restrict__ delta,
                                           __nv_bfloat16* __restrict__ dk, __nv_bfloat16* __restrict__ dv,
                                           float* __restrict__ dk_b, float* __restrict__ dv_b, int B, int T,
                                           long long P, int C, int nh, float scale, int kv_bcast, int tiles,
-                                          long long chunk, long long nchunk) {
+                                          long long chunk, long long nchunk, const DropParams* dr) {
   using G = Geo<D>;
   constexpr int kTileBytes = G::kTileBytes, kPitch = G::kPitch, NTHR = G::kDkdvThreads;
   extern __shared__ __align__(16) uint8_t smem_l[];
@@ -456,6 +532,8 @@ __global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
   load_item(0, 0);
   cp_async_commit();
   const float cl2 = scale * kLog2e;
+  uint2 dkey;
+  if constexpr (kDrop) dkey = drop_key(dr->seed);
   const int key0 = j * kTile + wr * 16 + g;   // this lane's key rows: key0, key0 + 8
   const uint8_t* kw = ks + wr * 16 * kPitch;
   const uint8_t* vw = vs + wr * 16 * kPitch;
@@ -482,6 +560,10 @@ __global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
     float s[4][2][4], dp[4][2][4];
     gemm_nt<D>(s, kw, qsn, lane);
     gemm_nt<D>(dp, vw, dosn, lane);
+    uint32_t keep = 0;   // dropout: rows are keys (S^T); the sequence is pixel p0 + n / nq of (b, h)
+    if constexpr (kDrop)
+      keep = drop_keep_tile<true>(key0, i * kTile + 2 * qd, ((uint64_t)s0.b * P + p0 + n / nq) * nh + s0.h, dkey,
+                                  dr->thresh);
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
       const int c = nt * 8 + 2 * qd;
@@ -492,8 +574,14 @@ __global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
         const int rr = e >> 1, ce = e & 1;
         float p = ex2_approx(fmaf(s[nt >> 1][nt & 1][e], cl2, -(ce ? ls.y : ls.x) * kLog2e));
         if (i == j && i * kTile + c + ce < key0 + 8 * rr) p = 0.f;
-        s[nt >> 1][nt & 1][e] = p;
-        dp[nt >> 1][nt & 1][e] = p * (dp[nt >> 1][nt & 1][e] - (ce ? dl.y : dl.x));
+        if constexpr (kDrop) {   // dV takes P~ = P Z (1 / (1 - p) at the flush); dS = P (dP Z - delta)
+          const bool kp = (keep >> (4 * nt + e)) & 1u;
+          s[nt >> 1][nt & 1][e] = kp ? p : 0.f;
+          dp[nt >> 1][nt & 1][e] = p * ((kp ? dp[nt >> 1][nt & 1][e] * dr->rscale : 0.f) - (ce ? dl.y : dl.x));
+        } else {
+          s[nt >> 1][nt & 1][e] = p;
+          dp[nt >> 1][nt & 1][e] = p * (dp[nt >> 1][nt & 1][e] - (ce ? dl.y : dl.x));
+        }
       }
     }
     gemm_nn_acc<D, kAN>(dva, s, dosn, n0, lane);    // dV += P^T dO
@@ -507,7 +595,10 @@ __global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
     uint8_t* kw_out = ks + wr * 16 * kPitch;
     uint8_t* vw_out = vs + wr * 16 * kPitch;
     frags_to_rows<D, kAN>(kw_out, dka, scale, scale, n0, lane);
-    frags_to_rows<D, kAN>(vw_out, dva, 1.f, 1.f, n0, lane);
+    if constexpr (kDrop)
+      frags_to_rows<D, kAN>(vw_out, dva, dr->rscale, dr->rscale, n0, lane);
+    else
+      frags_to_rows<D, kAN>(vw_out, dva, 1.f, 1.f, n0, lane);
     __syncwarp();
     rows_to_global<D, kAN>(kw_out, dk + s0.q0, qpitch, t_w, T, half * 8, lane);
     rows_to_global<D, kAN>(vw_out, dv + s0.q0, qpitch, t_w, T, half * 8, lane);
@@ -521,9 +612,38 @@ __global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
         if (t >= T) continue;
         const long long off = ((long long)s0.b * T + t) * C + (long long)s0.h * D + n0 + nt * 8 + 2 * qd + (e & 1);
         atomicAdd(dk_b + off, dka[nt][e] * scale);
-        atomicAdd(dv_b + off, dva[nt][e]);
+        if constexpr (kDrop)
+          atomicAdd(dv_b + off, dva[nt][e] * dr->rscale);
+        else
+          atomicAdd(dv_b + off, dva[nt][e]);
       }
   }
+}
+
+template <int D>
+__global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
+    og_temporal_attn_long_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                          const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ dout,
+                                          const float* __restrict__ lse, const float* __restrict__ delta,
+                                          __nv_bfloat16* __restrict__ dk, __nv_bfloat16* __restrict__ dv,
+                                          float* __restrict__ dk_b, float* __restrict__ dv_b, int B, int T,
+                                          long long P, int C, int nh, float scale, int kv_bcast, int tiles,
+                                          long long chunk, long long nchunk) {
+  long_dkdv_body<D, false>(q, k, v, dout, lse, delta, dk, dv, dk_b, dv_b, B, T, P, C, nh, scale, kv_bcast, tiles, chunk,
+                           nchunk, nullptr);
+}
+
+template <int D>
+__global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
+    og_temporal_attn_long_dropout_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                          const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ dout,
+                                          const float* __restrict__ lse, const float* __restrict__ delta,
+                                          __nv_bfloat16* __restrict__ dk, __nv_bfloat16* __restrict__ dv,
+                                          float* __restrict__ dk_b, float* __restrict__ dv_b, int B, int T,
+                                          long long P, int C, int nh, float scale, int kv_bcast, int tiles,
+                                          long long chunk, long long nchunk, const DropParams d) {
+  long_dkdv_body<D, true>(q, k, v, dout, lse, delta, dk, dv, dk_b, dv_b, B, T, P, C, nh, scale, kv_bcast, tiles, chunk,
+                          nchunk, &d);
 }
 
 }  // namespace tlong
@@ -538,8 +658,21 @@ namespace {
 template <int D>
 int long_fwd(const void* q, const void* k, const void* v, void* out, const void* residual, void* out_res, float* lse,
              int B, int T, int64_t P, int C, int n_head, float scale, int kv_bcast, int tiles, long long grid,
-             cudaStream_t stream) {
+             const DropParams* drop, cudaStream_t stream) {
   using namespace og::tlong;
+  if (drop) {
+    static bool dattr = false;
+    if (!dattr) {
+      OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_dropout_fwd_kernel<D>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Geo<D>::kFwdSmem));
+      dattr = true;
+    }
+    og_temporal_attn_long_dropout_fwd_kernel<D><<<(unsigned)grid, kThreads, Geo<D>::kFwdSmem, stream>>>(
+        (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)residual,
+        (__nv_bfloat16*)out, (__nv_bfloat16*)out_res, lse, B, T, P, C, n_head, scale, kv_bcast, tiles, *drop);
+    OG_CHECK_CUDA(cudaGetLastError());
+    return OG_OK;
+  }
   static bool attr = false;
   if (!attr) {   // above the 48 KiB default at D = 128
     OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_fwd_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -556,11 +689,18 @@ int long_fwd(const void* q, const void* k, const void* v, void* out, const void*
 template <int D>
 int long_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout, const float* lse,
              float* delta_ws, void* dq, void* dk, void* dv, float* dk_bcast, float* dv_bcast, int B, int T, int64_t P,
-             int C, int n_head, float scale, int kv_bcast, int tiles, cudaStream_t s) {
+             int C, int n_head, float scale, int kv_bcast, int tiles, const DropParams* drop, cudaStream_t s) {
   using namespace og::tlong;
   const long long ntask = (long long)B * n_head * P;
-  static bool attr = false;
-  if (!attr) {
+  static bool attr = false, dattr = false;
+  if (drop && !dattr) {
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_dropout_bwd_dq_kernel<D>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Geo<D>::kDqSmem));
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_dropout_bwd_dkdv_kernel<D>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Geo<D>::kDkdvSmem));
+    dattr = true;
+  }
+  if (!drop && !attr) {
     OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_bwd_dq_kernel<D>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Geo<D>::kDqSmem));
     OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_bwd_dkdv_kernel<D>,
@@ -568,9 +708,15 @@ int long_bwd(const void* q, const void* k, const void* v, const void* out, const
     attr = true;
   }
   // dQ first: it also writes delta, which the dK / dV kernel reads
-  og_temporal_attn_long_bwd_dq_kernel<D><<<(unsigned)(ntask * tiles), kThreads, Geo<D>::kDqSmem, s>>>(
-      (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)out,
-      (const __nv_bfloat16*)dout, lse, delta_ws, (__nv_bfloat16*)dq, B, T, P, C, n_head, scale, kv_bcast, tiles);
+  if (drop)
+    og_temporal_attn_long_dropout_bwd_dq_kernel<D><<<(unsigned)(ntask * tiles), kThreads, Geo<D>::kDqSmem, s>>>(
+        (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)out,
+        (const __nv_bfloat16*)dout, lse, delta_ws, (__nv_bfloat16*)dq, B, T, P, C, n_head, scale, kv_bcast, tiles,
+        *drop);
+  else
+    og_temporal_attn_long_bwd_dq_kernel<D><<<(unsigned)(ntask * tiles), kThreads, Geo<D>::kDqSmem, s>>>(
+        (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)out,
+        (const __nv_bfloat16*)dout, lse, delta_ws, (__nv_bfloat16*)dq, B, T, P, C, n_head, scale, kv_bcast, tiles);
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   // dK / dV: one pixel per CTA, or with kv_bcast contiguous pixel chunks of one (b, h), enough of them for ~4 CTAs
@@ -585,19 +731,26 @@ int long_bwd(const void* q, const void* k, const void* v, const void* out, const
     nchunk = (P + chunk - 1) / chunk;
   }
   const long long grid = (long long)B * n_head * nchunk * tiles;
-  og_temporal_attn_long_bwd_dkdv_kernel<D><<<(unsigned)grid, Geo<D>::kDkdvThreads, Geo<D>::kDkdvSmem, s>>>(
-      (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)dout, lse,
-      delta_ws, (__nv_bfloat16*)dk, (__nv_bfloat16*)dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale, kv_bcast, tiles,
-      chunk, nchunk);
+  if (drop)
+    og_temporal_attn_long_dropout_bwd_dkdv_kernel<D><<<(unsigned)grid, Geo<D>::kDkdvThreads, Geo<D>::kDkdvSmem, s>>>(
+        (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)dout, lse,
+        delta_ws, (__nv_bfloat16*)dk, (__nv_bfloat16*)dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale, kv_bcast,
+        tiles, chunk, nchunk, *drop);
+  else
+    og_temporal_attn_long_bwd_dkdv_kernel<D><<<(unsigned)grid, Geo<D>::kDkdvThreads, Geo<D>::kDkdvSmem, s>>>(
+        (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)dout, lse,
+        delta_ws, (__nv_bfloat16*)dk, (__nv_bfloat16*)dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale, kv_bcast,
+        tiles, chunk, nchunk);
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   return OG_OK;
 }
 }  // namespace
 
-extern "C" int og_temporal_attn_long_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
-                                         void* out_res, float* lse, int B, int T, int64_t P, int C, int n_head,
-                                         float scale, int kv_bcast, og_stream_t stream) {
+// og_temporal_attn_long_fwd, and og_temporal_attn_long_dropout_fwd when `drop` is given
+static int long_fwd_call(const void* q, const void* k, const void* v, void* out, const void* residual, void* out_res,
+                         float* lse, int B, int T, int64_t P, int C, int n_head, float scale, int kv_bcast,
+                         const DropParams* drop, og_stream_t stream) {
   using namespace og::tlong;
   OG_REQUIRE(q && k && v && out && lse, "temporal_attn_long_fwd: null pointer");
   OG_REQUIRE(!residual == !out_res, "temporal_attn_long_fwd: residual and out_res must be given together");
@@ -617,20 +770,36 @@ extern "C" int og_temporal_attn_long_fwd(const void* q, const void* k, const voi
   const long long grid = (long long)B * n_head * P * tiles;
   OG_REQUIRE(grid < (1LL << 31), "temporal_attn_long_fwd: too many tiles");
   const int r = dh == 64    ? long_fwd<64>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
-                                           tiles, grid, (cudaStream_t)stream)
+                                           tiles, grid, drop, (cudaStream_t)stream)
                  : dh == 128 ? long_fwd<128>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
-                                             tiles, grid, (cudaStream_t)stream)
+                                             tiles, grid, drop, (cudaStream_t)stream)
                              : long_fwd<16>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
-                                            tiles, grid, (cudaStream_t)stream);
+                                            tiles, grid, drop, (cudaStream_t)stream);
   if (r != OG_OK) return r;
   g_launches.fetch_add(1);
   return OG_OK;
 }
 
-extern "C" int og_temporal_attn_long_bwd(const void* q, const void* k, const void* v, const void* out,
-                                         const void* dout, const float* lse, float* delta_ws, void* dq, void* dk,
-                                         void* dv, float* dk_bcast, float* dv_bcast, int B, int T, int64_t P, int C,
-                                         int n_head, float scale, int kv_bcast, og_stream_t stream) {
+extern "C" int og_temporal_attn_long_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
+                                         void* out_res, float* lse, int B, int T, int64_t P, int C, int n_head,
+                                         float scale, int kv_bcast, og_stream_t stream) {
+  return long_fwd_call(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast, nullptr, stream);
+}
+
+extern "C" int og_temporal_attn_long_dropout_fwd(const void* q, const void* k, const void* v, void* out,
+                                                 const void* residual, void* out_res, float* lse, int B, int T,
+                                                 int64_t P, int C, int n_head, float scale, int kv_bcast, float p,
+                                                 const uint64_t* seed, og_stream_t stream) {
+  DropParams d;
+  if (const int r = drop_params(p, seed, "temporal_attn_long_dropout_fwd", &d)) return r;
+  return long_fwd_call(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast, &d, stream);
+}
+
+// og_temporal_attn_long_bwd, and og_temporal_attn_long_dropout_bwd when `drop` is given
+static int long_bwd_call(const void* q, const void* k, const void* v, const void* out, const void* dout,
+                         const float* lse, float* delta_ws, void* dq, void* dk, void* dv, float* dk_bcast,
+                         float* dv_bcast, int B, int T, int64_t P, int C, int n_head, float scale, int kv_bcast,
+                         const DropParams* drop, og_stream_t stream) {
   using namespace og::tlong;
   OG_REQUIRE(q && k && v && out && dout && lse && delta_ws && dq, "temporal_attn_long_bwd: null pointer");
   OG_REQUIRE(kv_bcast ? (dk_bcast && dv_bcast) : (dk && dv), "temporal_attn_long_bwd: missing dk/dv buffers");
@@ -651,9 +820,28 @@ extern "C" int og_temporal_attn_long_bwd(const void* q, const void* k, const voi
   OG_REQUIRE(ntask * tiles < (1LL << 31), "temporal_attn_long_bwd: too many tiles");
   if (dh == 16)
     return long_bwd<16>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale,
-                        kv_bcast, tiles, (cudaStream_t)stream);
+                        kv_bcast, tiles, drop, (cudaStream_t)stream);
   return dh == 64 ? long_bwd<64>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C,
-                                 n_head, scale, kv_bcast, tiles, (cudaStream_t)stream)
+                                 n_head, scale, kv_bcast, tiles, drop, (cudaStream_t)stream)
                   : long_bwd<128>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C,
-                                  n_head, scale, kv_bcast, tiles, (cudaStream_t)stream);
+                                  n_head, scale, kv_bcast, tiles, drop, (cudaStream_t)stream);
+}
+
+extern "C" int og_temporal_attn_long_bwd(const void* q, const void* k, const void* v, const void* out,
+                                         const void* dout, const float* lse, float* delta_ws, void* dq, void* dk,
+                                         void* dv, float* dk_bcast, float* dv_bcast, int B, int T, int64_t P, int C,
+                                         int n_head, float scale, int kv_bcast, og_stream_t stream) {
+  return long_bwd_call(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale,
+                       kv_bcast, nullptr, stream);
+}
+
+extern "C" int og_temporal_attn_long_dropout_bwd(const void* q, const void* k, const void* v, const void* out,
+                                                 const void* dout, const float* lse, float* delta_ws, void* dq,
+                                                 void* dk, void* dv, float* dk_bcast, float* dv_bcast, int B, int T,
+                                                 int64_t P, int C, int n_head, float scale, int kv_bcast, float p,
+                                                 const uint64_t* seed, og_stream_t stream) {
+  DropParams d;
+  if (const int r = drop_params(p, seed, "temporal_attn_long_dropout_bwd", &d)) return r;
+  return long_bwd_call(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale,
+                       kv_bcast, &d, stream);
 }

@@ -9,6 +9,10 @@ Head widths: d_head = 16, 64 or 128 (flash attention and the temporal kernels ha
 and 128 runs the tiled kernels at every clip length). Space and time attention may use different widths when n_head * d_head
 matches, e.g. SpaceTimeAttention(n_head=(2, 1), d_head=(64, 128)) or (n_head=(4, 1), d_head=(16, 64)); the FFN
 GroupNorm takes the temporal head count.
+Dropout: `dropout` (0 <= p < 1) drops attention probabilities as SDPA's dropout_p does, in both the spatial and the
+temporal attention. Like the reference, which passes dropout_p to the functional SDPA, it drops in eval mode and under
+no_grad too; set `module.dropout = 0` (read at every call) for deterministic inference. The masks come from Philox
+seeds drawn from the CUDA generator (csrc/attn_dropout.cuh), so torch.manual_seed governs them.
 The FFN is the reference's ForwardBlock: GroupNorm -> conv (-> GELU -> conv)* with `hid_dim` hidden widths, ending at
 `d_out` channels (with transpose=True, where the skip becomes the 1x1x1 ffn_skip conv); `bias` gives every FFN conv a
 bias. Hidden widths and d_out are multiples of 64.
@@ -82,8 +86,8 @@ class Attention(nn.Module):
         self.d_out = default(d_out, self.d_inp)
         if self.d_inp != hid or self.d_out != hid:
             raise NotImplementedError('only d_inp == d_out == n_head*d_head is valid at the reference HEAD')
-        if dropout != 0.0:
-            raise NotImplementedError('attention dropout is not used by any shipped blueprint')
+        if not 0.0 <= dropout < 1.0:
+            raise NotImplementedError(f'attention dropout must lie in [0, 1), not {dropout}')
         if not embed:
             raise NotImplementedError('embed=False is not used by any shipped blueprint')
         if d_head not in (16, 64, 128):
@@ -96,6 +100,7 @@ class Attention(nn.Module):
         self.scale = default(scale, n_head * d_head ** -0.5)
         self.causal = causal
         self.transpose = transpose
+        self.dropout = dropout      # read at every forward call, as SDPA's dropout_p is (attention.py:229-234)
 
     def _rows(self, video: Tensor, transpose: bool | None) -> Tuple[Tensor, bool]:
         t = default(transpose, self.transpose)
@@ -118,7 +123,7 @@ class SpatialAttention(Attention):
             raise NotImplementedError('spatial cond / mask are dead code at the reference HEAD (attention.py:290,296)')
         x, t = self._rows(video, transpose)
         y = ops.space_attention_res(x, self.embed.freq, self.norm.weight, self.norm.bias, self.n_head, self.scale,
-                                    self.norm.eps)
+                                    self.norm.eps, self.dropout)
         if not _residual:
             y = y - ops._rows_bf16(x)          # rarely used stand-alone path
         return self._back(y, t)
@@ -140,7 +145,7 @@ class TemporalAttention(Attention):
             kc = self.to_qkv.to_k(c)            # (B, T, C): a few kFLOP of host-side plumbing (torch, autograd)
             vc = self.to_qkv.to_v(c)
         y = ops.time_attention_res(x, self.embed.freq, self.norm.weight, self.norm.bias, self.n_head, self.scale,
-                                   kc, vc, self.norm.eps)
+                                   kc, vc, self.norm.eps, self.dropout)
         if not _residual:
             y = y - ops._rows_bf16(x)
         return self._back(y, t)

@@ -925,12 +925,20 @@ def _rope_table(freq: Tensor, npos: int) -> Optional[Tensor]:
     return t
 
 
+def _dropout_seed(device) -> Tensor:
+    """The seed of one attention call with dropout: one int64 (read by the kernels as a uint64) drawn from the current
+    CUDA generator on the device, so torch.manual_seed governs the masks and a CUDA-graph replay, whose capture
+    registers the generator, draws a fresh seed. The forward pass saves it for the backward pass."""
+    return torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64, device=device)
+
+
 class _SpaceAttnFn(torch.autograd.Function):
-    """y = SDPA(q, q, q; scale) + x with q = LayerNorm(RoPE2d(x)), sequences = frames (H*W tokens).
-    SpatialAttention.forward + the residual of SpaceTimeAttention.forward (attention.py:279-307, 470)."""
+    """y = SDPA(q, q, q; scale, dropout_p) + x with q = LayerNorm(RoPE2d(x)), sequences = frames (H*W tokens).
+    SpatialAttention.forward + the residual of SpaceTimeAttention.forward (attention.py:279-307, 470).
+    dropout > 0 runs og_flash_attn_dropout_fwd / bwd with a seed from _dropout_seed; 0 runs og_flash_attn_fwd / bwd."""
 
     @staticmethod
-    def forward(ctx, x, freq, gamma, beta, n_head: int, scale: float, eps: float):
+    def forward(ctx, x, freq, gamma, beta, n_head: int, scale: float, eps: float, dropout: float):
         _require_cuda(x, 'attention input')
         x = _rows_bf16(x)
         B, T, H, W, C = x.shape
@@ -942,53 +950,68 @@ class _SpaceAttnFn(torch.autograd.Function):
                   q.data_ptr(), rows, C, 1, S, _ptr(tab), s)
         y, o = torch.empty_like(x), torch.empty_like(x)
         lse = torch.empty((B * T, n_head, S), dtype=f32, device=x.device)
-        _conv_call('attn_fwd', 4.0 * B * T * S * S * C, 'og_flash_attn_fwd', q.data_ptr(), q.data_ptr(), q.data_ptr(),
-                   o.data_ptr(), x.data_ptr(), y.data_ptr(), lse.data_ptr(), B * T, S, C, n_head, scale, s)
-        ctx.cfg = (n_head, scale, eps)
-        ctx.save_for_backward(x, q, o, lse, freq, gamma)
+        seed = None
+        if dropout > 0:
+            seed = _dropout_seed(x.device)
+            _conv_call('attn_fwd', 4.0 * B * T * S * S * C, 'og_flash_attn_dropout_fwd', q.data_ptr(), q.data_ptr(),
+                       q.data_ptr(), o.data_ptr(), x.data_ptr(), y.data_ptr(), lse.data_ptr(), B * T, S, C, n_head,
+                       scale, dropout, seed.data_ptr(), s)
+        else:
+            _conv_call('attn_fwd', 4.0 * B * T * S * S * C, 'og_flash_attn_fwd', q.data_ptr(), q.data_ptr(),
+                       q.data_ptr(), o.data_ptr(), x.data_ptr(), y.data_ptr(), lse.data_ptr(), B * T, S, C, n_head,
+                       scale, s)
+        ctx.cfg = (n_head, scale, eps, dropout)
+        ctx.save_for_backward(x, q, o, lse, freq, gamma, seed)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, q, o, lse, freq, gamma = ctx.saved_tensors
-        n_head, scale, eps = ctx.cfg
+        x, q, o, lse, freq, gamma, seed = ctx.saved_tensors
+        n_head, scale, eps, dropout = ctx.cfg
         B, T, H, W, C = x.shape
         rows, S = B * T * H * W, H * W
         s = _stream()
         dy = _rows_bf16(dy)
         dq, dk, dv = torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)
         delta = torch.empty_like(lse)
-        _conv_call('attn_bwd', 10.0 * B * T * S * S * C, 'og_flash_attn_bwd', q.data_ptr(), q.data_ptr(), q.data_ptr(),
-                   o.data_ptr(), dy.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), dk.data_ptr(),
-                   dv.data_ptr(), B * T, S, C, n_head, scale, s)
+        if dropout > 0:
+            _conv_call('attn_bwd', 10.0 * B * T * S * S * C, 'og_flash_attn_dropout_bwd', q.data_ptr(), q.data_ptr(),
+                       q.data_ptr(), o.data_ptr(), dy.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(),
+                       dk.data_ptr(), dv.data_ptr(), B * T, S, C, n_head, scale, dropout, seed.data_ptr(), s)
+        else:
+            _conv_call('attn_bwd', 10.0 * B * T * S * S * C, 'og_flash_attn_bwd', q.data_ptr(), q.data_ptr(),
+                       q.data_ptr(), o.data_ptr(), dy.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(),
+                       dk.data_ptr(), dv.data_ptr(), B * T, S, C, n_head, scale, s)
         dx = torch.empty_like(x)
         dgamma = _zeros(C, f32, x.device)
         dbeta = _zeros(C, f32, x.device)
         _lib.call('og_rope_ln_bwd', x.data_ptr(), freq.data_ptr(), gamma.data_ptr(), eps, dq.data_ptr(), dk.data_ptr(),
                   dv.data_ptr(), dy.data_ptr(), dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), rows, C, 1, S,
                   _ptr(_rope_table(freq, S)), s)
-        return dx, None, dgamma, dbeta, None, None, None
+        return dx, None, dgamma, dbeta, None, None, None, None
 
 
 # Longest clip of the per-pixel temporal kernels (og_temporal_attn_fwd / bwd); longer ones take the tiled kernels.
 _TIME_ATTN_SHORT_T = 32
 
 
-def _time_attn_tiled(T: int, C: int, n_head: int) -> bool:
+def _time_attn_tiled(T: int, C: int, n_head: int, dropout: float = 0.0) -> bool:
     """Whether temporal attention runs on the tiled kernels (og_temporal_attn_long_fwd / bwd): clips longer than
-    _TIME_ATTN_SHORT_T, and every clip at d_head = 128 or 16. The per-pixel kernels do not take 128 (a lane would hold
+    _TIME_ATTN_SHORT_T, and every clip at d_head = 128 or 16. With dropout every clip does: only the tiled kernels
+    drop (og_temporal_attn_long_dropout_fwd / bwd), and they take any T >= 1. The per-pixel kernels do not take 128 (a lane would hold
     2 x 128 fp32 values). At 16 they would not be faster: timed at T = 16, B = 8, 256 pixels, 16 heads of 16 (H100
     80GB HBM3, 700 W), the per-pixel kernels instantiated at 16 took 0.124 + 0.333 ms (fwd + bwd) against the tiled
     kernels' 0.123 + 0.334 ms, and 0.111 + 0.287 ms against 0.123 + 0.252 ms with broadcast K / V."""
-    return T > _TIME_ATTN_SHORT_T or C == 128 * n_head or C == 16 * n_head
+    return dropout > 0 or T > _TIME_ATTN_SHORT_T or C == 128 * n_head or C == 16 * n_head
 
 
 class _TimeAttnFn(torch.autograd.Function):
-    """y = SDPA_causal(q, k, v; scale) + x over t for every pixel; q = LayerNorm(RoPE1d(x)); k = v = q, or the
-    projected latent-action conditioning (B, T, C) shared by all pixels (attention.py:347-371, 471)."""
+    """y = SDPA_causal(q, k, v; scale, dropout_p) + x over t for every pixel; q = LayerNorm(RoPE1d(x)); k = v = q, or
+    the projected latent-action conditioning (B, T, C) shared by all pixels (attention.py:347-371, 471).
+    dropout > 0 runs og_temporal_attn_long_dropout_fwd / bwd with a seed from _dropout_seed."""
 
     @staticmethod
-    def forward(ctx, x, freq, gamma, beta, k_cond, v_cond, n_head: int, scale: float, eps: float):
+    def forward(ctx, x, freq, gamma, beta, k_cond, v_cond, n_head: int, scale: float, eps: float, dropout: float):
         _require_cuda(x, 'attention input')
         x = _rows_bf16(x)
         B, T, H, W, C = x.shape
@@ -1004,24 +1027,33 @@ class _TimeAttnFn(torch.autograd.Function):
             vc = v_cond.detach().to(bf16).contiguous()
         else:
             kc = vc = q
-        o = lse = None
-        if not _time_attn_tiled(T, C, n_head):
+        o = lse = seed = None
+        if not _time_attn_tiled(T, C, n_head, dropout):
             _lib.call('og_temporal_attn_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), x.data_ptr(), y.data_ptr(),
                       B, T, P, C, n_head, scale, int(bcast), s)
         else:
             # the tiled kernels, which keep the attention output and log-sum-exp for the backward pass
             o = torch.empty_like(x)
             lse = torch.empty((B, n_head, P, T), dtype=f32, device=x.device)
-            _lib.call('og_temporal_attn_long_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), o.data_ptr(),
-                      x.data_ptr(), y.data_ptr(), lse.data_ptr(), B, T, P, C, n_head, scale, int(bcast), s)
-        ctx.cfg = (n_head, scale, eps, bcast)
-        ctx.save_for_backward(x, q, kc if bcast else None, vc if bcast else None, freq, gamma, o, lse)
+            if dropout > 0:
+                seed = _dropout_seed(x.device)
+                _lib.call('og_temporal_attn_long_dropout_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), o.data_ptr(),
+                          x.data_ptr(), y.data_ptr(), lse.data_ptr(), B, T, P, C, n_head, scale, int(bcast), dropout,
+                          seed.data_ptr(), s)
+            else:
+                _lib.call('og_temporal_attn_long_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), o.data_ptr(),
+                          x.data_ptr(), y.data_ptr(), lse.data_ptr(), B, T, P, C, n_head, scale, int(bcast), s)
+        ctx.cfg = (n_head, scale, eps, bcast, dropout)
+        ctx.save_for_backward(x, q, kc if bcast else None, vc if bcast else None, freq, gamma, o, lse, seed)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, q, kc, vc, freq, gamma, o, lse = ctx.saved_tensors
-        n_head, scale, eps, bcast = ctx.cfg
+        x, q, kc, vc, freq, gamma, o, lse, seed = ctx.saved_tensors
+        n_head, scale, eps, bcast, dropout = ctx.cfg
+        # the tiled backward, with the forward's dropout seed when it dropped
+        long_bwd = 'og_temporal_attn_long_dropout_bwd' if dropout > 0 else 'og_temporal_attn_long_bwd'
+        drop_args = (dropout, seed.data_ptr()) if dropout > 0 else ()
         B, T, H, W, C = x.shape
         P = H * W
         s = _stream()
@@ -1036,9 +1068,9 @@ class _TimeAttnFn(torch.autograd.Function):
                 _lib.call('og_temporal_attn_bwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), dy.data_ptr(),
                           dq.data_ptr(), None, None, dkc.data_ptr(), dvc.data_ptr(), B, T, P, C, n_head, scale, 1, s)
             else:
-                _lib.call('og_temporal_attn_long_bwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), o.data_ptr(),
+                _lib.call(long_bwd, q.data_ptr(), kc.data_ptr(), vc.data_ptr(), o.data_ptr(),
                           dy.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), None, None,
-                          dkc.data_ptr(), dvc.data_ptr(), B, T, P, C, n_head, scale, 1, s)
+                          dkc.data_ptr(), dvc.data_ptr(), B, T, P, C, n_head, scale, 1, *drop_args, s)
             g1 = g2 = None
         else:
             dk, dv = torch.empty_like(x), torch.empty_like(x)
@@ -1046,9 +1078,9 @@ class _TimeAttnFn(torch.autograd.Function):
                 _lib.call('og_temporal_attn_bwd', q.data_ptr(), q.data_ptr(), q.data_ptr(), dy.data_ptr(),
                           dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), None, None, B, T, P, C, n_head, scale, 0, s)
             else:
-                _lib.call('og_temporal_attn_long_bwd', q.data_ptr(), q.data_ptr(), q.data_ptr(), o.data_ptr(),
+                _lib.call(long_bwd, q.data_ptr(), q.data_ptr(), q.data_ptr(), o.data_ptr(),
                           dy.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(),
-                          dk.data_ptr(), dv.data_ptr(), None, None, B, T, P, C, n_head, scale, 0, s)
+                          dk.data_ptr(), dv.data_ptr(), None, None, B, T, P, C, n_head, scale, 0, *drop_args, s)
             g1, g2 = dk, dv
         dx = torch.empty_like(x)
         dgamma = _zeros(C, f32, x.device)
@@ -1056,7 +1088,7 @@ class _TimeAttnFn(torch.autograd.Function):
         _lib.call('og_rope_ln_bwd', x.data_ptr(), freq.data_ptr(), gamma.data_ptr(), eps, dq.data_ptr(), _ptr(g1),
                   _ptr(g2), dy.data_ptr(), dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), B * T * P, C, P, T,
                   _ptr(_rope_table(freq, T)), s)
-        return dx, None, dgamma, dbeta, dkc, dvc, None, None, None
+        return dx, None, dgamma, dbeta, dkc, dvc, None, None, None, None
 
 
 class _FfnFn(torch.autograd.Function):
@@ -1184,12 +1216,12 @@ class _FfnFn(torch.autograd.Function):
         return (dx, dgw, dgb, None, None, None, dskip_w, dskip_b, *grads)
 
 
-def space_attention_res(x, freq, gamma, beta, n_head, scale, eps=1e-5):
-    return _SpaceAttnFn.apply(x, freq, gamma, beta, n_head, float(scale), float(eps))
+def space_attention_res(x, freq, gamma, beta, n_head, scale, eps=1e-5, dropout=0.0):
+    return _SpaceAttnFn.apply(x, freq, gamma, beta, n_head, float(scale), float(eps), float(dropout))
 
 
-def time_attention_res(x, freq, gamma, beta, n_head, scale, k_cond=None, v_cond=None, eps=1e-5):
-    return _TimeAttnFn.apply(x, freq, gamma, beta, k_cond, v_cond, n_head, float(scale), float(eps))
+def time_attention_res(x, freq, gamma, beta, n_head, scale, k_cond=None, v_cond=None, eps=1e-5, dropout=0.0):
+    return _TimeAttnFn.apply(x, freq, gamma, beta, k_cond, v_cond, n_head, float(scale), float(eps), float(dropout))
 
 
 def ffn_res(x, gn_w, gn_b, convs, num_groups, eps=1e-5, skip_w=None, skip_b=None):
