@@ -310,6 +310,24 @@ int og_lfq_bwd(const float* x, int ldx, int64_t ntok, int D, float beta, float w
                const float* gloss, const float* dout, int ld_dout, float* dx_f32, void* dx_bf16, int ld_dx,
                void* workspace, og_stream_t stream);
 
+/* Several codebooks (num_codebook = n_codebook = C >= 1, quantization.py:39-133). x: fp32 [ntok][ldx], ldx >= C*D;
+ * token n's first C*D columns are C independent D-wide rows (n, c). out_f32 [ntok][C*D], out_bf16 [ntok][ld_bf16]
+ * (ld_bf16 >= C*D, zero padded), idx int64 [ntok][C] (MSB-first bits of slice c). The reference's codebook holds
+ * each of the 2^D codes C times, so its softmax is q/C per copy, q the row's own distribution; with R = ntok*C rows,
+ * eps' = C * 1e-6 and H'(p) = -sum_j p_j log max(p_j, eps'), training writes
+ *   loss[0] = w_entropy * (sum_r H'(q_r) / R + w_div * mean_c H'(mean_n q_(n,c)) + (1 + w_div) log C)
+ *           + w_commit * sum (x - sign x)^2 / (R D).
+ * C = 1 is og_lfq_fwd / og_lfq_bwd exactly. D in [1, 20], C in [1, 65535] and ntok * C <= INT_MAX, else -1;
+ * og_lfq_multi_workspace_bytes returns 0 for such arguments. dx_f32 / dx_bf16 / dout as in og_lfq_bwd, with
+ * ld_dx, ld_dout >= C*D and columns >= C*D of dx zeroed. */
+size_t og_lfq_multi_workspace_bytes(int64_t ntok, int D, int n_codebook);
+int og_lfq_multi_fwd(const float* x, int ldx, int64_t ntok, int D, int n_codebook, float beta, int training,
+                     float w_commit, float w_entropy, float w_div, float* out_f32, void* out_bf16, int ld_bf16,
+                     int64_t* idx, float* loss, void* workspace, og_stream_t stream);
+int og_lfq_multi_bwd(const float* x, int ldx, int64_t ntok, int D, int n_codebook, float beta, float w_commit,
+                     float w_entropy, const float* gloss, const float* dout, int ld_dout, float* dx_f32, void* dx_bf16,
+                     int ld_dx, void* workspace, og_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * factored space-time attention (genie/module/attention.py)
  * All tensors are NDHWC rows [B*T*H*W][C] bf16; a spatial sequence is the H*W rows of one frame, a

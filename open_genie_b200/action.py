@@ -53,6 +53,11 @@ class LatentAction(nn.Module):
                  lfq_frac_sample: float = 1., lfq_commit_weight: float = 0.25, lfq_entropy_weight: float = 0.1,
                  lfq_diversity_weight: float = 1., quant_loss_weight: float = 1.) -> None:
         super().__init__()
+        if n_codebook != 1:
+            # the reference's quantiser here projects from 2^d_codebook * n_codebook inputs and cannot run; this
+            # class feeds it the d_codebook-wide output of to_act, which n_codebook > 1 codebooks cannot split
+            raise NotImplementedError(f'LatentAction supports n_codebook = 1 only (got {n_codebook}): the action '
+                                      f'head to_act emits d_codebook = {d_codebook} values per frame, one codebook')
         if isinstance(inp_shape, int):
             inp_shape = (inp_shape, inp_shape)
         self.proj_in = CausalConv3d(inp_channels, out_channels=n_embd, kernel_size=ker_size)

@@ -15,6 +15,13 @@
 //   * backward needs, per token, sum_j p_j G_j c_jd with G = dL/dp: the per-sample part is again a
 //     pair loop, the batch part reduces to two more small GEMMs (U = B G2^T, V = A G2).
 // The op is bound by SFU/FP32 throughput, not HBM: algorithmic bytes are N*D*(4+2+8) only.
+//
+// Several codebooks (num_codebook = C > 1, quantization.py:52,74,90): token n's C*D inputs are C rows r = n*C + c of
+// D inputs each, quantised independently. The reference's codebook repeats each of the 2^D sign codes C times, so
+// its softmax gives every code q_j / C, C times over, where q is the row's factorised distribution above. Hence
+//   H(p) = H_{C eps}(q) + log C   per row,   and   H(avg_c) = H_{C eps}(mean_n q_(n,c)) + log C   per codebook,
+// i.e. the kernels below run per row with the clamp at eps' = C * eps, the batch mean (and U, V) once per codebook,
+// and the loss adds the constant (1 + w_div) log C. With C = 1 every formula is the single-codebook one.
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 
@@ -62,21 +69,25 @@ __device__ __forceinline__ void build_ab(const float* __restrict__ xr, const Lfq
 }
 
 // ------------------------------------------------------------------------------------------------
-// forward, one block per token
+// forward, one block per row r = n * C + c (token n, codebook c)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kLfqThreads)
-    og_lfq_fwd_kernel(const float* __restrict__ x, int ldx, const LfqDims d, float beta, int training,
-                      float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16, int ld_bf16,
+    og_lfq_fwd_kernel(const float* __restrict__ x, int ldx, const LfqDims d, int C, float eps, float beta,
+                      int training, float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16, int ld_bf16,
                       long long* __restrict__ idx, float* __restrict__ A, float* __restrict__ B,
-                      float* __restrict__ stats /* [0]=sum H_n, [1]=sum (x-q)^2 */) {
+                      float* __restrict__ stats /* [0]=sum H_r, [1]=sum (x-q)^2 */) {
   extern __shared__ float sh[];
   float* sp = sh;
   float* sm = sp + 32;
   float* ws = sm + 32;
   float* a = ws + 32;
   float* b = a + d.H;
-  const long long n = blockIdx.x;
-  const float* xr = x + n * ldx;
+  const long long r = blockIdx.x;
+  const long long n = r / C;
+  const int col0 = (int)(r - n * C) * d.D;  // this row's first column in the token's C*D
+  const float* xr = x + n * ldx + col0;
+  // the last codebook's row also zero-fills the bf16 pad columns [C*D, ld_bf16)
+  const int ncol = (col0 + d.D == C * d.D && ld_bf16 - col0 > d.D) ? ld_bf16 - col0 : d.D;
 
   // quantise / indices / straight-through output (lines 97-101)
   float commit = 0.f;
@@ -84,9 +95,9 @@ __global__ void __launch_bounds__(kLfqThreads)
     long long bits = 0;
     if (threadIdx.x == 0) {
       for (int i = 0; i < d.D; ++i) bits |= (long long)(xr[i] > 0.f) << (d.D - 1 - i);
-      idx[n] = bits;
+      idx[r] = bits;
     }
-    for (int i = threadIdx.x; i < ld_bf16 || i < d.D; i += 32) {
+    for (int i = threadIdx.x; i < ncol; i += 32) {
       float code = 0.f;
       if (i < d.D) {
         const float v = xr[i];
@@ -94,16 +105,16 @@ __global__ void __launch_bounds__(kLfqThreads)
         // training: x + (sign(x) - x), evaluated in this order like the reference's STE (not bit-equal to sign(x))
         code = training ? __fadd_rn(v, __fsub_rn(q, v)) : q;
         commit += (v - q) * (v - q);
-        if (out_f32) out_f32[n * d.D + i] = code;
+        if (out_f32) out_f32[r * d.D + i] = code;
       }
-      if (out_bf16 && i < ld_bf16) out_bf16[n * ld_bf16 + i] = __float2bfloat16_rn(code);
+      if (out_bf16 && col0 + i < ld_bf16) out_bf16[n * ld_bf16 + col0 + i] = __float2bfloat16_rn(code);
     }
   }
   if (!training) return;
 
   build_ab(xr, d, beta, sp, sm, a, b);
-  for (int h = threadIdx.x; h < d.H; h += blockDim.x) A[n * d.H + h] = a[h];
-  for (int l = threadIdx.x; l < d.L; l += blockDim.x) B[n * d.L + l] = b[l];
+  for (int h = threadIdx.x; h < d.H; h += blockDim.x) A[r * d.H + h] = a[h];
+  for (int l = threadIdx.x; l < d.L; l += blockDim.x) B[r * d.L + l] = b[l];
 
   float bmax = 0.f, bsum = 0.f, asum = 0.f;
   for (int l = 0; l < d.L; ++l) {
@@ -111,14 +122,14 @@ __global__ void __launch_bounds__(kLfqThreads)
     bsum += b[l];
   }
   for (int h = 0; h < d.H; ++h) asum += a[h];
-  const float log_eps = logf(kEps);
+  const float log_eps = logf(eps);
   float acc = 0.f;
   for (int h = 0; h < d.H; ++h) {
     const float ah = a[h];
-    if (ah * bmax < kEps) continue;  // block-uniform
+    if (ah * bmax < eps) continue;  // block-uniform
     for (int l = threadIdx.x; l < d.L; l += blockDim.x) {
       const float p = ah * b[l];
-      if (p >= kEps) acc += p * (logf(p) - log_eps);
+      if (p >= eps) acc += p * (logf(p) - log_eps);
     }
   }
   const float tot = block_sum(acc, ws);
@@ -129,42 +140,51 @@ __global__ void __launch_bounds__(kLfqThreads)
   }
 }
 
-// entropy of the batch-mean distribution + G2 = dL/d(avg) (scaled) ; single block, then final loss
+// entropy of each codebook's batch-mean distribution + G2 = dL/d(avg) (scaled); single block, then the final loss
+//   loss = w_e (sum_r H_r / R + w_div mean_c H(avg_c) + (1 + w_div) log C) + w_c sum (x - q)^2 / (R D)
 __global__ void __launch_bounds__(1024)
-    og_lfq_avg_kernel(const float* __restrict__ avg, long long ncodes, long long ntok, int D, float w_commit,
-                      float w_entropy, float w_div, float* __restrict__ g2, float* __restrict__ stats,
+    og_lfq_avg_kernel(const float* __restrict__ avg, long long ncodes, int C, long long nrow, int D, float eps,
+                      float w_commit, float w_entropy, float w_div, float* __restrict__ g2, float* __restrict__ stats,
                       float* __restrict__ loss) {
   __shared__ float ws[32];
-  const float log_eps = logf(kEps);
-  float acc = 0.f;
-  const float gs = w_entropy * w_div / (float)ntok;
-  for (long long j = threadIdx.x; j < ncodes; j += blockDim.x) {
-    const float p = avg[j];
-    const float lp = logf(fmaxf(p, kEps));
-    acc += p * lp;
-    if (g2) g2[j] = -(lp + (p >= kEps ? 1.f : 0.f)) * gs;
+  const float gs = w_entropy * w_div / (float)nrow;
+  float h_sum = 0.f;
+  for (int c = 0; c < C; ++c) {
+    const float* avg_c = avg + c * ncodes;
+    float acc = 0.f;
+    for (long long j = threadIdx.x; j < ncodes; j += blockDim.x) {
+      const float p = avg_c[j];
+      const float lp = logf(fmaxf(p, eps));
+      acc += p * lp;
+      if (g2) g2[c * ncodes + j] = -(lp + (p >= eps ? 1.f : 0.f)) * gs;
+    }
+    h_sum += -block_sum(acc, ws);
   }
-  const float tot = block_sum(acc, ws);
   if (threadIdx.x == 0) {
-    const float h_avg = -tot;
+    const float h_avg = h_sum / (float)C;
     stats[2] = h_avg;
-    const float inp_ent = stats[0] / (float)ntok;
-    const float commit = stats[1] / ((float)ntok * (float)D);
-    loss[0] = (inp_ent + w_div * h_avg) * w_entropy + commit * w_commit;
+    const float inp_ent = stats[0] / (float)nrow;
+    const float commit = stats[1] / ((float)nrow * (float)D);
+    float ent = inp_ent + w_div * h_avg;
+    if (C > 1) ent += (1.f + w_div) * logf((float)C);  // the duplicated codes; no gradient
+    loss[0] = ent * w_entropy + commit * w_commit;
   }
-  (void)log_eps;
 }
 
 // ------------------------------------------------------------------------------------------------
 // generic small fp32 GEMM on CUDA cores: C[i][j] = alpha * sum_k X[i*sxi + k*sxk] * Y[j*syj + k*syk]
-// 64x64 tile, 16-deep, 256 threads (4x4 per thread).
+// 64x64 tile, 16-deep, 256 threads (4x4 per thread). Batched over blockIdx.z (one codebook each): X, Y and C
+// start sxz, syz and scz elements further per batch.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-    og_sgemm_kernel(const float* __restrict__ X, long long sxi, long long sxk, const float* __restrict__ Y,
-                    long long syj, long long syk, float* __restrict__ C, long long ldc, int M, int N, int K,
-                    float alpha) {
+    og_sgemm_kernel(const float* __restrict__ X, long long sxi, long long sxk, long long sxz,
+                    const float* __restrict__ Y, long long syj, long long syk, long long syz, float* __restrict__ C,
+                    long long ldc, long long scz, int M, int N, int K, float alpha) {
   __shared__ float xs[16][65];
   __shared__ float ys[16][65];
+  X += blockIdx.z * sxz;
+  Y += blockIdx.z * syz;
+  C += blockIdx.z * scz;
   const int i0 = blockIdx.y * 64, j0 = blockIdx.x * 64;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   float acc[4][4] = {};
@@ -208,14 +228,14 @@ __global__ void __launch_bounds__(256)
 }
 
 // ------------------------------------------------------------------------------------------------
-// backward, one block per token
-//   dx[d] = gl * 2 beta * ( M[d] - Gbar * tanh[d] ) + gl * w_c * 2 (x - q) / (N D) + dout[d]
+// backward, one block per row r = n * C + c (token n, codebook c), R = N C rows
+//   dx[d] = gl * 2 beta * ( M[d] - Gbar * tanh[d] ) + gl * w_c * 2 (x - q) / (R D) + dout[d]
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kLfqThreads)
-    og_lfq_bwd_kernel(const float* __restrict__ x, int ldx, const LfqDims d, float beta, long long ntok,
-                      float w_commit, float w_entropy, const float* __restrict__ U, const float* __restrict__ Vm,
-                      const float* __restrict__ gloss, const float* __restrict__ dout, int ld_dout,
-                      float* __restrict__ dx_f32, __nv_bfloat16* __restrict__ dx_bf16, int ld_dx) {
+    og_lfq_bwd_kernel(const float* __restrict__ x, int ldx, const LfqDims d, int C, float eps, float beta,
+                      long long nrow, float w_commit, float w_entropy, const float* __restrict__ U,
+                      const float* __restrict__ Vm, const float* __restrict__ gloss, const float* __restrict__ dout,
+                      int ld_dout, float* __restrict__ dx_f32, __nv_bfloat16* __restrict__ dx_bf16, int ld_dx) {
   extern __shared__ float sh[];
   float* sp = sh;
   float* sm = sp + 32;
@@ -223,13 +243,15 @@ __global__ void __launch_bounds__(kLfqThreads)
   float* red = ws + 32;  // [kMaxD + 1] reduced sums
   float* a = red + 32;
   float* b = a + d.H;
-  const long long n = blockIdx.x;
-  const float* xr = x + n * ldx;
+  const long long r = blockIdx.x;
+  const long long n = r / C;
+  const int col0 = (int)(r - n * C) * d.D;
+  const float* xr = x + n * ldx + col0;
   build_ab(xr, d, beta, sp, sm, a, b);
 
   float bmax = 0.f;
   for (int l = 0; l < d.L; ++l) bmax = fmaxf(bmax, b[l]);
-  const float log_eps = logf(kEps);
+  const float log_eps = logf(eps);
 
   // per-sample part: val = p (log p - log eps + 1) over pairs with p >= eps
   float m[kMaxD];
@@ -238,10 +260,10 @@ __global__ void __launch_bounds__(kLfqThreads)
   float w1 = 0.f;
   for (int h = 0; h < d.H; ++h) {
     const float ah = a[h];
-    if (ah * bmax < kEps) continue;
+    if (ah * bmax < eps) continue;
     for (int l = threadIdx.x; l < d.L; l += blockDim.x) {
       const float p = ah * b[l];
-      if (p >= kEps) {
+      if (p >= eps) {
         const float val = p * (logf(p) - log_eps + 1.f);
         w1 += val;
 #pragma unroll
@@ -260,14 +282,14 @@ __global__ void __launch_bounds__(kLfqThreads)
 #pragma unroll
   for (int i = 0; i < kMaxD; ++i) m2[i] = 0.f;
   for (int h = threadIdx.x; h < d.H; h += blockDim.x) {
-    const float au = a[h] * U[n * d.H + h];
+    const float au = a[h] * U[r * d.H + h];
     g2bar += au;
 #pragma unroll
     for (int i = 0; i < kMaxD; ++i)
       if (i < d.D1) m2[i] += ((h >> (d.D1 - 1 - i)) & 1) ? au : -au;
   }
   for (int l = threadIdx.x; l < d.L; l += blockDim.x) {
-    const float bv = b[l] * Vm[n * d.L + l];
+    const float bv = b[l] * Vm[r * d.L + l];
 #pragma unroll
     for (int i = 0; i < kMaxD; ++i)
       if (i >= d.D1 && i < d.D) m2[i] += ((l >> (d.D - 1 - i)) & 1) ? bv : -bv;
@@ -275,7 +297,7 @@ __global__ void __launch_bounds__(kLfqThreads)
   const float w1s = block_sum(w1, ws);
   const float g2s = block_sum(g2bar, ws);
   const float gl = gloss ? *gloss : 1.f;
-  const float we_n = w_entropy / (float)ntok;
+  const float we_n = w_entropy / (float)nrow;
   const float gbar = -we_n * (log_eps + w1s) + g2s;
 #pragma unroll
   for (int i = 0; i < kMaxD; ++i) {
@@ -291,15 +313,16 @@ __global__ void __launch_bounds__(kLfqThreads)
     const float v = xr[i];
     const float q = (v > 0.f) ? 1.f : ((v < 0.f) ? -1.f : 0.f);
     float g = gl * 2.f * beta * (red[i] - gbar * (sp[i] - sm[i]));
-    g += gl * w_commit * 2.f * (v - q) / ((float)ntok * (float)d.D);
-    if (dout) g += dout[n * ld_dout + i];
-    if (dx_f32) dx_f32[n * ld_dx + i] = g;
-    if (dx_bf16) dx_bf16[n * ld_dx + i] = __float2bfloat16_rn(g);
+    g += gl * w_commit * 2.f * (v - q) / ((float)nrow * (float)d.D);
+    if (dout) g += dout[n * ld_dout + col0 + i];
+    if (dx_f32) dx_f32[n * ld_dx + col0 + i] = g;
+    if (dx_bf16) dx_bf16[n * ld_dx + col0 + i] = __float2bfloat16_rn(g);
   }
+  if (col0 + d.D != C * d.D) return;  // the last codebook's row zeroes the pad columns [C*D, ld_dx)
   if (dx_bf16)
-    for (int i = d.D + threadIdx.x; i < ld_dx; i += blockDim.x) dx_bf16[n * ld_dx + i] = __float2bfloat16_rn(0.f);
+    for (int i = C * d.D + threadIdx.x; i < ld_dx; i += blockDim.x) dx_bf16[n * ld_dx + i] = __float2bfloat16_rn(0.f);
   if (dx_f32)
-    for (int i = d.D + threadIdx.x; i < ld_dx; i += blockDim.x) dx_f32[n * ld_dx + i] = 0.f;
+    for (int i = C * d.D + threadIdx.x; i < ld_dx; i += blockDim.x) dx_f32[n * ld_dx + i] = 0.f;
 }
 
 static LfqDims make_dims(int D) {
@@ -312,10 +335,90 @@ static LfqDims make_dims(int D) {
   return d;
 }
 
-static int launch_sgemm(const float* X, long long sxi, long long sxk, const float* Y, long long syj, long long syk,
-                        float* C, long long ldc, int M, int N, int K, float alpha, cudaStream_t s) {
-  dim3 grid((N + 63) / 64, (M + 63) / 64);
-  og_sgemm_kernel<<<grid, 256, 0, s>>>(X, sxi, sxk, Y, syj, syk, C, ldc, M, N, K, alpha);
+static int launch_sgemm(const float* X, long long sxi, long long sxk, long long sxz, const float* Y, long long syj,
+                        long long syk, long long syz, float* C, long long ldc, long long scz, int M, int N, int K,
+                        int batch, float alpha, cudaStream_t s) {
+  dim3 grid((N + 63) / 64, (M + 63) / 64, batch);
+  og_sgemm_kernel<<<grid, 256, 0, s>>>(X, sxi, sxk, sxz, Y, syj, syk, syz, C, ldc, scz, M, N, K, alpha);
+  OG_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1);
+  return OG_OK;
+}
+
+// Workspace (floats), R = ntok * C rows: A[R*H] B[R*L] U[R*H] V[R*L] avg[C*2^D] g2[C*2^D] stats[4]
+static size_t lfq_workspace_floats(int64_t ntok, const LfqDims& d, int C) {
+  const size_t rows = (size_t)ntok * (size_t)C;
+  return rows * (size_t)(d.H + d.L) * 2 + ((size_t)C << d.D) * 2 + 4;
+}
+
+struct LfqWorkspace {
+  float *A, *B, *U, *V, *avg, *g2, *stats;
+};
+
+static LfqWorkspace lfq_workspace(void* workspace, int64_t ntok, const LfqDims& d, int C) {
+  const size_t rows = (size_t)ntok * (size_t)C;
+  LfqWorkspace w;
+  w.A = reinterpret_cast<float*>(workspace);
+  w.B = w.A + rows * d.H;
+  w.U = w.B + rows * d.L;
+  w.V = w.U + rows * d.H;
+  w.avg = w.V + rows * d.L;
+  w.g2 = w.avg + ((size_t)C << d.D);
+  w.stats = w.g2 + ((size_t)C << d.D);
+  return w;
+}
+
+// forward on validated arguments: 1 + 3 launches in training (stats memset, rows, batch means, entropy + loss)
+static int lfq_fwd(const float* x, int ldx, int64_t ntok, int D, int C, float beta, int training, float w_commit,
+                   float w_entropy, float w_div, float* out_f32, void* out_bf16, int ld_bf16, int64_t* idx,
+                   float* loss, void* workspace, cudaStream_t s) {
+  const LfqDims d = make_dims(D);
+  const float eps = kEps * (float)C;
+  const long long nrow = (long long)ntok * C;
+  LfqWorkspace w = {};
+  if (training) {
+    w = lfq_workspace(workspace, ntok, d, C);
+    OG_CHECK_CUDA(cudaMemsetAsync(w.stats, 0, 4 * sizeof(float), s));
+  }
+  const size_t smem = sizeof(float) * (96 + d.H + d.L);
+  og_lfq_fwd_kernel<<<(unsigned)nrow, kLfqThreads, smem, s>>>(x, ldx, d, C, eps, beta, training, out_f32,
+                                                              (__nv_bfloat16*)out_bf16, ld_bf16, (long long*)idx, w.A,
+                                                              w.B, w.stats);
+  OG_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1);
+  if (!training) return OG_OK;
+  // avg_c[h][l] = (1/N) sum_n A[n*C+c][h] B[n*C+c][l], one batch per codebook
+  const long long ncodes = 1LL << D;
+  int r = launch_sgemm(w.A, 1, (long long)C * d.H, d.H, w.B, 1, (long long)C * d.L, d.L, w.avg, d.L, ncodes, d.H,
+                       d.L, (int)ntok, C, 1.f / (float)ntok, s);
+  if (r != OG_OK) return r;
+  og_lfq_avg_kernel<<<1, 1024, 0, s>>>(w.avg, ncodes, C, nrow, D, eps, w_commit, w_entropy, w_div, w.g2, w.stats,
+                                       loss);
+  OG_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1);
+  return OG_OK;
+}
+
+// backward on validated arguments: 3 launches (U, V, rows)
+static int lfq_bwd(const float* x, int ldx, int64_t ntok, int D, int C, float beta, float w_commit, float w_entropy,
+                   const float* gloss, const float* dout, int ld_dout, float* dx_f32, void* dx_bf16, int ld_dx,
+                   void* workspace, cudaStream_t s) {
+  const LfqDims d = make_dims(D);
+  const float eps = kEps * (float)C;
+  const long long nrow = (long long)ntok * C;
+  const LfqWorkspace w = lfq_workspace(workspace, ntok, d, C);
+  const long long ncodes = 1LL << D;
+  // per codebook c, over its rows r = n*C + c:  U[r][h] = sum_l B[r][l] g2_c[h][l] ;  V[r][l] = sum_h A[r][h] g2_c[h][l]
+  int r = launch_sgemm(w.B, (long long)C * d.L, 1, d.L, w.g2, d.L, 1, ncodes, w.U, (long long)C * d.H, d.H, (int)ntok,
+                       d.H, d.L, C, 1.f, s);
+  if (r != OG_OK) return r;
+  r = launch_sgemm(w.A, (long long)C * d.H, 1, d.H, w.g2, 1, d.L, ncodes, w.V, (long long)C * d.L, d.L, (int)ntok, d.L,
+                   d.H, C, 1.f, s);
+  if (r != OG_OK) return r;
+  const size_t smem = sizeof(float) * (128 + d.H + d.L);
+  og_lfq_bwd_kernel<<<(unsigned)nrow, kLfqThreads, smem, s>>>(x, ldx, d, C, eps, beta, nrow, w_commit, w_entropy,
+                                                              w.U, w.V, gloss, dout, ld_dout, dx_f32,
+                                                              (__nv_bfloat16*)dx_bf16, ld_dx);
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   return OG_OK;
@@ -327,46 +430,17 @@ using namespace og;
 
 extern "C" size_t og_lfq_workspace_bytes(int64_t ntok, int D) {
   if (D < 1 || D > kMaxD) return 0;
-  const LfqDims d = make_dims(D);
-  // A, B, U, V (per token) + avg, g2 (per code) + stats[4]
-  return sizeof(float) * ((size_t)ntok * (d.H + d.L) * 2 + ((size_t)1 << D) * 2 + 4);
+  return sizeof(float) * lfq_workspace_floats(ntok, make_dims(D), 1);
 }
 
-/* Workspace layout (floats): A[ntok*H] B[ntok*L] U[ntok*H] V[ntok*L] avg[2^D] g2[2^D] stats[4] */
 extern "C" int og_lfq_fwd(const float* x, int ldx, int64_t ntok, int D, float beta, int training, float w_commit,
                           float w_entropy, float w_div, float* out_f32, void* out_bf16, int ld_bf16, int64_t* idx,
                           float* loss, void* workspace, og_stream_t stream) {
   OG_REQUIRE(x && idx && ntok > 0, "lfq_fwd: bad arguments");
   OG_REQUIRE(D >= 1 && D <= kMaxD, "lfq_fwd: codebook_dim=%d outside [1,%d]", D, kMaxD);
   OG_REQUIRE(!training || (loss && workspace), "lfq_fwd: training needs loss and workspace");
-  cudaStream_t s = (cudaStream_t)stream;
-  const LfqDims d = make_dims(D);
-  float* ws = reinterpret_cast<float*>(workspace);
-  float *A = nullptr, *B = nullptr, *avg = nullptr, *g2 = nullptr, *stats = nullptr;
-  if (training) {
-    A = ws;
-    B = A + ntok * d.H;
-    float* U = B + ntok * d.L;
-    float* V = U + ntok * d.H;
-    avg = V + ntok * d.L;
-    g2 = avg + ((size_t)1 << D);
-    stats = g2 + ((size_t)1 << D);
-    OG_CHECK_CUDA(cudaMemsetAsync(stats, 0, 4 * sizeof(float), s));
-  }
-  const size_t smem = sizeof(float) * (96 + d.H + d.L);
-  og_lfq_fwd_kernel<<<(unsigned)ntok, kLfqThreads, smem, s>>>(x, ldx, d, beta, training, out_f32,
-                                                             (__nv_bfloat16*)out_bf16, ld_bf16, (long long*)idx, A, B,
-                                                             stats);
-  OG_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1);
-  if (!training) return OG_OK;
-  // avg[h][l] = (1/N) sum_n A[n][h] B[n][l]
-  int r = launch_sgemm(A, 1, d.H, B, 1, d.L, avg, d.L, d.H, d.L, (int)ntok, 1.f / (float)ntok, s);
-  if (r != OG_OK) return r;
-  og_lfq_avg_kernel<<<1, 1024, 0, s>>>(avg, (long long)1 << D, ntok, D, w_commit, w_entropy, w_div, g2, stats, loss);
-  OG_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1);
-  return OG_OK;
+  return lfq_fwd(x, ldx, ntok, D, 1, beta, training, w_commit, w_entropy, w_div, out_f32, out_bf16, ld_bf16, idx, loss,
+                 workspace, (cudaStream_t)stream);
 }
 
 extern "C" int og_lfq_bwd(const float* x, int ldx, int64_t ntok, int D, float beta, float w_commit, float w_entropy,
@@ -374,25 +448,49 @@ extern "C" int og_lfq_bwd(const float* x, int ldx, int64_t ntok, int D, float be
                           void* workspace, og_stream_t stream) {
   OG_REQUIRE(x && workspace && (dx_f32 || dx_bf16) && ld_dx >= D, "lfq_bwd: bad arguments");
   OG_REQUIRE(D >= 1 && D <= kMaxD, "lfq_bwd: codebook_dim=%d outside [1,%d]", D, kMaxD);
-  cudaStream_t s = (cudaStream_t)stream;
-  const LfqDims d = make_dims(D);
-  float* ws = reinterpret_cast<float*>(workspace);
-  float* A = ws;
-  float* B = A + ntok * d.H;
-  float* U = B + ntok * d.L;
-  float* V = U + ntok * d.H;
-  float* avg = V + ntok * d.L;
-  float* g2 = avg + ((size_t)1 << D);
-  (void)avg;
-  // U[n][h] = sum_l B[n][l] g2[h][l] ;  V[n][l] = sum_h A[n][h] g2[h][l]
-  int r = launch_sgemm(B, d.L, 1, g2, d.L, 1, U, d.H, (int)ntok, d.H, d.L, 1.f, s);
-  if (r != OG_OK) return r;
-  r = launch_sgemm(A, d.H, 1, g2, 1, d.L, V, d.L, (int)ntok, d.L, d.H, 1.f, s);
-  if (r != OG_OK) return r;
-  const size_t smem = sizeof(float) * (128 + d.H + d.L);
-  og_lfq_bwd_kernel<<<(unsigned)ntok, kLfqThreads, smem, s>>>(x, ldx, d, beta, ntok, w_commit, w_entropy, U, V, gloss,
-                                                             dout, ld_dout, dx_f32, (__nv_bfloat16*)dx_bf16, ld_dx);
-  OG_CHECK_CUDA(cudaGetLastError());
-  g_launches.fetch_add(1);
-  return OG_OK;
+  return lfq_bwd(x, ldx, ntok, D, 1, beta, w_commit, w_entropy, gloss, dout, ld_dout, dx_f32, dx_bf16, ld_dx, workspace,
+                 (cudaStream_t)stream);
+}
+
+// rows r = n * C + c index the grid and must fit an int; each codebook is one SGEMM batch (grid z <= 65535)
+static constexpr int kMaxCodebooks = 65535;
+static bool lfq_rows_fit(int64_t ntok, int C) {
+  return ntok > 0 && C >= 1 && C <= kMaxCodebooks && ntok <= INT_MAX / C;
+}
+
+extern "C" size_t og_lfq_multi_workspace_bytes(int64_t ntok, int D, int n_codebook) {
+  if (D < 1 || D > kMaxD || !lfq_rows_fit(ntok, n_codebook)) return 0;
+  return sizeof(float) * lfq_workspace_floats(ntok, make_dims(D), n_codebook);
+}
+
+extern "C" int og_lfq_multi_fwd(const float* x, int ldx, int64_t ntok, int D, int n_codebook, float beta, int training,
+                                float w_commit, float w_entropy, float w_div, float* out_f32, void* out_bf16,
+                                int ld_bf16, int64_t* idx, float* loss, void* workspace, og_stream_t stream) {
+  const int C = n_codebook;
+  OG_REQUIRE(x && idx, "lfq_multi_fwd: bad arguments");
+  OG_REQUIRE(D >= 1 && D <= kMaxD, "lfq_multi_fwd: codebook_dim=%d outside [1,%d]", D, kMaxD);
+  OG_REQUIRE(lfq_rows_fit(ntok, C), "lfq_multi_fwd: ntok=%lld, n_codebook=%d: need ntok >= 1, n_codebook in [1,%d] "
+             "and ntok * n_codebook <= %d", (long long)ntok, C, kMaxCodebooks, INT_MAX);
+  OG_REQUIRE((long long)ldx >= (long long)C * D, "lfq_multi_fwd: ldx=%d < n_codebook * codebook_dim", ldx);
+  OG_REQUIRE(!out_bf16 || (long long)ld_bf16 >= (long long)C * D,
+             "lfq_multi_fwd: ld_bf16=%d < n_codebook * codebook_dim", ld_bf16);
+  OG_REQUIRE(!training || (loss && workspace), "lfq_multi_fwd: training needs loss and workspace");
+  return lfq_fwd(x, ldx, ntok, D, C, beta, training, w_commit, w_entropy, w_div, out_f32, out_bf16, ld_bf16, idx, loss,
+                 workspace, (cudaStream_t)stream);
+}
+
+extern "C" int og_lfq_multi_bwd(const float* x, int ldx, int64_t ntok, int D, int n_codebook, float beta,
+                                float w_commit, float w_entropy, const float* gloss, const float* dout, int ld_dout,
+                                float* dx_f32, void* dx_bf16, int ld_dx, void* workspace, og_stream_t stream) {
+  const int C = n_codebook;
+  OG_REQUIRE(x && workspace && (dx_f32 || dx_bf16), "lfq_multi_bwd: bad arguments");
+  OG_REQUIRE(D >= 1 && D <= kMaxD, "lfq_multi_bwd: codebook_dim=%d outside [1,%d]", D, kMaxD);
+  OG_REQUIRE(lfq_rows_fit(ntok, C), "lfq_multi_bwd: ntok=%lld, n_codebook=%d: need ntok >= 1, n_codebook in [1,%d] "
+             "and ntok * n_codebook <= %d", (long long)ntok, C, kMaxCodebooks, INT_MAX);
+  const long long cd = (long long)C * D;
+  OG_REQUIRE(ldx >= cd && ld_dx >= cd && (!dout || ld_dout >= cd),
+             "lfq_multi_bwd: ldx=%d, ld_dx=%d, ld_dout=%d: each must be >= n_codebook * codebook_dim", ldx, ld_dx,
+             ld_dout);
+  return lfq_bwd(x, ldx, ntok, D, C, beta, w_commit, w_entropy, gloss, dout, ld_dout, dx_f32, dx_bf16, ld_dx, workspace,
+                 (cudaStream_t)stream);
 }

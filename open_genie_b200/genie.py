@@ -31,6 +31,10 @@ class Genie(LightningModule):
     def __init__(self, tokenizer: VideoTokenizer, latent_action: LatentAction | dict, dynamics_model: DynamicsModel | dict,
                  optimizer: OptimizerCallable = FusedAdamW, img_prompt: Tensor | None = None):
         super().__init__()
+        if tokenizer.quant.num_codebooks != 1:
+            raise NotImplementedError(f'Genie needs a tokenizer with n_codebook = 1 (got '
+                                      f'{tokenizer.quant.num_codebooks}): DynamicsModel takes one token id per '
+                                      f'position, (B, T, H, W)')
         self.tokenizer = tokenizer.requires_grad_(False)          # pre-trained, frozen (find_unused_parameters=False)
         self.latent_action = latent_action if isinstance(latent_action, LatentAction) else LatentAction(**latent_action)
         self.dynamics_model = (dynamics_model if isinstance(dynamics_model, DynamicsModel)

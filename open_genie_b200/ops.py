@@ -847,49 +847,66 @@ def mse_loss(rec, target):
 # Lookup-free quantisation
 # ------------------------------------------------------------------------------------------------
 class _LfqFn(torch.autograd.Function):
-    """x: fp32 [ntok, D] -> (out fp32 [ntok, D], idx int64 [ntok], loss scalar or None)."""
+    """x: fp32 [ntok, C*D] -> (out fp32 [ntok, C*D], idx int64 [ntok] (C = 1) or [ntok, C], loss scalar or None).
+    C = 1 runs og_lfq_fwd / og_lfq_bwd; C > 1 the multi-codebook entry points."""
 
     @staticmethod
-    def forward(ctx, x, D, beta, training, w_commit, w_entropy, w_div):
+    def forward(ctx, x, D, beta, training, w_commit, w_entropy, w_div, C):
         _require_cuda(x, 'lfq input')
         xs = x.detach()
         if xs.dtype != f32 or not xs.is_contiguous():
             xs = xs.to(f32).contiguous()
         ntok = xs.shape[0]
         dev = xs.device
-        out = torch.empty((ntok, D), dtype=f32, device=dev)
-        idx = torch.empty((ntok,), dtype=torch.int64, device=dev)
+        out = torch.empty((ntok, C * D), dtype=f32, device=dev)
+        idx = torch.empty((ntok,) if C == 1 else (ntok, C), dtype=torch.int64, device=dev)
         loss = torch.zeros((), dtype=f32, device=dev)
         ws = None
         if training:
-            nbytes = _lib.load().og_lfq_workspace_bytes(ntok, D)
+            if C == 1:
+                nbytes = _lib.load().og_lfq_workspace_bytes(ntok, D)
+            else:
+                nbytes = _lib.load().og_lfq_multi_workspace_bytes(ntok, D, C)
             if nbytes == 0:
-                raise RuntimeError(f'lfq: codebook_dim={D} is outside the supported range [1, 20]')
+                raise RuntimeError(f'lfq: codebook_dim={D}, n_codebook={C} is outside the supported range '
+                                   f'(codebook_dim in [1, 20], n_codebook in [1, 65535])')
             ws = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
-        _lib.call('og_lfq_fwd', xs.data_ptr(), xs.shape[1], ntok, D, beta, int(training), w_commit, w_entropy, w_div,
-                  out.data_ptr(), None, 0, idx.data_ptr(), loss.data_ptr(), _ptr(ws), _stream())
-        ctx.cfg = (D, beta, w_commit, w_entropy, training)
+        if C == 1:
+            _lib.call('og_lfq_fwd', xs.data_ptr(), xs.shape[1], ntok, D, beta, int(training), w_commit, w_entropy,
+                      w_div, out.data_ptr(), None, 0, idx.data_ptr(), loss.data_ptr(), _ptr(ws), _stream())
+        else:
+            _lib.call('og_lfq_multi_fwd', xs.data_ptr(), xs.shape[1], ntok, D, C, beta, int(training), w_commit,
+                      w_entropy, w_div, out.data_ptr(), None, 0, idx.data_ptr(), loss.data_ptr(), _ptr(ws), _stream())
+        ctx.cfg = (D, beta, w_commit, w_entropy, training, C)
         ctx.save_for_backward(xs, ws)
         ctx.mark_non_differentiable(idx)
         return out, idx, loss
 
     @staticmethod
     def backward(ctx, dout, _didx, dloss):
-        D, beta, w_commit, w_entropy, training = ctx.cfg
+        D, beta, w_commit, w_entropy, training, C = ctx.cfg
         xs, ws = ctx.saved_tensors
         if not training:
-            return (None,) * 7     # eval: code = sign(x) has no gradient path (quantization.py:101)
+            return (None,) * 8     # eval: code = sign(x) has no gradient path (quantization.py:101)
         ntok = xs.shape[0]
-        dx = torch.empty((ntok, D), dtype=f32, device=xs.device)
+        dx = torch.empty((ntok, C * D), dtype=f32, device=xs.device)
         do = None if dout is None else dout.detach().to(f32).contiguous()
         gl = dloss.detach().to(f32).contiguous() if dloss is not None else torch.zeros((), device=xs.device)
-        _lib.call('og_lfq_bwd', xs.data_ptr(), xs.shape[1], ntok, D, beta, w_commit, w_entropy, gl.data_ptr(),
-                  _ptr(do), D, dx.data_ptr(), None, D, ws.data_ptr(), _stream())
-        return dx, None, None, None, None, None, None
+        if C == 1:
+            _lib.call('og_lfq_bwd', xs.data_ptr(), xs.shape[1], ntok, D, beta, w_commit, w_entropy, gl.data_ptr(),
+                      _ptr(do), D, dx.data_ptr(), None, D, ws.data_ptr(), _stream())
+        else:
+            _lib.call('og_lfq_multi_bwd', xs.data_ptr(), xs.shape[1], ntok, D, C, beta, w_commit, w_entropy,
+                      gl.data_ptr(), _ptr(do), C * D, dx.data_ptr(), None, C * D, ws.data_ptr(), _stream())
+        return dx, None, None, None, None, None, None, None
 
 
-def lfq(x2d, D, beta, training, w_commit, w_entropy, w_div):
-    return _LfqFn.apply(x2d, D, float(beta), bool(training), float(w_commit), float(w_entropy), float(w_div))
+def lfq(x2d, D, beta, training, w_commit, w_entropy, w_div, n_codebook=1):
+    """Lookup-free quantisation of x2d [ntok, n_codebook * D] (quantization.py:77-133): n_codebook independent D-bit
+    codes per token, their straight-through output, indices ([ntok], or [ntok, n_codebook] when n_codebook > 1) and,
+    in training, the entropy + commitment loss."""
+    return _LfqFn.apply(x2d, D, float(beta), bool(training), float(w_commit), float(w_entropy), float(w_div),
+                        int(n_codebook))
 
 
 # ------------------------------------------------------------------------------------------------
