@@ -68,7 +68,9 @@ uint64_t og_launch_count(void);
  * shrinks to the slabs that fit (20 MB always suffices); with room for fewer than two it runs unsplit.
  * gn_sums (optional): fp64 [N][2] += (sum, sum of squares) of the bf16 output per sample — the og_gn_stats
  * result for a following GroupNorm(1, C) — produced in the GEMM epilogue when the tiling allows it, otherwise
- * by an internal og_gn_stats pass; either way the caller just zeroes it first. */
+ * by an internal og_gn_stats pass; either way the caller just zeroes it first. gn_sums needs a bf16 output
+ * (out_f32 == 0); when the launch can neither fuse the sums nor make them in its split-K finish pass, it also needs
+ * og_gn_stats's cout % 8 == 0 and cout <= 2048. A call that breaks either returns -1 before anything is launched. */
 int og_conv3d_fwd(const void* x0, int c0, int kt, int kh, int kw, int pt, int ph, int pw, const void* x1, int c1,
                   const void* w, int ldw, const float* bias0, const float* bias1, const void* residual, void* out,
                   int out_f32, int N, int T, int H, int W, int cout, void* workspace, size_t workspace_bytes,
@@ -79,7 +81,8 @@ int og_conv3d_fwd(const void* x0, int c0, int kt, int kh, int kw, int pt, int ph
  *   dx[n,t,h,w,ci] = sum_{it,ih,iw,co} dy[n, t-(it-pt), h-(ih-ph), w-(iw-pw), co] * w[co][k_off + tap*cin + ci]
  * dy: bf16 [N,T,H,W,cout] (cout % 64 == 0; a narrower gradient is zero-padded by the caller and
  * w_rows <= cout gives the number of real weight rows); w as above (k_off selects the segment inside
- * a packed row, k_off % 8 == 0); dx: [N,T,H,W,cin] (cin % 64 == 0), bf16 or fp32.
+ * a packed row, k_off % 8 == 0, k_off >= 0, ldw >= k_off + kt*kh*kw*cin); kt, kh, kw >= 1 and 0 <= pt < kt
+ * (likewise ph, pw); dx: [N,T,H,W,cin] (cin % 64 == 0), bf16 or fp32. Each of these is checked before any CUDA call.
  * workspace (optional): split-K scratch as for og_conv3d_fwd, with slabs of N*T*H*W*cin floats. */
 int og_conv3d_dgrad(const void* dy, int cout, int w_rows, const void* w, int ldw, int k_off, int kt, int kh, int kw,
                     int pt, int ph, int pw, void* dx, int dx_f32, int N, int T, int H, int W, int cin,

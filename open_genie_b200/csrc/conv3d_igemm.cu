@@ -1008,6 +1008,16 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   p.num_stages = stages;
   const size_t smem_bytes = (size_t)stages * stage_bytes + 1024 + tail_bytes;
 
+  // the fused GroupNorm sums need: staged bf16 stores, no split-K, every CTA tile inside one sample. Requested sums
+  // that neither the epilogue nor the split-K finish pass can make come from og_gn_stats over the stored output; its
+  // conditions are checked here, before anything is launched, so that a refused call leaves `out` untouched.
+  const bool can_fuse = plain && p.fast_store && p.splits == 1 && bn == 1 && n_out <= 65536;
+  const bool finish_did_stats = L.gn_sums && p.splits > 1 && !L.out_f32;
+  const bool stats_pass = L.gn_sums && !can_fuse && !finish_did_stats;
+  OG_REQUIRE(!stats_pass || (!L.out_f32 && plain && n_out % 8 == 0 && n_out <= 2048),
+             "conv3d: GroupNorm statistics of this launch need a plain bf16 output with cout %% 8 == 0 and cout <= 2048 "
+             "(cout=%d)", n_out);
+
   CUtensorMap mapA0, mapA1, mapB;
   {
     // forward strided convolution: the box spans bw*sw input positions and TMA traverses it with element stride sw,
@@ -1051,8 +1061,6 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
     if (r != OG_OK) return r;
   }
 
-  // the fused GroupNorm sums need: staged bf16 stores, no split-K, every CTA tile inside one sample
-  const bool can_fuse = plain && p.fast_store && p.splits == 1 && bn == 1 && n_out <= 65536;
   p.gn_sums = (L.gn_sums && can_fuse) ? L.gn_sums : nullptr;
   const int total_tiles = p.num_m_tiles * p.num_n_tiles * p.splits;
   int grid = num_sms();
@@ -1075,10 +1083,8 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   }
   if (rc != OG_OK) return rc;
   g_launches.fetch_add(1);
-  bool finish_did_stats = false;
   if (p.splits > 1) {
     const long long per_sample = (long long)T * H * W * n_out;
-    finish_did_stats = L.gn_sums && !L.out_f32;
     double* gs = finish_did_stats ? L.gn_sums : nullptr;
     const int vec = (n_out % 4 == 0) ? 4 : 1;
     long long bx = (per_sample / vec + 255) / 256;
@@ -1096,8 +1102,7 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
     g_launches.fetch_add(1);
   }
   // requested statistics that could not be fused: run the stand-alone pass on the stored output
-  if (L.gn_sums && !p.gn_sums && !finish_did_stats) {
-    OG_REQUIRE(!L.out_f32 && plain, "conv3d: GroupNorm statistics need a plain bf16 output");
+  if (stats_pass) {
     int r = og_gn_stats(L.out, N, (int64_t)T * H * W, n_out, 1, L.gn_sums, (og_stream_t)stream);
     if (r != OG_OK) return r;
   }
@@ -1118,6 +1123,7 @@ extern "C" int og_conv3d_fwd(const void* x0, int c0, int kt, int kh, int kw, int
              "conv3d_fwd: bad kernel/padding (%d,%d,%d)/(%d,%d,%d)", kt, kh, kw, pt, ph, pw);
   const int ktot = kt * kh * kw * c0 + (x1 ? c1 : 0);
   OG_REQUIRE(ldw >= ktot && ldw % 8 == 0, "conv3d_fwd: ldw=%d must be >= %d and a multiple of 8", ldw, ktot);
+  OG_REQUIRE(!gn_sums || !out_f32, "conv3d_fwd: gn_sums needs a bf16 output (out_f32 = 0)");
   IgemmLaunch L;
   L.a0 = x0; L.c0 = c0; L.aT = T; L.aH = H; L.aW = W;
   L.a1 = x1; L.c1 = c1;
@@ -1142,6 +1148,11 @@ extern "C" int og_conv3d_dgrad(const void* dy, int cout, int w_rows, const void*
   OG_REQUIRE(cin > 0 && cin % 64 == 0, "conv3d_dgrad: cin=%d must be a multiple of 64", cin);
   OG_REQUIRE(k_off % 8 == 0 && ldw % 8 == 0, "conv3d_dgrad: k_off/ldw must be multiples of 8");
   OG_REQUIRE(w_rows > 0 && w_rows <= cout, "conv3d_dgrad: w_rows=%d must be in (0, cout]", w_rows);
+  OG_REQUIRE(kt >= 1 && kh >= 1 && kw >= 1 && pt >= 0 && ph >= 0 && pw >= 0 && pt < kt && ph < kh && pw < kw,
+             "conv3d_dgrad: bad kernel/padding (%d,%d,%d)/(%d,%d,%d)", kt, kh, kw, pt, ph, pw);
+  OG_REQUIRE(k_off >= 0, "conv3d_dgrad: k_off=%d must be >= 0", k_off);
+  const long long kend = (long long)k_off + (long long)kt * kh * kw * cin;
+  OG_REQUIRE(ldw >= kend, "conv3d_dgrad: ldw=%d must be >= k_off + kt*kh*kw*cin = %lld", ldw, kend);
   IgemmLaunch L;
   L.a0 = dy; L.c0 = cout; L.aT = T; L.aH = H; L.aW = W;
   L.segs[0] = make_seg(cout / 64, kt, kh, kw, pt, ph, pw, -1);
