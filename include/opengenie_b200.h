@@ -350,6 +350,15 @@ int og_rope_ln_fwd(const void* x, const float* freq, const float* gamma, const f
 int og_rope_ln_bwd(const void* x, const float* freq, const float* gamma, float eps, const void* g0, const void* g1,
                    const void* g2, const void* add, void* dx, float* dgamma, float* dbeta, int64_t rows, int C,
                    int64_t pos_div, int pos_mod, const float* cos_sin, og_stream_t stream);
+/* Attention without a rotary embedding (embed=False: RotaryEmbedding replaced by nn.Identity, attention.py:199-239):
+ * y = LayerNorm(x) on rows [rows][C], and dx = LN'(g0 + g1 + g2) + add with dgamma / dbeta accumulated (+=); g1, g2,
+ * add may be NULL. The og_rope_ln_* passes without the rotation: fp32 statistics, the same kernels for C = 256, 512
+ * and 1024 with 16-byte aligned pointers, one warp per row otherwise. -1 unless C is even and in [2, 1024], rows > 0
+ * and the bf16 pointers (and dgamma / dbeta) are 4-byte aligned. */
+int og_ln_rows_fwd(const void* x, const float* gamma, const float* beta, float eps, void* y, int64_t rows, int C,
+                   og_stream_t stream);
+int og_ln_rows_bwd(const void* x, const float* gamma, float eps, const void* g0, const void* g1, const void* g2,
+                   const void* add, void* dx, float* dgamma, float* dbeta, int64_t rows, int C, og_stream_t stream);
 
 /* Spatial attention: F.scaled_dot_product_attention(q,k,v, scale) non-causal (attention.py:229-234) on
  * wgmma tensor cores. q,k,v,out: [nseq][S][C], C = n_head*64, n_head*128 or n_head*16 (d_head 64, 128 or 16; any

@@ -1,5 +1,10 @@
 // attention_rows.cu — the bandwidth-bound parts of the factored space-time attention:
 //   * fused RoPE + LayerNorm (forward / backward) on NDHWC rows
+//   * LayerNorm alone on the same rows (attention with embed=False, where the reference's embed is nn.Identity): the
+//     same kernel bodies, templated on kRope, so the og_ln_rows_* kernels are the og_rope_ln_* ones minus the rotation
+//     and the kRope = true instantiations compile to the same instructions as before the flag existed.
+//     Registers (sm_90a, no spills): og_ln_rows_fwd_kernel 64, og_ln_rows_fwd_vec_kernel<1, 2, 4> 40 / 64 / 116,
+//     og_ln_rows_bwd_kernel 190, og_ln_rows_bwd_vec_kernel<1, 2, 4> 72 / 128 / 248.
 //   * temporal (causal, T <= 32) attention per pixel and head, forward / backward, on CUDA cores
 //
 // Reference (genie/module/attention.py, HEAD-valid configuration — SURVEY.md §7 H6):
@@ -27,17 +32,18 @@ __device__ __forceinline__ float warp_sum(float v) {
 // RoPE + LayerNorm forward: one warp per row. Lane l owns channel pairs l, l+32, ...
 // pos(row) = (row / pos_div) % pos_mod   (spatial: div 1, mod H*W ; temporal: div H*W, mod T)
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-    og_rope_ln_fwd_kernel(const __nv_bfloat162* __restrict__ x, const float* __restrict__ freq,
-                          const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                          __nv_bfloat162* __restrict__ y, long long rows, int C, long long pos_div, int pos_mod) {
+template <bool kRope>
+__device__ __forceinline__ void rope_ln_fwd_rows(const __nv_bfloat162* __restrict__ x, const float* __restrict__ freq,
+                                                 const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                 float eps, __nv_bfloat162* __restrict__ y, long long rows, int C,
+                                                 long long pos_div, int pos_mod) {
   const int lane = threadIdx.x & 31;
   const int pairs = C >> 1;
   const int ppl = (pairs + 31) >> 5;
   const long long warp0 = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const long long nwarps = (long long)gridDim.x * (blockDim.x >> 5);
   for (long long row = warp0; row < rows; row += nwarps) {
-    const float pos = (float)((row / pos_div) % pos_mod);
+    const float pos = kRope ? (float)((row / pos_div) % pos_mod) : 0.f;
     float r0[kMaxPairsPerLane], r1[kMaxPairsPerLane];
     float s = 0.f;
 #pragma unroll
@@ -45,10 +51,15 @@ __global__ void __launch_bounds__(256)
       const int p = lane + 32 * j;
       if (j < ppl && p < pairs) {
         const float2 v = __bfloat1622float2(x[row * pairs + p]);
-        float sn, cs;
-        sincosf(pos * __ldg(freq + p), &sn, &cs);
-        r0[j] = v.x * cs - v.y * sn;
-        r1[j] = v.y * cs + v.x * sn;
+        if constexpr (kRope) {
+          float sn, cs;
+          sincosf(pos * __ldg(freq + p), &sn, &cs);
+          r0[j] = v.x * cs - v.y * sn;
+          r1[j] = v.y * cs + v.x * sn;
+        } else {
+          r0[j] = v.x;
+          r1[j] = v.y;
+        }
         s += r0[j] + r1[j];
       } else {
         r0[j] = r1[j] = 0.f;
@@ -77,14 +88,27 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+__global__ void __launch_bounds__(256)
+    og_rope_ln_fwd_kernel(const __nv_bfloat162* __restrict__ x, const float* __restrict__ freq,
+                          const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
+                          __nv_bfloat162* __restrict__ y, long long rows, int C, long long pos_div, int pos_mod) {
+  rope_ln_fwd_rows<true>(x, freq, gamma, beta, eps, y, rows, C, pos_div, pos_mod);
+}
+
+__global__ void __launch_bounds__(256)
+    og_ln_rows_fwd_kernel(const __nv_bfloat162* __restrict__ x, const float* __restrict__ gamma,
+                          const float* __restrict__ beta, float eps, __nv_bfloat162* __restrict__ y, long long rows,
+                          int C) {
+  rope_ln_fwd_rows<false>(x, nullptr, gamma, beta, eps, y, rows, C, 1, 1);
+}
+
 // Vector form of the forward pass for C % 256 == 0 (same lane -> channel mapping as the vector backward below:
 // lane l owns the 4 consecutive pairs [128 j + 4 l, +4) of chunk j, i.e. one 16-byte load / store per chunk).
-template <int NCH>
-__global__ void __launch_bounds__(256)
-    og_rope_ln_fwd_vec_kernel(const uint4* __restrict__ x, const float* __restrict__ freq,
-                              const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                              uint4* __restrict__ y, long long rows, long long pos_div, int pos_mod,
-                              const float4* __restrict__ tab) {
+template <int NCH, bool kRope>
+__device__ __forceinline__ void rope_ln_fwd_vec_rows(const uint4* __restrict__ x, const float* __restrict__ freq,
+                                                     const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                     float eps, uint4* __restrict__ y, long long rows,
+                                                     long long pos_div, int pos_mod, const float4* __restrict__ tab) {
   constexpr int NP = 4 * NCH;
   constexpr int C = 256 * NCH;
   constexpr int VPR = 32 * NCH;
@@ -97,14 +121,14 @@ __global__ void __launch_bounds__(256)
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const int p = 128 * j + 4 * lane + e;
-      fq[4 * j + e] = __ldg(freq + p);
+      if constexpr (kRope) fq[4 * j + e] = __ldg(freq + p);
       gm0[4 * j + e] = __ldg(gamma + 2 * p);
       gm1[4 * j + e] = __ldg(gamma + 2 * p + 1);
       bt0[4 * j + e] = __ldg(beta + 2 * p);
       bt1[4 * j + e] = __ldg(beta + 2 * p + 1);
     }
   for (long long row = warp0; row < rows; row += nwarps) {
-    const int ipos = (int)((row / pos_div) % pos_mod);
+    const int ipos = kRope ? (int)((row / pos_div) % pos_mod) : 0;
     const float pos = (float)ipos;
     const long long vb = row * VPR + lane;
     uint4 ux[NCH];
@@ -114,7 +138,7 @@ __global__ void __launch_bounds__(256)
     // once per (frequencies, sequence length) instead of once per element — the '2d' angles reach ~4000 rad, where
     // sincosf takes its slow range-reduction path and made this pass SM-bound at 0.4 of the HBM roofline)
     float tcs[NP], tsn[NP];
-    if (tab) {
+    if (kRope && tab) {
       const float4* tr = tab + (long long)ipos * (C / 4);      // row of C/2 (cos, sin) pairs = C/4 float4
 #pragma unroll
       for (int j = 0; j < NCH; ++j) {
@@ -132,15 +156,20 @@ __global__ void __launch_bounds__(256)
       for (int e = 0; e < 4; ++e) {
         const int i = 4 * j + e;
         const float2 v = __bfloat1622float2(h[e]);
-        float sn, cs;
-        if (tab) {
-          sn = tsn[i];
-          cs = tcs[i];
+        if constexpr (kRope) {
+          float sn, cs;
+          if (tab) {
+            sn = tsn[i];
+            cs = tcs[i];
+          } else {
+            sincosf(pos * fq[i], &sn, &cs);
+          }
+          r0[i] = v.x * cs - v.y * sn;
+          r1[i] = v.y * cs + v.x * sn;
         } else {
-          sincosf(pos * fq[i], &sn, &cs);
+          r0[i] = v.x;
+          r1[i] = v.y;
         }
-        r0[i] = v.x * cs - v.y * sn;
-        r1[i] = v.y * cs + v.x * sn;
         s += r0[i] + r1[i];
       }
     }
@@ -166,15 +195,34 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+template <int NCH>
+__global__ void __launch_bounds__(256)
+    og_rope_ln_fwd_vec_kernel(const uint4* __restrict__ x, const float* __restrict__ freq,
+                              const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
+                              uint4* __restrict__ y, long long rows, long long pos_div, int pos_mod,
+                              const float4* __restrict__ tab) {
+  rope_ln_fwd_vec_rows<NCH, true>(x, freq, gamma, beta, eps, y, rows, pos_div, pos_mod, tab);
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(256)
+    og_ln_rows_fwd_vec_kernel(const uint4* __restrict__ x, const float* __restrict__ gamma,
+                              const float* __restrict__ beta, float eps, uint4* __restrict__ y, long long rows) {
+  rope_ln_fwd_vec_rows<NCH, false>(x, nullptr, gamma, beta, eps, y, rows, 1, 1, nullptr);
+}
+
 // backward: g = g0 (+ g1 + g2) ; dx = R^T LN'(g) (+ add). dgamma / dbeta accumulated per lane over the
 // warp's rows, then shared + global atomics once per block.
-__global__ void __launch_bounds__(256)
-    og_rope_ln_bwd_kernel(const __nv_bfloat162* __restrict__ x, const float* __restrict__ freq,
-                          const float* __restrict__ gamma, float eps, const __nv_bfloat162* __restrict__ g0,
-                          const __nv_bfloat162* __restrict__ g1, const __nv_bfloat162* __restrict__ g2,
-                          const __nv_bfloat162* __restrict__ add, __nv_bfloat162* __restrict__ dx,
-                          float* __restrict__ dgamma, float* __restrict__ dbeta, long long rows, int C,
-                          long long pos_div, int pos_mod) {
+template <bool kRope>
+__device__ __forceinline__ void rope_ln_bwd_rows(const __nv_bfloat162* __restrict__ x, const float* __restrict__ freq,
+                                                 const float* __restrict__ gamma, float eps,
+                                                 const __nv_bfloat162* __restrict__ g0,
+                                                 const __nv_bfloat162* __restrict__ g1,
+                                                 const __nv_bfloat162* __restrict__ g2,
+                                                 const __nv_bfloat162* __restrict__ add,
+                                                 __nv_bfloat162* __restrict__ dx, float* __restrict__ dgamma,
+                                                 float* __restrict__ dbeta, long long rows, int C, long long pos_div,
+                                                 int pos_mod) {
   extern __shared__ float sh[];  // [2][C]
   for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) sh[i] = 0.f;
   __syncthreads();
@@ -187,7 +235,7 @@ __global__ void __launch_bounds__(256)
 #pragma unroll
   for (int j = 0; j < kMaxPairsPerLane; ++j) dg0[j] = dg1[j] = db0[j] = db1[j] = 0.f;
   for (long long row = warp0; row < rows; row += nwarps) {
-    const float pos = (float)((row / pos_div) % pos_mod);
+    const float pos = kRope ? (float)((row / pos_div) % pos_mod) : 0.f;
     float r0[kMaxPairsPerLane], r1[kMaxPairsPerLane], sn[kMaxPairsPerLane], cs[kMaxPairsPerLane];
     float s = 0.f;
 #pragma unroll
@@ -195,9 +243,14 @@ __global__ void __launch_bounds__(256)
       const int p = lane + 32 * j;
       if (j < ppl && p < pairs) {
         const float2 v = __bfloat1622float2(x[row * pairs + p]);
-        sincosf(pos * __ldg(freq + p), &sn[j], &cs[j]);
-        r0[j] = v.x * cs[j] - v.y * sn[j];
-        r1[j] = v.y * cs[j] + v.x * sn[j];
+        if constexpr (kRope) {
+          sincosf(pos * __ldg(freq + p), &sn[j], &cs[j]);
+          r0[j] = v.x * cs[j] - v.y * sn[j];
+          r1[j] = v.y * cs[j] + v.x * sn[j];
+        } else {
+          r0[j] = v.x;
+          r1[j] = v.y;
+        }
         s += r0[j] + r1[j];
       } else {
         r0[j] = r1[j] = sn[j] = cs[j] = 0.f;
@@ -255,8 +308,8 @@ __global__ void __launch_bounds__(256)
       if (j < ppl && p < pairs) {
         const float d0 = rstd * (gh0[j] - m1 - r0[j] * m2);
         const float d1 = rstd * (gh1[j] - m1 - r1[j] * m2);
-        float o0 = d0 * cs[j] + d1 * sn[j];   // R^T
-        float o1 = -d0 * sn[j] + d1 * cs[j];
+        float o0 = kRope ? d0 * cs[j] + d1 * sn[j] : d0;   // R^T
+        float o1 = kRope ? -d0 * sn[j] + d1 * cs[j] : d1;
         if (add) {
           const float2 t = __bfloat1622float2(add[row * pairs + p]);
           o0 += t.x;
@@ -283,18 +336,37 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+__global__ void __launch_bounds__(256)
+    og_rope_ln_bwd_kernel(const __nv_bfloat162* __restrict__ x, const float* __restrict__ freq,
+                          const float* __restrict__ gamma, float eps, const __nv_bfloat162* __restrict__ g0,
+                          const __nv_bfloat162* __restrict__ g1, const __nv_bfloat162* __restrict__ g2,
+                          const __nv_bfloat162* __restrict__ add, __nv_bfloat162* __restrict__ dx,
+                          float* __restrict__ dgamma, float* __restrict__ dbeta, long long rows, int C,
+                          long long pos_div, int pos_mod) {
+  rope_ln_bwd_rows<true>(x, freq, gamma, eps, g0, g1, g2, add, dx, dgamma, dbeta, rows, C, pos_div, pos_mod);
+}
+
+__global__ void __launch_bounds__(256)
+    og_ln_rows_bwd_kernel(const __nv_bfloat162* __restrict__ x, const float* __restrict__ gamma, float eps,
+                          const __nv_bfloat162* __restrict__ g0, const __nv_bfloat162* __restrict__ g1,
+                          const __nv_bfloat162* __restrict__ g2, const __nv_bfloat162* __restrict__ add,
+                          __nv_bfloat162* __restrict__ dx, float* __restrict__ dgamma, float* __restrict__ dbeta,
+                          long long rows, int C) {
+  rope_ln_bwd_rows<false>(x, nullptr, gamma, eps, g0, g1, g2, add, dx, dgamma, dbeta, rows, C, 1, 1);
+}
+
 // Vector form of the backward pass for C % 256 == 0: lane l owns the 4 consecutive channel pairs
 // [128 j + 4 l, +4) of chunk j (one 16-byte load per tensor and chunk instead of four 4-byte ones) and the
 // per-lane arrays are sized by the template, not by the C <= 1024 maximum: 216 -> ~128 registers, two resident
 // blocks per SM and 4x the bytes in flight. Same arithmetic as the scalar kernel above.
-template <int NCH>
-__global__ void __launch_bounds__(256, (NCH <= 2 ? 2 : 1))
-    og_rope_ln_bwd_vec_kernel(const uint4* __restrict__ x, const float* __restrict__ freq,
-                              const float* __restrict__ gamma, float eps, const uint4* __restrict__ g0,
-                              const uint4* __restrict__ g1, const uint4* __restrict__ g2,
-                              const uint4* __restrict__ add, uint4* __restrict__ dx, float* __restrict__ dgamma,
-                              float* __restrict__ dbeta, long long rows, long long pos_div, int pos_mod,
-                              const float4* __restrict__ tab) {
+template <int NCH, bool kRope>
+__device__ __forceinline__ void rope_ln_bwd_vec_rows(const uint4* __restrict__ x, const float* __restrict__ freq,
+                                                     const float* __restrict__ gamma, float eps,
+                                                     const uint4* __restrict__ g0, const uint4* __restrict__ g1,
+                                                     const uint4* __restrict__ g2, const uint4* __restrict__ add,
+                                                     uint4* __restrict__ dx, float* __restrict__ dgamma,
+                                                     float* __restrict__ dbeta, long long rows, long long pos_div,
+                                                     int pos_mod, const float4* __restrict__ tab) {
   constexpr int NP = 4 * NCH;      // pairs per lane
   constexpr int C = 256 * NCH;
   constexpr int VPR = 32 * NCH;    // uint4 vectors per row
@@ -310,7 +382,7 @@ __global__ void __launch_bounds__(256, (NCH <= 2 ? 2 : 1))
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const int p = 128 * j + 4 * lane + e;
-      fq[4 * j + e] = __ldg(freq + p);
+      if constexpr (kRope) fq[4 * j + e] = __ldg(freq + p);
       gm0[4 * j + e] = __ldg(gamma + 2 * p);
       gm1[4 * j + e] = __ldg(gamma + 2 * p + 1);
     }
@@ -327,7 +399,7 @@ __global__ void __launch_bounds__(256, (NCH <= 2 ? 2 : 1))
     }
   };
   for (long long row = warp0; row < rows; row += nwarps) {
-    const int ipos = (int)((row / pos_div) % pos_mod);
+    const int ipos = kRope ? (int)((row / pos_div) % pos_mod) : 0;
     const float pos = (float)ipos;
     const long long vb = row * VPR + lane;
     uint4 ux[NCH], ug[NCH];
@@ -337,7 +409,7 @@ __global__ void __launch_bounds__(256, (NCH <= 2 ? 2 : 1))
       ug[j] = __ldg(g0 + vb + 32 * j);
     }
     float r0[NP], r1[NP], sn[NP], cs[NP];
-    if (tab) {   // see og_rope_ln_fwd_vec_kernel
+    if (kRope && tab) {   // see og_rope_ln_fwd_vec_kernel
       const float4* tr = tab + (long long)ipos * (C / 4);
 #pragma unroll
       for (int j = 0; j < NCH; ++j) {
@@ -354,9 +426,14 @@ __global__ void __launch_bounds__(256, (NCH <= 2 ? 2 : 1))
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int i = 4 * j + e;
-        if (!tab) sincosf(pos * fq[i], &sn[i], &cs[i]);
-        r0[i] = a[e] * cs[i] - b[e] * sn[i];
-        r1[i] = b[e] * cs[i] + a[e] * sn[i];
+        if constexpr (kRope) {
+          if (!tab) sincosf(pos * fq[i], &sn[i], &cs[i]);
+          r0[i] = a[e] * cs[i] - b[e] * sn[i];
+          r1[i] = b[e] * cs[i] + a[e] * sn[i];
+        } else {
+          r0[i] = a[e];
+          r1[i] = b[e];
+        }
         s += r0[i] + r1[i];
       }
     }
@@ -422,8 +499,8 @@ __global__ void __launch_bounds__(256, (NCH <= 2 ? 2 : 1))
         const int i = 4 * j + e;
         const float d0 = rstd * (gh0[i] - m1 - r0[i] * m2);
         const float d1 = rstd * (gh1[i] - m1 - r1[i] * m2);
-        const float o0 = d0 * cs[i] + d1 * sn[i] + aa[e];   // R^T
-        const float o1 = -d0 * sn[i] + d1 * cs[i] + ab[e];
+        const float o0 = (kRope ? d0 * cs[i] + d1 * sn[i] : d0) + aa[e];   // R^T
+        const float o1 = (kRope ? -d0 * sn[i] + d1 * cs[i] : d1) + ab[e];
         ow[e] = pack_bf16x2(o0, o1);
       }
       dx[vb + 32 * j] = o;
@@ -444,6 +521,27 @@ __global__ void __launch_bounds__(256, (NCH <= 2 ? 2 : 1))
     atomicAdd(&dgamma[i], sh[i]);
     atomicAdd(&dbeta[i], sh[C + i]);
   }
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(256, (NCH <= 2 ? 2 : 1))
+    og_rope_ln_bwd_vec_kernel(const uint4* __restrict__ x, const float* __restrict__ freq,
+                              const float* __restrict__ gamma, float eps, const uint4* __restrict__ g0,
+                              const uint4* __restrict__ g1, const uint4* __restrict__ g2,
+                              const uint4* __restrict__ add, uint4* __restrict__ dx, float* __restrict__ dgamma,
+                              float* __restrict__ dbeta, long long rows, long long pos_div, int pos_mod,
+                              const float4* __restrict__ tab) {
+  rope_ln_bwd_vec_rows<NCH, true>(x, freq, gamma, eps, g0, g1, g2, add, dx, dgamma, dbeta, rows, pos_div, pos_mod,
+                                  tab);
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(256, (NCH <= 2 ? 2 : 1))
+    og_ln_rows_bwd_vec_kernel(const uint4* __restrict__ x, const float* __restrict__ gamma, float eps,
+                              const uint4* __restrict__ g0, const uint4* __restrict__ g1,
+                              const uint4* __restrict__ g2, const uint4* __restrict__ add, uint4* __restrict__ dx,
+                              float* __restrict__ dgamma, float* __restrict__ dbeta, long long rows) {
+  rope_ln_bwd_vec_rows<NCH, false>(x, nullptr, gamma, eps, g0, g1, g2, add, dx, dgamma, dbeta, rows, 1, 1, nullptr);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -819,6 +917,67 @@ extern "C" int og_rope_ln_bwd(const void* x, const float* freq, const float* gam
       (const __nv_bfloat162*)x, freq, gamma, eps, (const __nv_bfloat162*)g0, (const __nv_bfloat162*)g1,
       (const __nv_bfloat162*)g2, (const __nv_bfloat162*)add, (__nv_bfloat162*)dx, dgamma, dbeta, rows, C, pos_div,
       pos_mod);
+  OG_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1);
+  return OG_OK;
+}
+
+// LayerNorm-only passes (attention without a rotary embedding): the RoPE passes' kernels and dispatch, no rotation.
+extern "C" int og_ln_rows_fwd(const void* x, const float* gamma, const float* beta, float eps, void* y, int64_t rows,
+                              int C, og_stream_t stream) {
+  OG_REQUIRE(x && gamma && beta && y && rows > 0, "ln_rows_fwd: bad arguments");
+  OG_REQUIRE(C >= 2 && C % 2 == 0 && C <= 2 * 32 * kMaxPairsPerLane, "ln_rows_fwd: C=%d must be even and in [2, 1024]",
+             C);
+  const uintptr_t align = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y);
+  OG_REQUIRE((align & 3) == 0, "ln_rows_fwd: x and y must be 4-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = row_grid(rows, 8);
+  if ((C == 256 || C == 512 || C == 1024) && (align & 15) == 0) {
+    if (C == 256)
+      og_ln_rows_fwd_vec_kernel<1><<<grid, 256, 0, st>>>((const uint4*)x, gamma, beta, eps, (uint4*)y, rows);
+    else if (C == 512)
+      og_ln_rows_fwd_vec_kernel<2><<<grid, 256, 0, st>>>((const uint4*)x, gamma, beta, eps, (uint4*)y, rows);
+    else
+      og_ln_rows_fwd_vec_kernel<4><<<grid, 256, 0, st>>>((const uint4*)x, gamma, beta, eps, (uint4*)y, rows);
+  } else {
+    og_ln_rows_fwd_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat162*)x, gamma, beta, eps, (__nv_bfloat162*)y, rows, C);
+  }
+  OG_CHECK_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1);
+  return OG_OK;
+}
+
+extern "C" int og_ln_rows_bwd(const void* x, const float* gamma, float eps, const void* g0, const void* g1,
+                              const void* g2, const void* add, void* dx, float* dgamma, float* dbeta, int64_t rows,
+                              int C, og_stream_t stream) {
+  OG_REQUIRE(x && gamma && g0 && dx && dgamma && dbeta && rows > 0, "ln_rows_bwd: bad arguments");
+  OG_REQUIRE(C >= 2 && C % 2 == 0 && C <= 2 * 32 * kMaxPairsPerLane, "ln_rows_bwd: C=%d must be even and in [2, 1024]",
+             C);
+  const uintptr_t align = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(g0) |
+                          reinterpret_cast<uintptr_t>(g1) | reinterpret_cast<uintptr_t>(g2) |
+                          reinterpret_cast<uintptr_t>(add) | reinterpret_cast<uintptr_t>(dx);
+  OG_REQUIRE((align & 3) == 0, "ln_rows_bwd: x, g0, g1, g2, add and dx must be 4-byte aligned");
+  OG_REQUIRE((((reinterpret_cast<uintptr_t>(dgamma) | reinterpret_cast<uintptr_t>(dbeta))) & 3) == 0,
+             "ln_rows_bwd: dgamma and dbeta must be 4-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  int grid = row_grid(rows, 8);
+  const size_t shb = 2 * C * sizeof(float);
+  if ((C == 256 || C == 512 || C == 1024) && (align & 15) == 0) {
+    if (grid > num_sms() * 4) grid = num_sms() * 4;  // as og_rope_ln_bwd
+#define OG_LN_BWD(NCH)                                                                                                \
+    og_ln_rows_bwd_vec_kernel<NCH><<<grid, 256, shb, st>>>((const uint4*)x, gamma, eps, (const uint4*)g0,              \
+                                                           (const uint4*)g1, (const uint4*)g2, (const uint4*)add,      \
+                                                           (uint4*)dx, dgamma, dbeta, rows)
+    if (C == 256) OG_LN_BWD(1);
+    else if (C == 512) OG_LN_BWD(2);
+    else OG_LN_BWD(4);
+#undef OG_LN_BWD
+  } else {
+    if (grid > num_sms() * 2) grid = num_sms() * 2;
+    og_ln_rows_bwd_kernel<<<grid, 256, shb, st>>>(
+        (const __nv_bfloat162*)x, gamma, eps, (const __nv_bfloat162*)g0, (const __nv_bfloat162*)g1,
+        (const __nv_bfloat162*)g2, (const __nv_bfloat162*)add, (__nv_bfloat162*)dx, dgamma, dbeta, rows, C);
+  }
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
   return OG_OK;

@@ -9,6 +9,9 @@ Head widths: d_head = 16, 64 or 128 (flash attention and the temporal kernels ha
 and 128 runs the tiled kernels at every clip length). Space and time attention may use different widths when n_head * d_head
 matches, e.g. SpaceTimeAttention(n_head=(2, 1), d_head=(64, 128)) or (n_head=(4, 1), d_head=(16, 64)); the FFN
 GroupNorm takes the temporal head count.
+Rotary embeddings: `embed=False` (SpaceTimeAttention: a bool or a (space, time) pair) replaces the RotaryEmbedding by
+nn.Identity, as the reference does, so q = k = v = LayerNorm(x) and the state_dict has no embed.freq key; the row
+pass is then og_ln_rows_fwd / bwd instead of the fused RoPE+LayerNorm pass. It combines with every option below.
 Dropout: `dropout` (0 <= p < 1) drops attention probabilities as SDPA's dropout_p does, in both the spatial and the
 temporal attention. Like the reference, which passes dropout_p to the functional SDPA, it drops in eval mode and under
 no_grad too; set `module.dropout = 0` (read at every call) for deterministic inference. The masks come from Philox
@@ -16,7 +19,7 @@ seeds drawn from the CUDA generator (csrc/attn_dropout.cuh), so torch.manual_see
 The FFN is the reference's ForwardBlock: GroupNorm -> conv (-> GELU -> conv)* with `hid_dim` hidden widths, ending at
 `d_out` channels (with transpose=True, where the skip becomes the 1x1x1 ffn_skip conv); `bias` gives every FFN conv a
 bias. Hidden widths and d_out are multiples of 64.
-state_dict keys: {space,temp}_attn.norm.{weight,bias}, {space,temp}_attn.embed.freq,
+state_dict keys: {space,temp}_attn.norm.{weight,bias}, {space,temp}_attn.embed.freq (with embed),
 temp_attn.to_qkv.to_{k,v}.{weight[,bias]} (with key_dim), ffn.1.net.0.{weight,bias}, ffn.1.net.{i}.0.{weight[,bias]}
 (i = 1 .. len(hid_dim) + 1), ffn_skip.{weight,bias} (d_out != n_head*d_head).
 """
@@ -88,12 +91,11 @@ class Attention(nn.Module):
             raise NotImplementedError('only d_inp == d_out == n_head*d_head is valid at the reference HEAD')
         if not 0.0 <= dropout < 1.0:
             raise NotImplementedError(f'attention dropout must lie in [0, 1), not {dropout}')
-        if not embed:
-            raise NotImplementedError('embed=False is not used by any shipped blueprint')
         if d_head not in (16, 64, 128):
             raise NotImplementedError(f'the attention kernels take d_head = 16, 64 or 128, not {d_head}')
         self.norm = nn.LayerNorm(hid)
-        self.embed = RotaryEmbedding(self.d_inp, kind=self.rope_kind)
+        # embed=False: no positional encoding, q = LayerNorm(x); nn.Identity as in the reference, so no embed.freq key
+        self.embed = RotaryEmbedding(self.d_inp, kind=self.rope_kind) if embed else nn.Identity()
         self.to_qkv = Adapter(qry_dim=self.d_inp, n_head=n_head, d_head=d_head, bias=bias, **kwargs)
         self.n_head, self.d_head = n_head, d_head
         # reference precedence: default(scale, n_head * d_head ** -0.5)   (attention.py:195)
@@ -106,6 +108,11 @@ class Attention(nn.Module):
         t = default(transpose, self.transpose)
         x = video.permute(0, 2, 3, 4, 1) if t else video            # -> (B, T, H, W, C), free for internal tensors
         return x, t
+
+    @property
+    def _freq(self) -> Tensor | None:
+        """The rotary frequencies, or None without a rotary embedding (the attention functions then skip the rotation)."""
+        return self.embed.freq if isinstance(self.embed, RotaryEmbedding) else None
 
     @staticmethod
     def _back(y: Tensor, t: bool) -> Tensor:
@@ -122,7 +129,7 @@ class SpatialAttention(Attention):
         if exists(cond) or exists(mask):
             raise NotImplementedError('spatial cond / mask are dead code at the reference HEAD (attention.py:290,296)')
         x, t = self._rows(video, transpose)
-        y = ops.space_attention_res(x, self.embed.freq, self.norm.weight, self.norm.bias, self.n_head, self.scale,
+        y = ops.space_attention_res(x, self._freq, self.norm.weight, self.norm.bias, self.n_head, self.scale,
                                     self.norm.eps, self.dropout)
         if not _residual:
             y = y - ops._rows_bf16(x)          # rarely used stand-alone path
@@ -144,7 +151,7 @@ class TemporalAttention(Attention):
             c = cond.float()
             kc = self.to_qkv.to_k(c)            # (B, T, C): a few kFLOP of host-side plumbing (torch, autograd)
             vc = self.to_qkv.to_v(c)
-        y = ops.time_attention_res(x, self.embed.freq, self.norm.weight, self.norm.bias, self.n_head, self.scale,
+        y = ops.time_attention_res(x, self._freq, self.norm.weight, self.norm.bias, self.n_head, self.scale,
                                    kc, vc, self.norm.eps, self.dropout)
         if not _residual:
             y = y - ops._rows_bf16(x)

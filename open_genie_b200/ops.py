@@ -942,6 +942,28 @@ def _rope_table(freq: Tensor, npos: int) -> Optional[Tensor]:
     return t
 
 
+def _ln_rows_fwd(x: Tensor, freq: Optional[Tensor], gamma: Tensor, beta: Tensor, eps: float, q: Tensor, rows: int,
+                 C: int, pos_div: int, pos_mod: int, s) -> None:
+    """q = LayerNorm(RoPE(x)) with the rotary frequencies `freq`, or q = LayerNorm(x) when freq is None (embed=False)."""
+    if freq is None:
+        _lib.call('og_ln_rows_fwd', x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), eps, q.data_ptr(), rows, C, s)
+    else:
+        _lib.call('og_rope_ln_fwd', x.data_ptr(), freq.data_ptr(), gamma.data_ptr(), beta.data_ptr(), eps,
+                  q.data_ptr(), rows, C, pos_div, pos_mod, _ptr(_rope_table(freq, pos_mod)), s)
+
+
+def _ln_rows_bwd(x: Tensor, freq: Optional[Tensor], gamma: Tensor, eps: float, g0: Tensor, g1, g2, add: Tensor,
+                 dx: Tensor, dgamma: Tensor, dbeta: Tensor, rows: int, C: int, pos_div: int, pos_mod: int, s) -> None:
+    """The backward pass of _ln_rows_fwd for the gradient g0 + g1 + g2 (g1, g2 may be None), plus `add`."""
+    if freq is None:
+        _lib.call('og_ln_rows_bwd', x.data_ptr(), gamma.data_ptr(), eps, g0.data_ptr(), _ptr(g1), _ptr(g2),
+                  add.data_ptr(), dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), rows, C, s)
+    else:
+        _lib.call('og_rope_ln_bwd', x.data_ptr(), freq.data_ptr(), gamma.data_ptr(), eps, g0.data_ptr(), _ptr(g1),
+                  _ptr(g2), add.data_ptr(), dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), rows, C, pos_div,
+                  pos_mod, _ptr(_rope_table(freq, pos_mod)), s)
+
+
 def _dropout_seed(device) -> Tensor:
     """The seed of one attention call with dropout: one int64 (read by the kernels as a uint64) drawn from the current
     CUDA generator on the device, so torch.manual_seed governs the masks and a CUDA-graph replay, whose capture
@@ -952,6 +974,7 @@ def _dropout_seed(device) -> Tensor:
 class _SpaceAttnFn(torch.autograd.Function):
     """y = SDPA(q, q, q; scale, dropout_p) + x with q = LayerNorm(RoPE2d(x)), sequences = frames (H*W tokens).
     SpatialAttention.forward + the residual of SpaceTimeAttention.forward (attention.py:279-307, 470).
+    freq = None (embed=False) gives q = LayerNorm(x), through og_ln_rows_fwd / bwd.
     dropout > 0 runs og_flash_attn_dropout_fwd / bwd with a seed from _dropout_seed; 0 runs og_flash_attn_fwd / bwd."""
 
     @staticmethod
@@ -962,9 +985,7 @@ class _SpaceAttnFn(torch.autograd.Function):
         rows, S = B * T * H * W, H * W
         s = _stream()
         q = torch.empty_like(x)
-        tab = _rope_table(freq, S)
-        _lib.call('og_rope_ln_fwd', x.data_ptr(), freq.data_ptr(), gamma.data_ptr(), beta.data_ptr(), eps,
-                  q.data_ptr(), rows, C, 1, S, _ptr(tab), s)
+        _ln_rows_fwd(x, freq, gamma, beta, eps, q, rows, C, 1, S, s)
         y, o = torch.empty_like(x), torch.empty_like(x)
         lse = torch.empty((B * T, n_head, S), dtype=f32, device=x.device)
         seed = None
@@ -1002,9 +1023,7 @@ class _SpaceAttnFn(torch.autograd.Function):
         dx = torch.empty_like(x)
         dgamma = _zeros(C, f32, x.device)
         dbeta = _zeros(C, f32, x.device)
-        _lib.call('og_rope_ln_bwd', x.data_ptr(), freq.data_ptr(), gamma.data_ptr(), eps, dq.data_ptr(), dk.data_ptr(),
-                  dv.data_ptr(), dy.data_ptr(), dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), rows, C, 1, S,
-                  _ptr(_rope_table(freq, S)), s)
+        _ln_rows_bwd(x, freq, gamma, eps, dq, dk, dv, dy, dx, dgamma, dbeta, rows, C, 1, S, s)
         return dx, None, dgamma, dbeta, None, None, None, None
 
 
@@ -1025,6 +1044,7 @@ def _time_attn_tiled(T: int, C: int, n_head: int, dropout: float = 0.0) -> bool:
 class _TimeAttnFn(torch.autograd.Function):
     """y = SDPA_causal(q, k, v; scale, dropout_p) + x over t for every pixel; q = LayerNorm(RoPE1d(x)); k = v = q, or
     the projected latent-action conditioning (B, T, C) shared by all pixels (attention.py:347-371, 471).
+    freq = None (embed=False) gives q = LayerNorm(x), through og_ln_rows_fwd / bwd.
     dropout > 0 runs og_temporal_attn_long_dropout_fwd / bwd with a seed from _dropout_seed."""
 
     @staticmethod
@@ -1035,8 +1055,7 @@ class _TimeAttnFn(torch.autograd.Function):
         P = H * W
         s = _stream()
         q = torch.empty_like(x)
-        _lib.call('og_rope_ln_fwd', x.data_ptr(), freq.data_ptr(), gamma.data_ptr(), beta.data_ptr(), eps,
-                  q.data_ptr(), B * T * P, C, P, T, _ptr(_rope_table(freq, T)), s)
+        _ln_rows_fwd(x, freq, gamma, beta, eps, q, B * T * P, C, P, T, s)
         y = torch.empty_like(x)
         bcast = k_cond is not None
         if bcast:
@@ -1102,9 +1121,7 @@ class _TimeAttnFn(torch.autograd.Function):
         dx = torch.empty_like(x)
         dgamma = _zeros(C, f32, x.device)
         dbeta = _zeros(C, f32, x.device)
-        _lib.call('og_rope_ln_bwd', x.data_ptr(), freq.data_ptr(), gamma.data_ptr(), eps, dq.data_ptr(), _ptr(g1),
-                  _ptr(g2), dy.data_ptr(), dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), B * T * P, C, P, T,
-                  _ptr(_rope_table(freq, T)), s)
+        _ln_rows_bwd(x, freq, gamma, eps, dq, g1, g2, dy, dx, dgamma, dbeta, B * T * P, C, P, T, s)
         return dx, None, dgamma, dbeta, dkc, dvc, None, None, None, None
 
 
