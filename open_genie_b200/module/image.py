@@ -156,6 +156,10 @@ class ImageResidualBlock(nn.Module):
     def forward(self, inp: Tensor) -> Tensor:
         g1, c1, g2, c2 = self.main[0], self.main[2], self.main[3], self.main[5]
         G = g1.num_groups
+        if self._fusable and (self.inp_channel % 64 or self.out_channel % 64):
+            raise NotImplementedError(f'ImageResidualBlock({self.inp_channel}, {self.out_channel}): a block with a 1x1 '
+                                      f'shortcut runs it as extra K columns of the last convolution, which needs '
+                                      f'channel counts that are multiples of 64')
         if self._fusable and all((c // G) % 8 == 0 for c in (self.inp_channel, self.out_channel)):
             y, _ = ops.residual_block(inp, None, g1.weight, g1.bias, c1.weight, c1.bias, g2.weight, g2.bias, c2.weight,
                                       c2.bias, self.res.weight, self.res.bias, c1.packed(), c2.packed(), c1.geom, c2.geom,
@@ -163,6 +167,8 @@ class ImageResidualBlock(nn.Module):
             return y
         h = c1(g1(inp))
         h = g2(h)
+        if self._fusable:        # the shortcut's only bf16 weights are main[5]'s extra K columns (FusedAdamW writes those)
+            return c2(h, x2=inp)
         skip = self.res(inp) if isinstance(self.res, Conv2dParams) else inp
         if self.downsample:
             h = c2(h)

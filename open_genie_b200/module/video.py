@@ -280,6 +280,20 @@ def _conv_params(m: nn.Module) -> Conv3dParams:
     return m.conv3d if isinstance(m, CausalConv3d) else m
 
 
+def _handed_over_sums(x: Tensor):
+    """The GroupNorm(1) sums a fused block stored on its output x, if they still describe x: not after an in-place
+    edit of x (its version moved), and not after a step boundary of the zero arena that holds them (they may have
+    been zeroed). None means the consumer computes them itself. Inference tensors have no version counter, so
+    inference_mode forwards never hand sums over."""
+    handed = getattr(x, '_og_gn_sums', None)
+    if handed is None or x.is_inference():
+        return None
+    sums, version, arena, generation = handed
+    if x._version != version or (arena is not None and arena.generation != generation):
+        return None
+    return sums
+
+
 class VideoResidualBlock(nn.Module):
     """GN -> act -> conv -> GN -> act -> conv, plus an (always present) 1x1x1 conv shortcut —
     genie/module/video.py:539-656. state_dict keys: main.{0,4}.{weight,bias}, main.{2,6}.{weight,bias},
@@ -347,11 +361,15 @@ class VideoResidualBlock(nn.Module):
             # ride along on the tensor so that the next block's first GroupNorm needs no pass of its own.
             g1, g2 = self.main[0], self.main[4]
             ops._require_cuda(c1.weight, 'module parameters')
-            sums = getattr(inp, '_og_gn_sums', None) if g1.num_groups == 1 else None
+            sums = _handed_over_sums(inp) if g1.num_groups == 1 else None
             y, y_sums = ops.residual_block(inp, sums, g1.weight, g1.bias, c1.weight, c1.bias, g2.weight, g2.bias,
                                            c2.weight, c2.bias, cr.weight, cr.bias, c1.packed(), c2.packed(), c1.geom,
                                            c2.geom, g1.num_groups, g1.eps, act=self.act_fn)
-            y._og_gn_sums = y_sums
+            if not y.is_inference():
+                arena = ops.current_arena()
+                if arena is not None and arena.locate(y_sums) is None:
+                    arena = None
+                y._og_gn_sums = (y_sums, y._version, arena, arena.generation if arena is not None else None)
             return y
         h = self.main[0](inp)                # GN + act (fused)
         h = c1(h)                            # conv k3

@@ -57,9 +57,11 @@ class ZeroArena:
         self.bwd0 = {}       # device -> (segment, offset) of the first allocation made inside backward this step
         self.dirty = {}      # device -> a step boundary passed since the last allocation
         self.frozen = False
+        self.generation = 0  # step boundaries passed: a value kept with an arena tensor tells whether it may be stale
 
     # -- step boundary ---------------------------------------------------------------------------
     def mark_step(self):
+        self.generation += 1
         for d in self.dirty:
             self.dirty[d] = True
 
