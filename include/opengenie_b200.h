@@ -389,6 +389,17 @@ int og_flash_attn_dropout_fwd(const void* q, const void* k, const void* v, void*
 int og_flash_attn_dropout_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout,
                               const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq, int S, int C,
                               int n_head, float scale, float p, const uint64_t* seed, og_stream_t stream);
+/* Causal spatial attention: SDPA is_causal=True (attention.py:196, 229-234, 257-269: SpatialAttention(causal=True)),
+ * key j <= query i over the S tokens of a sequence in raster order. The arguments of og_flash_attn_fwd / bwd plus p and
+ * seed, with the status codes and messages of og_flash_attn_fwd / bwd. p = 0 runs without dropout and seed may be
+ * NULL; p > 0 drops after the causal mask with the mask and rules of og_flash_attn_dropout_fwd / bwd (-1 for a null
+ * seed or p outside [0, 1)). lse is the log-sum-exp over the keys j <= i. */
+int og_flash_attn_causal_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
+                             void* out_res, float* lse, int nseq, int S, int C, int n_head, float scale, float p,
+                             const uint64_t* seed, og_stream_t stream);
+int og_flash_attn_causal_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout,
+                             const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq, int S, int C,
+                             int n_head, float scale, float p, const uint64_t* seed, og_stream_t stream);
 
 /* Temporal attention, is_causal=True (attention.py:347-371, 423): one sequence per (batch, pixel), T <= 32
  * (longer clips, and d_head = 16 or 128 at any T: og_temporal_attn_long_fwd / bwd below). d_head 32 or 64; other
@@ -428,6 +439,18 @@ int og_temporal_attn_long_dropout_bwd(const void* q, const void* k, const void* 
                                       const float* lse, float* delta_ws, void* dq, void* dk, void* dv,
                                       float* dk_bcast, float* dv_bcast, int B, int T, int64_t P, int C, int n_head,
                                       float scale, int kv_bcast, float p, const uint64_t* seed, og_stream_t stream);
+/* Bidirectional temporal attention: SDPA is_causal=False over t (attention.py:196, 229-234, 325-337: TemporalAttention
+ * with the default causal=False, the blueprint name time_attn), every query sees all T keys, on the tiled kernels at
+ * every T >= 1. The arguments, layouts and status codes of og_temporal_attn_long_fwd / bwd plus p and seed: p = 0 runs
+ * without dropout and seed may be NULL; p > 0 drops with the mask and rules of og_temporal_attn_long_dropout_fwd / bwd
+ * (-1 for a null seed or p outside [0, 1)). */
+int og_temporal_attn_bidir_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
+                               void* out_res, float* lse, int B, int T, int64_t P, int C, int n_head, float scale,
+                               int kv_bcast, float p, const uint64_t* seed, og_stream_t stream);
+int og_temporal_attn_bidir_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout,
+                               const float* lse, float* delta_ws, void* dq, void* dk, void* dv, float* dk_bcast,
+                               float* dv_bcast, int B, int T, int64_t P, int C, int n_head, float scale, int kv_bcast,
+                               float p, const uint64_t* seed, og_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * DynamicsModel rows (genie/dynamics.py)

@@ -85,4 +85,15 @@ static inline int drop_params(float p, const uint64_t* seed, const char* who, Dr
   return OG_OK;
 }
 
+// The same for the entry points that also run without dropout (og_flash_attn_causal_*, og_temporal_attn_bidir_*):
+// p = 0 gives *drop = nullptr, the kernels without a mask, and the seed may be null; any other p is checked as above.
+static inline int drop_params_opt(float p, const uint64_t* seed, const char* who, DropParams* d,
+                                  const DropParams** drop) {
+  *drop = nullptr;
+  if (p == 0.f) return OG_OK;
+  if (const int r = drop_params(p, seed, who, d)) return r;
+  *drop = d;
+  return OG_OK;
+}
+
 }  // namespace og

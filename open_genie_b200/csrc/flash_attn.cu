@@ -1,4 +1,4 @@
-// flash_attn.cu — spatial (non-causal) multi-head attention, FlashAttention-style, on the Hopper tensor cores (wgmma).
+// flash_attn.cu — spatial multi-head attention (non-causal, and causal below), FlashAttention-style, on the Hopper tensor cores (wgmma).
 //
 // Reference: F.scaled_dot_product_attention(q, k, v, scale = n_head * d_head**-0.5) reached from
 // SpatialAttention.forward -> Attention.forward (genie/module/attention.py:279-307, 199-239), with
@@ -51,6 +51,16 @@
 // (1 / (1 - p) at the store) and masks dP^T; MODE 1 masks dP; the delta kernels are unchanged (O is the dropped output).
 // With kDrop off the kernels are instruction-identical to those before dropout. Registers (no spills): d = 16: fwd 72,
 // MODE 0 126, MODE 1 117; d = 64: fwd 130, MODE 0 182, MODE 1 154; d = 128: fwd 128, MODE 0 195, MODE 1 198.
+//
+// Causal (og_flash_attn_causal_fwd_kernel<d, drop>, og_flash_attn_causal_bwd_kernel<MODE, d, drop>; SDPA
+// is_causal=True, key j <= query i): the same bodies with kCausal set. The forward and MODE 1 (query tile i) walk key
+// tiles 0 .. i, MODE 0 (key tile j) walks query tiles j .. tiles - 1; the diagonal tile masks key > query (-inf in the
+// forward, P = 0 in the backward) on top of the ragged-S mask. Dropout, when set, applies to what the causal mask keeps
+// (the Philox mask is unchanged); the delta kernels are unchanged. Query tile i costs i + 1 key tiles, so blockIdx maps
+// the longest items first: qt descending (forward, MODE 1) or j ascending (MODE 0) as the slowest index, (sequence,
+// head) the fastest. With kCausal off the kernels are instruction-identical to those before the flag. Registers (no
+// spills), without / with dropout: d = 16: fwd 66 / 72, MODE 0 106 / 152, MODE 1 98 / 130; d = 64: fwd 98 / 130,
+// MODE 0 154 / 204, MODE 1 122 / 152; d = 128: fwd 138 / 130, MODE 0 160 / 207 (256 threads), MODE 1 154 / 220.
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 #include "attn_dropout.cuh"
@@ -164,7 +174,7 @@ __device__ __forceinline__ void load_rows(uint8_t* dst, const CUtensorMap* map, 
 }
 
 // Forward of one (sequence, head, 64-query tile) at head width kDh; O as kH fragments of 64 x kN.
-template <int kDh, bool kDrop = false>
+template <int kDh, bool kDrop = false, bool kCausal = false>
 __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtensorMap* mapK, const CUtensorMap* mapV,
                                           const FaParams& p, const DropParams* dr = nullptr) {
   using G = FaGeo<kDh>;
@@ -179,11 +189,19 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int id = blockIdx.x;
-  const int qt = id % p.q_tiles;
-  id /= p.q_tiles;
+  int qt;
+  if constexpr (kCausal) {   // query tile qt reads qt + 1 key tiles: the longest are scheduled first
+    const int nsh = p.nh * p.nseq;
+    qt = p.q_tiles - 1 - id / nsh;
+    id %= nsh;
+  } else {
+    qt = id % p.q_tiles;
+    id /= p.q_tiles;
+  }
   const int h = id % p.nh;
   const int seq = id / p.nh;
   const int q0 = qt * kTile;
+  const int n_kv = kCausal ? qt + 1 : p.kv_tiles;   // key tiles 0 .. n_kv - 1
 
   if (tid == 0) {
     tma_prefetch_desc(mapQ);
@@ -198,7 +216,7 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
   if (tid == 0) {
     mbar_expect_tx(q_full, kTB);
     load_rows<kDh>(sQ, mapQ, q_full, h, q0, seq);
-    for (int j = 0; j < 2 && j < p.kv_tiles; ++j) {
+    for (int j = 0; j < 2 && j < n_kv; ++j) {
       mbar_expect_tx(&kv_full[j], 2 * kTB);
       load_rows<kDh>(sKV + j * 2 * kTB, mapK, &kv_full[j], h, j * kTile, seq);
       load_rows<kDh>(sKV + j * 2 * kTB + kTB, mapV, &kv_full[j], h, j * kTile, seq);
@@ -217,7 +235,7 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
   uint2 dkey;
   if constexpr (kDrop) dkey = drop_key(dr->seed);
   mbar_wait(q_full, 0);
-  for (int j = 0; j < p.kv_tiles; ++j) {
+  for (int j = 0; j < n_kv; ++j) {
     const int st = j & 1;
     mbar_wait(&kv_full[st], (j >> 1) & 1);
     const uint32_t k_addr = smem_u32(sKV + st * 2 * kTB), v_addr = k_addr + kTB;
@@ -232,6 +250,13 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
 #pragma unroll
       for (int i = 0; i < 32; ++i)
         if ((i >> 2) * 8 + 2 * (lane & 3) + (i & 1) >= kv_valid) s[i] = -INFINITY;
+    }
+    if constexpr (kCausal) {   // the diagonal tile: keys after the query are out (key 0 stays in every row)
+      if (j == qt) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+          if ((i >> 2) * 8 + 2 * (lane & 3) + (i & 1) > warp * 16 + (lane >> 2) + 8 * ((i >> 1) & 1)) s[i] = -INFINITY;
+      }
     }
     float alpha[2];
 #pragma unroll
@@ -277,7 +302,7 @@ __device__ __forceinline__ void flash_fwd(const CUtensorMap* mapQ, const CUtenso
 #pragma unroll
     for (int c = 0; c < kH; ++c) reg_fence(o[c]);
     __syncthreads();  // every warp is done with stage st
-    if (tid == 0 && j + 2 < p.kv_tiles) {
+    if (tid == 0 && j + 2 < n_kv) {
       mbar_expect_tx(&kv_full[st], 2 * kTB);
       load_rows<kDh>(sKV + st * 2 * kTB, mapK, &kv_full[st], h, (j + 2) * kTile, seq);
       load_rows<kDh>(sKV + st * 2 * kTB + kTB, mapV, &kv_full[st], h, (j + 2) * kTile, seq);
@@ -347,13 +372,21 @@ __global__ void __launch_bounds__(kFaThreads)
   flash_fwd<kDh, true>(&mapQ, &mapK, &mapV, p, &d);
 }
 
+// causal (SDPA is_causal=True: key j <= query i), without (kDrop false) or with dropout, d_head = kDh
+template <int kDh, bool kDrop>
+__global__ void __launch_bounds__(kFaThreads)
+    og_flash_attn_causal_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                    const __grid_constant__ CUtensorMap mapV, const FaParams p, const DropParams d) {
+  flash_fwd<kDh, kDrop, true>(&mapQ, &mapK, &mapV, p, &d);
+}
+
 // ------------------------------------------------------------------------------------------------
 // backward (see the file header). The softmax scale is applied once per output element of dK / dQ, not per score.
 // kH = d_head / 64 at d = 64, 128 (1 at d = 16). MODE 0 at kH = 2 runs two warpgroups: both compute the full S^T and
 // dP^T (contracting over all 128 head dims), warpgroup w keeps dV and dK for head columns [64 w, 64 w + 64). MODE 1
 // keeps dQ as kH fragments.
 // ------------------------------------------------------------------------------------------------
-template <int MODE, int kDh, bool kDrop = false>
+template <int MODE, int kDh, bool kDrop = false, bool kCausal = false>
 __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtensorMap* mapK, const CUtensorMap* mapV,
                                           const CUtensorMap* mapDO, const FaBwdParams& p,
                                           const DropParams* dr = nullptr) {
@@ -375,8 +408,18 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
   const int tid = threadIdx.x, warp = (tid >> 5) & 3, lane = tid & 31;
   const int wg = MODE == 0 && kH == 2 ? tid >> 7 : 0;   // MODE 0 at d_head 128: the head-column half this thread owns
   int id = blockIdx.x;
-  const int own = id % p.tiles;  // MODE 0: kv tile ; MODE 1: q tile
-  id /= p.tiles;
+  int own;   // MODE 0: kv tile ; MODE 1: q tile
+  if constexpr (kCausal) {   // the longest first: MODE 0 key tile j reads tiles - j query tiles, MODE 1 query tile i
+    const int nsh = p.nh * p.nseq;   // reads i + 1 key tiles
+    own = MODE == 0 ? id / nsh : p.tiles - 1 - id / nsh;
+    id %= nsh;
+  } else {
+    own = id % p.tiles;
+    id /= p.tiles;
+  }
+  // streamed tiles it0 .. it0 + n_it - 1 (causal: MODE 0 the query tiles i >= j, MODE 1 the key tiles j <= i)
+  const int it0 = kCausal && MODE == 0 ? own : 0;
+  const int n_it = !kCausal ? p.tiles : MODE == 0 ? p.tiles - own : own + 1;
   const int h = id % p.nh;
   const int seq = id / p.nh;
   const long long stat0 = ((long long)seq * p.nh + h) * p.S;   // lse / delta row of this (sequence, head)
@@ -396,10 +439,10 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
     mbar_expect_tx(fix_full, 2 * kTB);
     load_rows<kDh>(sFix, mapF0, fix_full, h, own * kTile, seq);
     load_rows<kDh>(sFix + kTB, mapF1, fix_full, h, own * kTile, seq);
-    for (int it = 0; it < 2 && it < p.tiles; ++it) {
+    for (int it = 0; it < 2 && it < n_it; ++it) {
       mbar_expect_tx(&str_full[it], 2 * kTB);
-      load_rows<kDh>(sStr + it * 2 * kTB, mapS0, &str_full[it], h, it * kTile, seq);
-      load_rows<kDh>(sStr + it * 2 * kTB + kTB, mapS1, &str_full[it], h, it * kTile, seq);
+      load_rows<kDh>(sStr + it * 2 * kTB, mapS0, &str_full[it], h, (it0 + it) * kTile, seq);
+      load_rows<kDh>(sStr + it * 2 * kTB + kTB, mapS1, &str_full[it], h, (it0 + it) * kTile, seq);
     }
   }
   const float cl2 = p.scale * 1.4426950408889634f;
@@ -426,7 +469,7 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
   uint2 dkey;
   if constexpr (kDrop) dkey = drop_key(dr->seed);
   mbar_wait(fix_full, 0);
-  for (int it = 0; it < p.tiles; ++it) {
+  for (int it = 0; it < n_it; ++it) {
     const int st = it & 1;
     mbar_wait(&str_full[st], (it >> 1) & 1);
     const uint32_t s0 = smem_u32(sStr + st * 2 * kTB), s1 = s0 + kTB;
@@ -440,7 +483,7 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
     wgmma_wait<0>();
     reg_fence(s);
     reg_fence(dp);
-    const int row_tile = own, col_tile = it;
+    const int row_tile = own, col_tile = it0 + it;
     const bool rows_full = (row_tile + 1) * kTile <= p.S, cols_full = (col_tile + 1) * kTile <= p.S;
     uint32_t keep = 0;   // dropout: MODE 0 holds S^T (rows are keys), MODE 1 holds S
     if constexpr (kDrop)
@@ -464,6 +507,10 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
           if (!(rows_full && cols_full)) {
             const int row = row_tile * kTile + r_base + rr * 8;
             if (row >= p.S || col >= p.S) pv = 0.f;
+          }
+          if constexpr (kCausal) {   // the diagonal tile: no key after the query (MODE 0 rows are keys)
+            const int rl = r_base + rr * 8, cl = 8 * j + c_base + e;
+            if (row_tile == col_tile && (MODE == 0 ? rl > cl : cl > rl)) pv = 0.f;
           }
           if constexpr (kDrop) {   // dV takes P~ = P Z (1 / (1 - p) at the store); dS = P (dP Z - delta)
             const bool kp = (keep >> i) & 1u;
@@ -495,10 +542,10 @@ __device__ __forceinline__ void flash_bwd(const CUtensorMap* mapQ, const CUtenso
       reg_fence(acc1[c]);
     }
     __syncthreads();  // every warp is done with stage st
-    if (tid == 0 && it + 2 < p.tiles) {
+    if (tid == 0 && it + 2 < n_it) {
       mbar_expect_tx(&str_full[st], 2 * kTB);
-      load_rows<kDh>(sStr + st * 2 * kTB, mapS0, &str_full[st], h, (it + 2) * kTile, seq);
-      load_rows<kDh>(sStr + st * 2 * kTB + kTB, mapS1, &str_full[st], h, (it + 2) * kTile, seq);
+      load_rows<kDh>(sStr + st * 2 * kTB, mapS0, &str_full[st], h, (it0 + it + 2) * kTile, seq);
+      load_rows<kDh>(sStr + st * 2 * kTB + kTB, mapS1, &str_full[st], h, (it0 + it + 2) * kTile, seq);
     }
   }
   const long long row0 = (long long)seq * p.S + own * kTile;
@@ -545,6 +592,14 @@ __global__ void __launch_bounds__(MODE == 0 && kDh == 128 ? 2 * kFaThreads : kFa
                                      const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
                                      const FaBwdParams p, const DropParams d) {
   flash_bwd<MODE, kDh, true>(&mapQ, &mapK, &mapV, &mapDO, p, &d);
+}
+
+template <int MODE, int kDh, bool kDrop>
+__global__ void __launch_bounds__(MODE == 0 && kDh == 128 ? 2 * kFaThreads : kFaThreads)
+    og_flash_attn_causal_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                    const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapDO,
+                                    const FaBwdParams p, const DropParams d) {
+  flash_bwd<MODE, kDh, kDrop, true>(&mapQ, &mapK, &mapV, &mapDO, p, &d);
 }
 
 // delta[seq][h][s] = sum_d dO * O   (one warp per row, lanes over the head's 64 dims)
@@ -671,10 +726,58 @@ static int flash_dropout_bwd_launch(const CUtensorMap& mq, const CUtensorMap& mk
   return OG_OK;
 }
 
-// og_flash_attn_fwd, and og_flash_attn_dropout_fwd when `drop` is given
+// the causal kernels at d_head = kDh, with dropout when `drop` is given (shared memory as without the mask)
+template <int kDh>
+static int flash_causal_fwd_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv,
+                                   const FaParams& p, const DropParams* drop, unsigned grid, cudaStream_t s) {
+  const size_t smem_bytes = 5 * FaGeo<kDh>::kTB + 1024 + 64;
+  static bool attr = false;
+  if (!attr) {
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_causal_fwd_kernel<kDh, false>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_causal_fwd_kernel<kDh, true>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    attr = true;
+  }
+  if (drop)
+    og_flash_attn_causal_fwd_kernel<kDh, true><<<grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, p, *drop);
+  else
+    og_flash_attn_causal_fwd_kernel<kDh, false><<<grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, p, DropParams{});
+  return OG_OK;
+}
+
+template <int kDh, bool kDrop>
+static int flash_causal_bwd_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv,
+                                   const CUtensorMap& mdo, const FaBwdParams& p, const DropParams& d, unsigned grid,
+                                   cudaStream_t s) {
+  const size_t smem_bytes = 6 * FaGeo<kDh>::kTB + 1024 + 64;
+  static bool attr = false;
+  if (!attr) {
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_causal_bwd_kernel<0, kDh, kDrop>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_flash_attn_causal_bwd_kernel<1, kDh, kDrop>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    attr = true;
+  }
+  og_flash_attn_causal_bwd_kernel<0, kDh, kDrop><<<grid, kDh == 128 ? 2 * kFaThreads : kFaThreads, smem_bytes, s>>>(
+      mq, mk, mv, mdo, p, d);
+  OG_CHECK_CUDA(cudaGetLastError());
+  og_flash_attn_causal_bwd_kernel<1, kDh, kDrop><<<grid, kFaThreads, smem_bytes, s>>>(mq, mk, mv, mdo, p, d);
+  return OG_OK;
+}
+
+template <int kDh>
+static int flash_causal_bwd_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv,
+                                   const CUtensorMap& mdo, const FaBwdParams& p, const DropParams* drop, unsigned grid,
+                                   cudaStream_t s) {
+  return drop ? flash_causal_bwd_launch<kDh, true>(mq, mk, mv, mdo, p, *drop, grid, s)
+              : flash_causal_bwd_launch<kDh, false>(mq, mk, mv, mdo, p, DropParams{}, grid, s);
+}
+
+// og_flash_attn_fwd, og_flash_attn_dropout_fwd when `drop` is given, og_flash_attn_causal_fwd when `causal` is set
 static int flash_fwd_call(const void* q, const void* k, const void* v, void* out, const void* residual, void* out_res,
                           float* lse, int nseq, int S, int C, int n_head, float scale, const DropParams* drop,
-                          og_stream_t stream) {
+                          og_stream_t stream, bool causal = false) {
   OG_REQUIRE(q && k && v && out, "flash_attn_fwd: null pointer");
   const int dh = flash_d_head(C, n_head);
   OG_REQUIRE(dh != 0, "flash_attn_fwd: needs d_head = 64, 128 or 16 (C=%d, n_head=%d)", C, n_head);
@@ -697,7 +800,12 @@ static int flash_fwd_call(const void* q, const void* k, const void* v, void* out
   if ((r = make_seq_map(&mv, v, nseq, S, C, dh)) != OG_OK) return r;
   const long long grid = (long long)nseq * n_head * p.q_tiles;
   OG_REQUIRE(grid < (1LL << 31), "flash_attn_fwd: too many tiles");
-  if (drop) {
+  if (causal) {
+    const int r2 = dh == 64    ? flash_causal_fwd_launch<64>(mq, mk, mv, p, drop, (unsigned)grid, (cudaStream_t)stream)
+                   : dh == 128 ? flash_causal_fwd_launch<128>(mq, mk, mv, p, drop, (unsigned)grid, (cudaStream_t)stream)
+                               : flash_causal_fwd_launch<16>(mq, mk, mv, p, drop, (unsigned)grid, (cudaStream_t)stream);
+    if (r2 != OG_OK) return r2;
+  } else if (drop) {
     const int r2 = dh == 64    ? flash_dropout_fwd_launch<64>(mq, mk, mv, p, *drop, (unsigned)grid, (cudaStream_t)stream)
                    : dh == 128 ? flash_dropout_fwd_launch<128>(mq, mk, mv, p, *drop, (unsigned)grid, (cudaStream_t)stream)
                                : flash_dropout_fwd_launch<16>(mq, mk, mv, p, *drop, (unsigned)grid, (cudaStream_t)stream);
@@ -743,10 +851,10 @@ extern "C" int og_flash_attn_dropout_fwd(const void* q, const void* k, const voi
   return flash_fwd_call(q, k, v, out, residual, out_res, lse, nseq, S, C, n_head, scale, &d, stream);
 }
 
-// og_flash_attn_bwd, and og_flash_attn_dropout_bwd when `drop` is given
+// og_flash_attn_bwd, og_flash_attn_dropout_bwd when `drop` is given, og_flash_attn_causal_bwd when `causal` is set
 static int flash_bwd_call(const void* q, const void* k, const void* v, const void* out, const void* dout,
                           const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq, int S, int C,
-                          int n_head, float scale, const DropParams* drop, og_stream_t stream) {
+                          int n_head, float scale, const DropParams* drop, og_stream_t stream, bool causal = false) {
   OG_REQUIRE(q && k && v && out && dout && lse && delta_ws && dq && dk && dv, "flash_attn_bwd: null pointer");
   const int dh = flash_d_head(C, n_head);
   OG_REQUIRE(dh != 0, "flash_attn_bwd: needs d_head = 64, 128 or 16 (C=%d, n_head=%d)", C, n_head);
@@ -785,7 +893,12 @@ static int flash_bwd_call(const void* q, const void* k, const void* v, const voi
   if ((r = make_seq_map(&mdo, dout, nseq, S, C, dh)) != OG_OK) return r;
   const long long grid = (long long)nseq * n_head * p.tiles;
   OG_REQUIRE(grid < (1LL << 31), "flash_attn_bwd: too many tiles");
-  if (drop) {
+  if (causal) {
+    const int r2 = dh == 64    ? flash_causal_bwd_launch<64>(mq, mk, mv, mdo, p, drop, (unsigned)grid, s)
+                   : dh == 128 ? flash_causal_bwd_launch<128>(mq, mk, mv, mdo, p, drop, (unsigned)grid, s)
+                               : flash_causal_bwd_launch<16>(mq, mk, mv, mdo, p, drop, (unsigned)grid, s);
+    if (r2 != OG_OK) return r2;
+  } else if (drop) {
     const int r2 = dh == 64    ? flash_dropout_bwd_launch<64>(mq, mk, mv, mdo, p, *drop, (unsigned)grid, s)
                    : dh == 128 ? flash_dropout_bwd_launch<128>(mq, mk, mv, mdo, p, *drop, (unsigned)grid, s)
                                : flash_dropout_bwd_launch<16>(mq, mk, mv, mdo, p, *drop, (unsigned)grid, s);
@@ -840,4 +953,23 @@ extern "C" int og_flash_attn_dropout_bwd(const void* q, const void* k, const voi
   DropParams d;
   if (const int r = drop_params(p, seed, "flash_attn_dropout_bwd", &d)) return r;
   return flash_bwd_call(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, nseq, S, C, n_head, scale, &d, stream);
+}
+
+extern "C" int og_flash_attn_causal_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
+                                        void* out_res, float* lse, int nseq, int S, int C, int n_head, float scale,
+                                        float p, const uint64_t* seed, og_stream_t stream) {
+  DropParams d;
+  const DropParams* drop;
+  if (const int r = drop_params_opt(p, seed, "flash_attn_causal_fwd", &d, &drop)) return r;
+  return flash_fwd_call(q, k, v, out, residual, out_res, lse, nseq, S, C, n_head, scale, drop, stream, true);
+}
+
+extern "C" int og_flash_attn_causal_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout,
+                                        const float* lse, float* delta_ws, void* dq, void* dk, void* dv, int nseq,
+                                        int S, int C, int n_head, float scale, float p, const uint64_t* seed,
+                                        og_stream_t stream) {
+  DropParams d;
+  const DropParams* drop;
+  if (const int r = drop_params_opt(p, seed, "flash_attn_causal_bwd", &d, &drop)) return r;
+  return flash_bwd_call(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, nseq, S, C, n_head, scale, drop, stream, true);
 }

@@ -1,4 +1,4 @@
-// temporal_attn_long.cu — temporal (causal, d_head = 16, 64 or 128) attention for clips of any length: FlashAttention-2
+// temporal_attn_long.cu — temporal (causal or bidirectional, d_head = 16, 64 or 128) attention for clips of any length: FlashAttention-2
 // on mma.sync m16n8k16, tiled over queries and keys, online softmax in fp32.
 //
 // STATUS: checked by tests/test_gpu_temporal_long.py (kernel level against float64 for T = 1 .. 1024, model level
@@ -46,6 +46,14 @@
 // masks dP; dK / dV takes P Z for dV (1 / (1 - p) at the store or the atomic flush) and masks dP^T. With kDrop off the
 // kernels are instruction-identical to those before dropout. Registers (no spills): D = 16: fwd 78, dQ 127, dK/dV 168;
 // D = 64: fwd 128, dQ 168, dK/dV 237; D = 128: fwd 168, dQ 240, dK/dV 238 (256 threads).
+// Bidirectional (og_temporal_attn_bidir_{fwd,bwd_dq,bwd_dkdv}_kernel<D, drop>; SDPA is_causal=False over t, the
+// reference TemporalAttention's default): the same bodies with kCausal off. The forward and dQ walk every key tile, dK /
+// dV every query tile (also on the kv_bcast chunked path). Rows >= T are zero-filled, so a padded key would score 0,
+// not -inf: the last key tile masks keys >= T explicitly (the causal kernels never reach them). Padded query rows need
+// no mask in dK / dV: their Q, dO, lse and delta are zero-filled, so P^T dO and dS vanish there. With kCausal on the
+// kernels are instruction-identical to those before the flag. Registers (no spills), without / with dropout: D = 16:
+// fwd 72 / 80, dQ 92 / 128, dK/dV 80 / 128; D = 64: fwd 128 / 130, dQ 167 / 165, dK/dV 168 / 242; D = 128: fwd 167 /
+// 168, dQ 246 / 233, dK/dV 234 / 254 (256 threads).
 #include "og_host.cuh"
 #include "og_ptx.cuh"
 #include "temporal_mma_frag.cuh"
@@ -202,9 +210,10 @@ __device__ __forceinline__ Seq decode(long long task, int T, long long P, int C,
   return s;
 }
 
-// Kernel bodies, templated on the head width and on dropout (attn_dropout.cuh; without it they are the kernels as they
-// were before dropout). The __global__ wrappers follow each body.
-template <int D, bool kDrop>
+// Kernel bodies, templated on the head width, on dropout (attn_dropout.cuh; without it they are the kernels as they
+// were before dropout) and on the causal mask (kCausal false: bidirectional, every query sees all T keys). The
+// __global__ wrappers follow each body.
+template <int D, bool kDrop, bool kCausal = true>
 __device__ __forceinline__ void long_fwd_body(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                      const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ res,
                                      __nv_bfloat16* __restrict__ out, __nv_bfloat16* __restrict__ out_res,
@@ -239,10 +248,11 @@ __device__ __forceinline__ void long_fwd_body(const __nv_bfloat16* __restrict__ 
   for (int nt = 0; nt < kNT; ++nt)
 #pragma unroll
     for (int e = 0; e < 4; ++e) o[nt][e] = 0.f;
-  for (int j = 0; j <= i; ++j) {
+  const int jl = kCausal ? i : tiles - 1;   // the last key tile this query tile reads
+  for (int j = 0; j <= jl; ++j) {
     cp_async_wait_all();
     __syncthreads();   // tile j has landed for every thread; every warp is done with tile j - 1
-    if (j < i) {
+    if (j < jl) {
       uint8_t* nx = ring + ((j + 1) & 1) * 2 * kTileBytes;
       load_tile<D>(nx, k + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
       load_tile<D>(nx + kTileBytes, v + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
@@ -251,8 +261,9 @@ __device__ __forceinline__ void long_fwd_body(const __nv_bfloat16* __restrict__ 
     const uint8_t* ks = ring + (j & 1) * 2 * kTileBytes;
     float s[4][2][4];
     gemm_nt<D>(s, qw, ks, lane);
-    // scores in the log2 domain; the diagonal tile masks keys after the query. Key 0 is in every row of tile 0, so
-    // the row maximum is finite from the first tile on.
+    // scores in the log2 domain; the diagonal tile masks keys after the query (bidirectional: the last tile masks the
+    // zero-filled keys >= T, whose scores would be 0). Key 0 is in every row of tile 0, so the row maximum is finite
+    // from the first tile on.
     float mx[2] = {m[0], m[1]};
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt)
@@ -260,7 +271,7 @@ __device__ __forceinline__ void long_fwd_body(const __nv_bfloat16* __restrict__ 
       for (int e = 0; e < 4; ++e) {
         const int rr = e >> 1, col = j * kTile + nt * 8 + 2 * qd + (e & 1);
         float x = s[nt >> 1][nt & 1][e] * cl2;
-        if (j == i && col > row0 + 8 * rr) x = -INFINITY;
+        if (kCausal ? j == i && col > row0 + 8 * rr : j == jl && col >= T) x = -INFINITY;
         s[nt >> 1][nt & 1][e] = x;
         mx[rr] = fmaxf(mx[rr], x);
       }
@@ -306,9 +317,9 @@ __device__ __forceinline__ void long_fwd_body(const __nv_bfloat16* __restrict__ 
     inv[0] *= dr->rscale;
     inv[1] *= dr->rscale;
   }
-  // fp32 staging of the normalised output in the ring stage the loop no longer reads (its last tile, i - 1, was
+  // fp32 staging of the normalised output in the ring stage the loop no longer reads (its last tile, jl - 1, was
   // finished by every warp before the last barrier); each warp writes and reads only its own 16 rows
-  uint8_t* st = ring + ((i + 1) & 1) * 2 * kTileBytes + warp * 16 * kFPitch;
+  uint8_t* st = ring + ((jl + 1) & 1) * 2 * kTileBytes + warp * 16 * kFPitch;
 #pragma unroll
   for (int nt = 0; nt < kNT; ++nt)
 #pragma unroll
@@ -364,7 +375,7 @@ __global__ void __launch_bounds__(kThreads)
   long_fwd_body<D, true>(q, k, v, res, out, out_res, lse, B, T, P, C, nh, scale, kv_bcast, tiles, &d);
 }
 
-template <int D, bool kDrop>
+template <int D, bool kDrop, bool kCausal = true>
 __device__ __forceinline__ void long_dq_body(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                         const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ o,
                                         const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse,
@@ -427,10 +438,11 @@ __device__ __forceinline__ void long_dq_body(const __nv_bfloat16* __restrict__ q
   for (int nt = 0; nt < kNT; ++nt)
 #pragma unroll
     for (int e = 0; e < 4; ++e) acc[nt][e] = 0.f;
-  for (int j = 0; j <= i; ++j) {
+  const int jl = kCausal ? i : tiles - 1;
+  for (int j = 0; j <= jl; ++j) {
     cp_async_wait_all();
     __syncthreads();
-    if (j < i) {
+    if (j < jl) {
       uint8_t* nx = ring + ((j + 1) & 1) * 2 * kTileBytes;
       load_tile<D>(nx, k + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
       load_tile<D>(nx + kTileBytes, v + sq.k0, sq.kpitch, (j + 1) * kTile, T, tid);
@@ -449,7 +461,8 @@ __device__ __forceinline__ void long_dq_body(const __nv_bfloat16* __restrict__ q
       for (int e = 0; e < 4; ++e) {
         const int rr = e >> 1, col = j * kTile + nt * 8 + 2 * qd + (e & 1);
         float p = ex2_approx(fmaf(s[nt >> 1][nt & 1][e], cl2, -lse2[rr]));
-        if (j == i && col > row0 + 8 * rr) p = 0.f;
+        // bidirectional: keys >= T are zero rows, with P = 2^-lse and dP = 0 they would add -P delta K
+        if (kCausal ? j == i && col > row0 + 8 * rr : j == jl && col >= T) p = 0.f;
         if constexpr (kDrop) {   // dS = P (dP Z - delta)
           const float d = (keep >> (4 * nt + e)) & 1u ? dp[nt >> 1][nt & 1][e] * dr->rscale : 0.f;
           s[nt >> 1][nt & 1][e] = p * (d - dl[rr]);
@@ -491,7 +504,7 @@ __global__ void __launch_bounds__(kThreads)
 // D = 128: eight warps; warps w and w + 4 own the same 16 key rows, each computes the full S^T and dP^T (over all 128
 // dims) and keeps dK / dV for head columns [64 (w / 4), 64 (w / 4) + 64) only, so a lane holds 2 x 32 accumulators
 // as at D = 64.
-template <int D, bool kDrop>
+template <int D, bool kDrop, bool kCausal = true>
 __device__ __forceinline__ void long_dkdv_body(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                                           const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ dout,
                                           const float* __restrict__ lse, const float* __restrict__ delta,
@@ -513,13 +526,15 @@ __device__ __forceinline__ void long_dkdv_body(const __nv_bfloat16* __restrict__
   const int j = (int)(blockIdx.x / per_j);   // key tile; the longest (j = 0) are scheduled first
   const long long rest = blockIdx.x % per_j, bh = rest / nchunk;
   const long long p0 = (rest % nchunk) * chunk, p1 = p0 + chunk < P ? p0 + chunk : P;
-  const int nq = tiles - j;                  // query tiles i = j .. tiles - 1 per pixel
+  // query tiles i = i0 .. tiles - 1 per pixel: i0 = j, or 0 when bidirectional. Query rows >= T need no mask: their Q
+  // and dO rows are zero-filled and so are their lse and delta, so P = 1 there but P^T dO = 0 and dS = 0.
+  const int i0 = kCausal ? j : 0, nq = tiles - i0;
   const long long items = (p1 - p0) * nq;
   const Seq s0 = decode(bh * P + p0, T, P, C, nh, D, kv_bcast);
   const long long qpitch = P * C;
   auto load_item = [&](long long n, int stage) {
     const long long task = bh * P + p0 + n / nq;
-    const int i = j + (int)(n % nq);
+    const int i = i0 + (int)(n % nq);
     const long long q0 = s0.q0 + (task - s0.task) * C;   // the pixels of one (b, h) are C elements apart
     uint8_t* st = ring + stage * kStage;
     load_tile<D, NTHR>(st, q + q0, qpitch, i * kTile, T, tid);
@@ -555,7 +570,7 @@ __device__ __forceinline__ void long_dkdv_body(const __nv_bfloat16* __restrict__
     const uint8_t* dosn = st + kTileBytes;
     const float* lse_s = reinterpret_cast<const float*>(st + 2 * kTileBytes);
     const float* del_s = reinterpret_cast<const float*>(st + 2 * kTileBytes + kVecBytes);
-    const int i = j + (int)(n % nq);
+    const int i = i0 + (int)(n % nq);
     // transposed products: rows = this warp's keys, columns = the 64 queries of tile i
     float s[4][2][4], dp[4][2][4];
     gemm_nt<D>(s, kw, qsn, lane);
@@ -573,7 +588,7 @@ __device__ __forceinline__ void long_dkdv_body(const __nv_bfloat16* __restrict__
       for (int e = 0; e < 4; ++e) {
         const int rr = e >> 1, ce = e & 1;
         float p = ex2_approx(fmaf(s[nt >> 1][nt & 1][e], cl2, -(ce ? ls.y : ls.x) * kLog2e));
-        if (i == j && i * kTile + c + ce < key0 + 8 * rr) p = 0.f;
+        if (kCausal && i == j && i * kTile + c + ce < key0 + 8 * rr) p = 0.f;
         if constexpr (kDrop) {   // dV takes P~ = P Z (1 / (1 - p) at the flush); dS = P (dP Z - delta)
           const bool kp = (keep >> (4 * nt + e)) & 1u;
           s[nt >> 1][nt & 1][e] = kp ? p : 0.f;
@@ -646,6 +661,41 @@ __global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
                           nchunk, &d);
 }
 
+// bidirectional (SDPA is_causal=False over t), without (kDrop false) or with dropout
+template <int D, bool kDrop>
+__global__ void __launch_bounds__(kThreads)
+    og_temporal_attn_bidir_fwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                      const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ res,
+                                      __nv_bfloat16* __restrict__ out, __nv_bfloat16* __restrict__ out_res,
+                                      float* __restrict__ lse, int B, int T, long long P, int C, int nh, float scale,
+                                      int kv_bcast, int tiles, const DropParams d) {
+  long_fwd_body<D, kDrop, false>(q, k, v, res, out, out_res, lse, B, T, P, C, nh, scale, kv_bcast, tiles, &d);
+}
+
+template <int D, bool kDrop>
+__global__ void __launch_bounds__(kThreads)
+    og_temporal_attn_bidir_bwd_dq_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                         const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ o,
+                                         const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse,
+                                         float* __restrict__ delta, __nv_bfloat16* __restrict__ dq, int B, int T,
+                                         long long P, int C, int nh, float scale, int kv_bcast, int tiles,
+                                         const DropParams d) {
+  long_dq_body<D, kDrop, false>(q, k, v, o, dout, lse, delta, dq, B, T, P, C, nh, scale, kv_bcast, tiles, &d);
+}
+
+template <int D, bool kDrop>
+__global__ void __launch_bounds__(Geo<D>::kDkdvThreads)
+    og_temporal_attn_bidir_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                           const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ dout,
+                                           const float* __restrict__ lse, const float* __restrict__ delta,
+                                           __nv_bfloat16* __restrict__ dk, __nv_bfloat16* __restrict__ dv,
+                                           float* __restrict__ dk_b, float* __restrict__ dv_b, int B, int T,
+                                           long long P, int C, int nh, float scale, int kv_bcast, int tiles,
+                                           long long chunk, long long nchunk, const DropParams d) {
+  long_dkdv_body<D, kDrop, false>(q, k, v, dout, lse, delta, dk, dv, dk_b, dv_b, B, T, P, C, nh, scale, kv_bcast,
+                                  tiles, chunk, nchunk, &d);
+}
+
 }  // namespace tlong
 
 }  // namespace og
@@ -655,11 +705,63 @@ using namespace og;
 static bool long_aligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 namespace {
+// the bidirectional kernels at head width D, with dropout when kDrop is set (shared memory as for the causal ones)
+template <int D, bool kDrop>
+int bidir_fwd(const void* q, const void* k, const void* v, void* out, const void* residual, void* out_res, float* lse,
+              int B, int T, int64_t P, int C, int n_head, float scale, int kv_bcast, int tiles, long long grid,
+              const DropParams& d, cudaStream_t stream) {
+  using namespace og::tlong;
+  static bool attr = false;
+  if (!attr) {
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_bidir_fwd_kernel<D, kDrop>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Geo<D>::kFwdSmem));
+    attr = true;
+  }
+  og_temporal_attn_bidir_fwd_kernel<D, kDrop><<<(unsigned)grid, kThreads, Geo<D>::kFwdSmem, stream>>>(
+      (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)residual,
+      (__nv_bfloat16*)out, (__nv_bfloat16*)out_res, lse, B, T, P, C, n_head, scale, kv_bcast, tiles, d);
+  OG_CHECK_CUDA(cudaGetLastError());
+  return OG_OK;
+}
+
+template <int D, bool kDrop>
+int bidir_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout, const float* lse,
+              float* delta_ws, void* dq, void* dk, void* dv, float* dk_bcast, float* dv_bcast, int B, int T, int64_t P,
+              int C, int n_head, float scale, int kv_bcast, int tiles, long long chunk, long long nchunk,
+              const DropParams& d, cudaStream_t s) {
+  using namespace og::tlong;
+  static bool attr = false;
+  if (!attr) {
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_bidir_bwd_dq_kernel<D, kDrop>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Geo<D>::kDqSmem));
+    OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_bidir_bwd_dkdv_kernel<D, kDrop>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Geo<D>::kDkdvSmem));
+    attr = true;
+  }
+  const long long ntask = (long long)B * n_head * P;
+  og_temporal_attn_bidir_bwd_dq_kernel<D, kDrop><<<(unsigned)(ntask * tiles), kThreads, Geo<D>::kDqSmem, s>>>(
+      (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)out,
+      (const __nv_bfloat16*)dout, lse, delta_ws, (__nv_bfloat16*)dq, B, T, P, C, n_head, scale, kv_bcast, tiles, d);
+  OG_CHECK_CUDA(cudaGetLastError());
+  const long long grid = (long long)B * n_head * nchunk * tiles;
+  og_temporal_attn_bidir_bwd_dkdv_kernel<D, kDrop><<<(unsigned)grid, Geo<D>::kDkdvThreads, Geo<D>::kDkdvSmem, s>>>(
+      (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)dout, lse,
+      delta_ws, (__nv_bfloat16*)dk, (__nv_bfloat16*)dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale, kv_bcast, tiles,
+      chunk, nchunk, d);
+  OG_CHECK_CUDA(cudaGetLastError());
+  return OG_OK;
+}
+
 template <int D>
 int long_fwd(const void* q, const void* k, const void* v, void* out, const void* residual, void* out_res, float* lse,
              int B, int T, int64_t P, int C, int n_head, float scale, int kv_bcast, int tiles, long long grid,
-             const DropParams* drop, cudaStream_t stream) {
+             const DropParams* drop, cudaStream_t stream, bool causal) {
   using namespace og::tlong;
+  if (!causal)
+    return drop ? bidir_fwd<D, true>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast, tiles,
+                                     grid, *drop, stream)
+                : bidir_fwd<D, false>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast, tiles,
+                                      grid, DropParams{}, stream);
   if (drop) {
     static bool dattr = false;
     if (!dattr) {
@@ -689,9 +791,30 @@ int long_fwd(const void* q, const void* k, const void* v, void* out, const void*
 template <int D>
 int long_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout, const float* lse,
              float* delta_ws, void* dq, void* dk, void* dv, float* dk_bcast, float* dv_bcast, int B, int T, int64_t P,
-             int C, int n_head, float scale, int kv_bcast, int tiles, const DropParams* drop, cudaStream_t s) {
+             int C, int n_head, float scale, int kv_bcast, int tiles, const DropParams* drop, cudaStream_t s,
+             bool causal) {
   using namespace og::tlong;
   const long long ntask = (long long)B * n_head * P;
+  // dK / dV: one pixel per CTA, or with kv_bcast contiguous pixel chunks of one (b, h), enough of them for ~4 CTAs
+  // per SM
+  long long chunk = 1, nchunk = P;
+  if (kv_bcast) {
+    const long long bht = (long long)B * n_head * tiles;
+    long long want = ((long long)num_sms() * 4 + bht - 1) / bht;
+    if (want < 1) want = 1;
+    if (want > P) want = P;
+    chunk = (P + want - 1) / want;
+    nchunk = (P + chunk - 1) / chunk;
+  }
+  if (!causal) {   // dQ first: it also writes delta, which the dK / dV kernel reads
+    const int r = drop ? bidir_bwd<D, true>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P,
+                                            C, n_head, scale, kv_bcast, tiles, chunk, nchunk, *drop, s)
+                       : bidir_bwd<D, false>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T,
+                                             P, C, n_head, scale, kv_bcast, tiles, chunk, nchunk, DropParams{}, s);
+    if (r != OG_OK) return r;
+    g_launches.fetch_add(2);
+    return OG_OK;
+  }
   static bool attr = false, dattr = false;
   if (drop && !dattr) {
     OG_CHECK_CUDA(cudaFuncSetAttribute(og_temporal_attn_long_dropout_bwd_dq_kernel<D>,
@@ -719,17 +842,6 @@ int long_bwd(const void* q, const void* k, const void* v, const void* out, const
         (const __nv_bfloat16*)dout, lse, delta_ws, (__nv_bfloat16*)dq, B, T, P, C, n_head, scale, kv_bcast, tiles);
   OG_CHECK_CUDA(cudaGetLastError());
   g_launches.fetch_add(1);
-  // dK / dV: one pixel per CTA, or with kv_bcast contiguous pixel chunks of one (b, h), enough of them for ~4 CTAs
-  // per SM
-  long long chunk = 1, nchunk = P;
-  if (kv_bcast) {
-    const long long bht = (long long)B * n_head * tiles;
-    long long want = ((long long)num_sms() * 4 + bht - 1) / bht;
-    if (want < 1) want = 1;
-    if (want > P) want = P;
-    chunk = (P + want - 1) / want;
-    nchunk = (P + chunk - 1) / chunk;
-  }
   const long long grid = (long long)B * n_head * nchunk * tiles;
   if (drop)
     og_temporal_attn_long_dropout_bwd_dkdv_kernel<D><<<(unsigned)grid, Geo<D>::kDkdvThreads, Geo<D>::kDkdvSmem, s>>>(
@@ -747,10 +859,11 @@ int long_bwd(const void* q, const void* k, const void* v, const void* out, const
 }
 }  // namespace
 
-// og_temporal_attn_long_fwd, and og_temporal_attn_long_dropout_fwd when `drop` is given
+// og_temporal_attn_long_fwd, og_temporal_attn_long_dropout_fwd when `drop` is given, og_temporal_attn_bidir_fwd
+// when `causal` is false
 static int long_fwd_call(const void* q, const void* k, const void* v, void* out, const void* residual, void* out_res,
                          float* lse, int B, int T, int64_t P, int C, int n_head, float scale, int kv_bcast,
-                         const DropParams* drop, og_stream_t stream) {
+                         const DropParams* drop, og_stream_t stream, bool causal = true) {
   using namespace og::tlong;
   OG_REQUIRE(q && k && v && out && lse, "temporal_attn_long_fwd: null pointer");
   OG_REQUIRE(!residual == !out_res, "temporal_attn_long_fwd: residual and out_res must be given together");
@@ -770,11 +883,11 @@ static int long_fwd_call(const void* q, const void* k, const void* v, void* out,
   const long long grid = (long long)B * n_head * P * tiles;
   OG_REQUIRE(grid < (1LL << 31), "temporal_attn_long_fwd: too many tiles");
   const int r = dh == 64    ? long_fwd<64>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
-                                           tiles, grid, drop, (cudaStream_t)stream)
+                                           tiles, grid, drop, (cudaStream_t)stream, causal)
                  : dh == 128 ? long_fwd<128>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
-                                             tiles, grid, drop, (cudaStream_t)stream)
+                                             tiles, grid, drop, (cudaStream_t)stream, causal)
                              : long_fwd<16>(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast,
-                                            tiles, grid, drop, (cudaStream_t)stream);
+                                            tiles, grid, drop, (cudaStream_t)stream, causal);
   if (r != OG_OK) return r;
   g_launches.fetch_add(1);
   return OG_OK;
@@ -795,11 +908,12 @@ extern "C" int og_temporal_attn_long_dropout_fwd(const void* q, const void* k, c
   return long_fwd_call(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast, &d, stream);
 }
 
-// og_temporal_attn_long_bwd, and og_temporal_attn_long_dropout_bwd when `drop` is given
+// og_temporal_attn_long_bwd, og_temporal_attn_long_dropout_bwd when `drop` is given, og_temporal_attn_bidir_bwd
+// when `causal` is false
 static int long_bwd_call(const void* q, const void* k, const void* v, const void* out, const void* dout,
                          const float* lse, float* delta_ws, void* dq, void* dk, void* dv, float* dk_bcast,
                          float* dv_bcast, int B, int T, int64_t P, int C, int n_head, float scale, int kv_bcast,
-                         const DropParams* drop, og_stream_t stream) {
+                         const DropParams* drop, og_stream_t stream, bool causal = true) {
   using namespace og::tlong;
   OG_REQUIRE(q && k && v && out && dout && lse && delta_ws && dq, "temporal_attn_long_bwd: null pointer");
   OG_REQUIRE(kv_bcast ? (dk_bcast && dv_bcast) : (dk && dv), "temporal_attn_long_bwd: missing dk/dv buffers");
@@ -820,11 +934,11 @@ static int long_bwd_call(const void* q, const void* k, const void* v, const void
   OG_REQUIRE(ntask * tiles < (1LL << 31), "temporal_attn_long_bwd: too many tiles");
   if (dh == 16)
     return long_bwd<16>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale,
-                        kv_bcast, tiles, drop, (cudaStream_t)stream);
+                        kv_bcast, tiles, drop, (cudaStream_t)stream, causal);
   return dh == 64 ? long_bwd<64>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C,
-                                 n_head, scale, kv_bcast, tiles, drop, (cudaStream_t)stream)
+                                 n_head, scale, kv_bcast, tiles, drop, (cudaStream_t)stream, causal)
                   : long_bwd<128>(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C,
-                                  n_head, scale, kv_bcast, tiles, drop, (cudaStream_t)stream);
+                                  n_head, scale, kv_bcast, tiles, drop, (cudaStream_t)stream, causal);
 }
 
 extern "C" int og_temporal_attn_long_bwd(const void* q, const void* k, const void* v, const void* out,
@@ -844,4 +958,25 @@ extern "C" int og_temporal_attn_long_dropout_bwd(const void* q, const void* k, c
   if (const int r = drop_params(p, seed, "temporal_attn_long_dropout_bwd", &d)) return r;
   return long_bwd_call(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale,
                        kv_bcast, &d, stream);
+}
+
+extern "C" int og_temporal_attn_bidir_fwd(const void* q, const void* k, const void* v, void* out, const void* residual,
+                                          void* out_res, float* lse, int B, int T, int64_t P, int C, int n_head,
+                                          float scale, int kv_bcast, float p, const uint64_t* seed, og_stream_t stream) {
+  DropParams d;
+  const DropParams* drop;
+  if (const int r = drop_params_opt(p, seed, "temporal_attn_bidir_fwd", &d, &drop)) return r;
+  return long_fwd_call(q, k, v, out, residual, out_res, lse, B, T, P, C, n_head, scale, kv_bcast, drop, stream, false);
+}
+
+extern "C" int og_temporal_attn_bidir_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout,
+                                          const float* lse, float* delta_ws, void* dq, void* dk, void* dv,
+                                          float* dk_bcast, float* dv_bcast, int B, int T, int64_t P, int C, int n_head,
+                                          float scale, int kv_bcast, float p, const uint64_t* seed,
+                                          og_stream_t stream) {
+  DropParams d;
+  const DropParams* drop;
+  if (const int r = drop_params_opt(p, seed, "temporal_attn_bidir_bwd", &d, &drop)) return r;
+  return long_bwd_call(q, k, v, out, dout, lse, delta_ws, dq, dk, dv, dk_bcast, dv_bcast, B, T, P, C, n_head, scale,
+                       kv_bcast, drop, stream, false);
 }

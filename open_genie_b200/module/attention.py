@@ -16,6 +16,10 @@ Dropout: `dropout` (0 <= p < 1) drops attention probabilities as SDPA's dropout_
 temporal attention. Like the reference, which passes dropout_p to the functional SDPA, it drops in eval mode and under
 no_grad too; set `module.dropout = 0` (read at every call) for deterministic inference. The masks come from Philox
 seeds drawn from the CUDA generator (csrc/attn_dropout.cuh), so torch.manual_seed governs them.
+Causality: `causal` is SDPA's is_causal, as in the reference. SpatialAttention(causal=True) masks the tokens after
+each one in raster order (og_flash_attn_causal_*); TemporalAttention defaults to causal=False, like the reference and
+the `time_attn` blueprint, and then attends over the whole clip (og_temporal_attn_bidir_*, the tiled kernels at every
+T). SpaceTimeAttention keeps the reference's spatial causal=False and temporal causal=True.
 The FFN is the reference's ForwardBlock: GroupNorm -> conv (-> GELU -> conv)* with `hid_dim` hidden widths, ending at
 `d_out` channels (with transpose=True, where the skip becomes the 1x1x1 ffn_skip conv); `bias` gives every FFN conv a
 bias. Hidden widths and d_out are multiples of 64.
@@ -130,15 +134,15 @@ class SpatialAttention(Attention):
             raise NotImplementedError('spatial cond / mask are dead code at the reference HEAD (attention.py:290,296)')
         x, t = self._rows(video, transpose)
         y = ops.space_attention_res(x, self._freq, self.norm.weight, self.norm.bias, self.n_head, self.scale,
-                                    self.norm.eps, self.dropout)
+                                    self.norm.eps, self.dropout, self.causal)
         if not _residual:
             y = y - ops._rows_bf16(x)          # rarely used stand-alone path
         return self._back(y, t)
 
 
 class TemporalAttention(Attention):
-    """Causal self-attention over t for every pixel, 1-D rotary embedding; optional (B, T, key_dim) conditioning
-    that provides K and V (attention.py:309-371)."""
+    """Self-attention over t for every pixel (causal with causal=True, bidirectional by default as in the reference),
+    1-D rotary embedding; optional (B, T, key_dim) conditioning that provides K and V (attention.py:309-371)."""
     rope_kind = '1d'
 
     def forward(self, video: Tensor, cond: Tensor | None = None, mask: Tensor | None = None,
@@ -152,7 +156,7 @@ class TemporalAttention(Attention):
             kc = self.to_qkv.to_k(c)            # (B, T, C): a few kFLOP of host-side plumbing (torch, autograd)
             vc = self.to_qkv.to_v(c)
         y = ops.time_attention_res(x, self._freq, self.norm.weight, self.norm.bias, self.n_head, self.scale,
-                                   kc, vc, self.norm.eps, self.dropout)
+                                   kc, vc, self.norm.eps, self.dropout, self.causal)
         if not _residual:
             y = y - ops._rows_bf16(x)
         return self._back(y, t)

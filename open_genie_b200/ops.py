@@ -977,10 +977,13 @@ class _SpaceAttnFn(torch.autograd.Function):
     """y = SDPA(q, q, q; scale, dropout_p) + x with q = LayerNorm(RoPE2d(x)), sequences = frames (H*W tokens).
     SpatialAttention.forward + the residual of SpaceTimeAttention.forward (attention.py:279-307, 470).
     freq = None (embed=False) gives q = LayerNorm(x), through og_ln_rows_fwd / bwd.
-    dropout > 0 runs og_flash_attn_dropout_fwd / bwd with a seed from _dropout_seed; 0 runs og_flash_attn_fwd / bwd."""
+    dropout > 0 runs og_flash_attn_dropout_fwd / bwd with a seed from _dropout_seed; 0 runs og_flash_attn_fwd / bwd.
+    causal (SpatialAttention(causal=True): SDPA is_causal=True over the H*W tokens in raster order) runs
+    og_flash_attn_causal_fwd / bwd at every dropout, with a seed only when dropout > 0."""
 
     @staticmethod
-    def forward(ctx, x, freq, gamma, beta, n_head: int, scale: float, eps: float, dropout: float):
+    def forward(ctx, x, freq, gamma, beta, n_head: int, scale: float, eps: float, dropout: float,
+                causal: bool = False):
         _require_cuda(x, 'attention input')
         x = _rows_bf16(x)
         B, T, H, W, C = x.shape
@@ -990,9 +993,12 @@ class _SpaceAttnFn(torch.autograd.Function):
         _ln_rows_fwd(x, freq, gamma, beta, eps, q, rows, C, 1, S, s)
         y, o = torch.empty_like(x), torch.empty_like(x)
         lse = torch.empty((B * T, n_head, S), dtype=f32, device=x.device)
-        seed = None
-        if dropout > 0:
-            seed = _dropout_seed(x.device)
+        seed = _dropout_seed(x.device) if dropout > 0 else None
+        if causal:   # the S (S + 1) / 2 scores with key <= query
+            _conv_call('attn_fwd', 2.0 * B * T * S * (S + 1) * C, 'og_flash_attn_causal_fwd', q.data_ptr(), q.data_ptr(),
+                       q.data_ptr(), o.data_ptr(), x.data_ptr(), y.data_ptr(), lse.data_ptr(), B * T, S, C, n_head,
+                       scale, dropout, _ptr(seed), s)
+        elif dropout > 0:
             _conv_call('attn_fwd', 4.0 * B * T * S * S * C, 'og_flash_attn_dropout_fwd', q.data_ptr(), q.data_ptr(),
                        q.data_ptr(), o.data_ptr(), x.data_ptr(), y.data_ptr(), lse.data_ptr(), B * T, S, C, n_head,
                        scale, dropout, seed.data_ptr(), s)
@@ -1000,21 +1006,25 @@ class _SpaceAttnFn(torch.autograd.Function):
             _conv_call('attn_fwd', 4.0 * B * T * S * S * C, 'og_flash_attn_fwd', q.data_ptr(), q.data_ptr(),
                        q.data_ptr(), o.data_ptr(), x.data_ptr(), y.data_ptr(), lse.data_ptr(), B * T, S, C, n_head,
                        scale, s)
-        ctx.cfg = (n_head, scale, eps, dropout)
+        ctx.cfg = (n_head, scale, eps, dropout, causal)
         ctx.save_for_backward(x, q, o, lse, freq, gamma, seed)
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x, q, o, lse, freq, gamma, seed = ctx.saved_tensors
-        n_head, scale, eps, dropout = ctx.cfg
+        n_head, scale, eps, dropout, causal = ctx.cfg
         B, T, H, W, C = x.shape
         rows, S = B * T * H * W, H * W
         s = _stream()
         dy = _rows_bf16(dy)
         dq, dk, dv = torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)
         delta = torch.empty_like(lse)
-        if dropout > 0:
+        if causal:
+            _conv_call('attn_bwd', 5.0 * B * T * S * (S + 1) * C, 'og_flash_attn_causal_bwd', q.data_ptr(), q.data_ptr(),
+                       q.data_ptr(), o.data_ptr(), dy.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(),
+                       dk.data_ptr(), dv.data_ptr(), B * T, S, C, n_head, scale, dropout, _ptr(seed), s)
+        elif dropout > 0:
             _conv_call('attn_bwd', 10.0 * B * T * S * S * C, 'og_flash_attn_dropout_bwd', q.data_ptr(), q.data_ptr(),
                        q.data_ptr(), o.data_ptr(), dy.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(),
                        dk.data_ptr(), dv.data_ptr(), B * T, S, C, n_head, scale, dropout, seed.data_ptr(), s)
@@ -1026,7 +1036,7 @@ class _SpaceAttnFn(torch.autograd.Function):
         dgamma = _zeros(C, f32, x.device)
         dbeta = _zeros(C, f32, x.device)
         _ln_rows_bwd(x, freq, gamma, eps, dq, dk, dv, dy, dx, dgamma, dbeta, rows, C, 1, S, s)
-        return dx, None, dgamma, dbeta, None, None, None, None
+        return dx, None, dgamma, dbeta, None, None, None, None, None
 
 
 # Longest clip of the per-pixel temporal kernels (og_temporal_attn_fwd / bwd); longer ones take the tiled kernels.
@@ -1047,10 +1057,13 @@ class _TimeAttnFn(torch.autograd.Function):
     """y = SDPA_causal(q, k, v; scale, dropout_p) + x over t for every pixel; q = LayerNorm(RoPE1d(x)); k = v = q, or
     the projected latent-action conditioning (B, T, C) shared by all pixels (attention.py:347-371, 471).
     freq = None (embed=False) gives q = LayerNorm(x), through og_ln_rows_fwd / bwd.
-    dropout > 0 runs og_temporal_attn_long_dropout_fwd / bwd with a seed from _dropout_seed."""
+    dropout > 0 runs og_temporal_attn_long_dropout_fwd / bwd with a seed from _dropout_seed.
+    causal=False (TemporalAttention's default, SDPA is_causal=False) runs og_temporal_attn_bidir_fwd / bwd at every T,
+    with a seed only when dropout > 0; the per-pixel kernels and _time_attn_tiled are causal only."""
 
     @staticmethod
-    def forward(ctx, x, freq, gamma, beta, k_cond, v_cond, n_head: int, scale: float, eps: float, dropout: float):
+    def forward(ctx, x, freq, gamma, beta, k_cond, v_cond, n_head: int, scale: float, eps: float, dropout: float,
+                causal: bool = True):
         _require_cuda(x, 'attention input')
         x = _rows_bf16(x)
         B, T, H, W, C = x.shape
@@ -1066,32 +1079,40 @@ class _TimeAttnFn(torch.autograd.Function):
         else:
             kc = vc = q
         o = lse = seed = None
-        if not _time_attn_tiled(T, C, n_head, dropout):
+        if causal and not _time_attn_tiled(T, C, n_head, dropout):
             _lib.call('og_temporal_attn_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), x.data_ptr(), y.data_ptr(),
                       B, T, P, C, n_head, scale, int(bcast), s)
         else:
             # the tiled kernels, which keep the attention output and log-sum-exp for the backward pass
             o = torch.empty_like(x)
             lse = torch.empty((B, n_head, P, T), dtype=f32, device=x.device)
-            if dropout > 0:
-                seed = _dropout_seed(x.device)
+            seed = _dropout_seed(x.device) if dropout > 0 else None
+            if not causal:
+                _lib.call('og_temporal_attn_bidir_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), o.data_ptr(),
+                          x.data_ptr(), y.data_ptr(), lse.data_ptr(), B, T, P, C, n_head, scale, int(bcast), dropout,
+                          _ptr(seed), s)
+            elif dropout > 0:
                 _lib.call('og_temporal_attn_long_dropout_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), o.data_ptr(),
                           x.data_ptr(), y.data_ptr(), lse.data_ptr(), B, T, P, C, n_head, scale, int(bcast), dropout,
                           seed.data_ptr(), s)
             else:
                 _lib.call('og_temporal_attn_long_fwd', q.data_ptr(), kc.data_ptr(), vc.data_ptr(), o.data_ptr(),
                           x.data_ptr(), y.data_ptr(), lse.data_ptr(), B, T, P, C, n_head, scale, int(bcast), s)
-        ctx.cfg = (n_head, scale, eps, bcast, dropout)
+        ctx.cfg = (n_head, scale, eps, bcast, dropout, causal)
         ctx.save_for_backward(x, q, kc if bcast else None, vc if bcast else None, freq, gamma, o, lse, seed)
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x, q, kc, vc, freq, gamma, o, lse, seed = ctx.saved_tensors
-        n_head, scale, eps, bcast, dropout = ctx.cfg
+        n_head, scale, eps, bcast, dropout, causal = ctx.cfg
         # the tiled backward, with the forward's dropout seed when it dropped
-        long_bwd = 'og_temporal_attn_long_dropout_bwd' if dropout > 0 else 'og_temporal_attn_long_bwd'
-        drop_args = (dropout, seed.data_ptr()) if dropout > 0 else ()
+        if not causal:
+            long_bwd, drop_args = 'og_temporal_attn_bidir_bwd', (dropout, _ptr(seed))
+        elif dropout > 0:
+            long_bwd, drop_args = 'og_temporal_attn_long_dropout_bwd', (dropout, seed.data_ptr())
+        else:
+            long_bwd, drop_args = 'og_temporal_attn_long_bwd', ()
         B, T, H, W, C = x.shape
         P = H * W
         s = _stream()
@@ -1124,7 +1145,7 @@ class _TimeAttnFn(torch.autograd.Function):
         dgamma = _zeros(C, f32, x.device)
         dbeta = _zeros(C, f32, x.device)
         _ln_rows_bwd(x, freq, gamma, eps, dq, g1, g2, dy, dx, dgamma, dbeta, B * T * P, C, P, T, s)
-        return dx, None, dgamma, dbeta, dkc, dvc, None, None, None, None
+        return dx, None, dgamma, dbeta, dkc, dvc, None, None, None, None, None
 
 
 class _FfnFn(torch.autograd.Function):
@@ -1252,12 +1273,14 @@ class _FfnFn(torch.autograd.Function):
         return (dx, dgw, dgb, None, None, None, dskip_w, dskip_b, *grads)
 
 
-def space_attention_res(x, freq, gamma, beta, n_head, scale, eps=1e-5, dropout=0.0):
-    return _SpaceAttnFn.apply(x, freq, gamma, beta, n_head, float(scale), float(eps), float(dropout))
+def space_attention_res(x, freq, gamma, beta, n_head, scale, eps=1e-5, dropout=0.0, causal=False):
+    return _SpaceAttnFn.apply(x, freq, gamma, beta, n_head, float(scale), float(eps), float(dropout), bool(causal))
 
 
-def time_attention_res(x, freq, gamma, beta, n_head, scale, k_cond=None, v_cond=None, eps=1e-5, dropout=0.0):
-    return _TimeAttnFn.apply(x, freq, gamma, beta, k_cond, v_cond, n_head, float(scale), float(eps), float(dropout))
+def time_attention_res(x, freq, gamma, beta, n_head, scale, k_cond=None, v_cond=None, eps=1e-5, dropout=0.0,
+                       causal=True):
+    return _TimeAttnFn.apply(x, freq, gamma, beta, k_cond, v_cond, n_head, float(scale), float(eps), float(dropout),
+                             bool(causal))
 
 
 def ffn_res(x, gn_w, gn_b, convs, num_groups, eps=1e-5, skip_w=None, skip_b=None):
